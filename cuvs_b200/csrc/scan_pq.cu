@@ -138,10 +138,16 @@ __device__ __forceinline__ uint64_t pq_filter_frag(const float (&d)[NQ / 2], uin
 {
   uint64_t left = 0;
   const int cq  = 2 * (lane & 3);
+  // All of the fragment's thresholds are loaded before any is tested.  Loaded one column pair at a time, each load waits
+  // behind the previous pair's candidate atomics (the compiler does not move it above them), and its latency is paid once
+  // per pair.  No thread changes a threshold while a tile is filtered: compaction runs between the per-tile barriers.
+  float2 ths[NQ / 8];
+#pragma unroll
+  for (int j = 0; j < NQ / 8; ++j) ths[j] = *reinterpret_cast<const float2*>(thr + 8 * j + cq);
 #pragma unroll
   for (int j = 0; j < NQ / 8; ++j) {
     const int c     = 8 * j + cq;
-    const float2 th = *reinterpret_cast<const float2*>(thr + c);
+    const float2 th = ths[j];
     // margin over the column's threshold: a candidate iff > 0 (exact: the difference of two floats keeps its sign)
     const float m = fmaxf(fmaxf(d[4 * j] - th.x, d[4 * j + 1] - th.y), fmaxf(d[4 * j + 2] - th.x, d[4 * j + 3] - th.y));
     if (m > 0.f) {
