@@ -33,6 +33,21 @@ __global__ void row_norms_kernel(const float* __restrict__ x, int64_t n, int d, 
   out[i] = acc;
 }
 
+__global__ void rsqrt_rows_kernel(const float* xn, float* out, int64_t n)
+{
+  int64_t i = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x;
+  if (i < n) out[i] = xn[i] > 0.f ? 1.0f / sqrtf(xn[i]) : 0.f;
+}
+
+__global__ void scale_rows_kernel(float* __restrict__ x, int64_t n, int d, int64_t ld, const float* __restrict__ scale)
+{
+  int64_t t = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x;
+  if (t >= n * d) return;
+  const int64_t r = t / d;
+  const int c     = static_cast<int>(t % d);
+  x[r * ld + c] *= scale[r];
+}
+
 __device__ __forceinline__ bool keep_sample(const filter_view& f, int64_t q, int64_t j)
 {
   if (f.kind == 0) return true;
@@ -274,6 +289,25 @@ void row_norms(cudaStream_t stream, const float* x, int64_t n, int d, int64_t ld
   if (n == 0) return;
   count_launch();
   row_norms_kernel<<<static_cast<unsigned>((n + 127) / 128), 128, 0, stream>>>(x, n, d, ld, out);
+  B2_CUDA(cudaGetLastError());
+}
+
+void rsqrt_rows(cudaStream_t stream, const float* xn, int64_t n, float* out)
+{
+  if (n == 0) return;
+  count_launch();
+  rsqrt_rows_kernel<<<static_cast<unsigned>((n + 255) / 256), 256, 0, stream>>>(xn, out, n);
+  B2_CUDA(cudaGetLastError());
+}
+
+void normalize_rows(cudaStream_t stream, float* x, int64_t n, int d, int64_t ld)
+{
+  if (n == 0) return;
+  dbuf<float> inv(static_cast<size_t>(n), stream);
+  row_norms(stream, x, n, d, ld, inv.data());
+  rsqrt_rows(stream, inv.data(), n, inv.data());
+  count_launch();
+  scale_rows_kernel<<<static_cast<unsigned>((n * d + 255) / 256), 256, 0, stream>>>(x, n, d, ld, inv.data());
   B2_CUDA(cudaGetLastError());
 }
 

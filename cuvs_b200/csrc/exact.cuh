@@ -15,6 +15,13 @@ namespace b200 {
 /** out[i] = sum_k x[i,k]^2 (ascending k, fmaf). */
 void row_norms(cudaStream_t stream, const float* x, int64_t n, int d, int64_t ld, float* out);
 
+/** out[i] = 1 / sqrt(xn[i]) from squared norms, and 0 where xn[i] is 0: the per-row scale of the cosine metric.  A zero row
+ *  scales to the zero vector, so its cosine distance to anything is 1.  out may alias xn. */
+void rsqrt_rows(cudaStream_t stream, const float* xn, int64_t n, float* out);
+
+/** x[i, :d] *= 1 / |x_i| in place (row_norms + rsqrt_rows, then one fp32 multiply per element); zero rows stay zero. */
+void normalize_rows(cudaStream_t stream, float* x, int64_t n, int d, int64_t ld);
+
 struct filter_view {
   const uint32_t* bits = nullptr;  // 1 = keep
   int kind             = 0;        // 0 none, 1 bitset (per sample), 2 bitmap (per query x sample)

@@ -99,12 +99,6 @@ __global__ void half_norms_filtered_kernel(const float* __restrict__ xn, const i
   hn[i]            = keep ? (zero ? 0.f : 0.5f * xn[i]) : INFINITY;
 }
 
-__global__ void rsqrt_rows_kernel(const float* __restrict__ xn, float* __restrict__ out, int64_t n)
-{
-  int64_t i = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x;
-  if (i < n) out[i] = xn[i] > 0.f ? 1.0f / sqrtf(xn[i]) : 0.f;
-}
-
 // positions of old rows in the new layout (same order inside each list)
 __global__ void remap_old_rows_kernel(const int64_t* __restrict__ old_off, const int64_t* __restrict__ new_off,
                                       const uint32_t* __restrict__ old_sizes, int64_t n_lists, int64_t* __restrict__ dst_rows,
@@ -142,8 +136,7 @@ void refresh_tc_side(resources* res, ivf_flat_index& idx)
   dbuf<float> scale;
   if (idx.metric == CosineExpanded) {
     scale.alloc(static_cast<size_t>(R), s);
-    count_launch();
-    rsqrt_rows_kernel<<<blocks_for(R, 256), 256, 0, s>>>(idx.xn.data(), scale.data(), R);
+    rsqrt_rows(s, idx.xn.data(), R, scale.data());
   }
   tc_split_planes(s, idx.data.data(), R, idx.dim, idx.dim, idx.Kp, idx.hi.data(), nullptr, R, scale.data());
   count_launch();
@@ -161,8 +154,7 @@ void refresh_centers_tc(resources* res, ivf_flat_index& idx)
   dbuf<float> scale;
   if (idx.metric == CosineExpanded) {
     scale.alloc(static_cast<size_t>(idx.n_lists), s);
-    count_launch();
-    rsqrt_rows_kernel<<<blocks_for(idx.n_lists, 256), 256, 0, s>>>(cn.data(), scale.data(), idx.n_lists);
+    rsqrt_rows(s, cn.data(), idx.n_lists, scale.data());
   }
   idx.centers_tc.build(s, idx.centers.data(), idx.n_lists, idx.dim, is_l2(idx.metric) ? cn.data() : nullptr, true, scale.data());
 }
@@ -179,8 +171,7 @@ void ivf_flat_extend(resources* res, ivf_flat_index& idx, const float* x, int64_
     dbuf<float> xn(static_cast<size_t>(n), s);
     row_norms(s, x, n, idx.dim, idx.dim, xn.data());
     scale.alloc(static_cast<size_t>(n), s);
-    count_launch();
-    rsqrt_rows_kernel<<<blocks_for(n, 256), 256, 0, s>>>(xn.data(), scale.data(), n);
+    rsqrt_rows(s, xn.data(), n, scale.data());
   }
   xp.build(s, x, n, idx.dim, true, 0, scale.data());
   dbuf<uint32_t> labels(static_cast<size_t>(n), s);
@@ -321,8 +312,7 @@ void ivf_flat_search(resources* res, const ivf_flat_index& idx, uint32_t n_probe
   dbuf<float> qscale;
   if (idx.metric == CosineExpanded) {
     qscale.alloc(static_cast<size_t>(nq), s);
-    count_launch();
-    rsqrt_rows_kernel<<<blocks_for(nq, 256), 256, 0, s>>>(qn.data(), qscale.data(), nq);
+    rsqrt_rows(s, qn.data(), nq, qscale.data());
   }
   tc_rows_tmp qp;
   qp.build(s, q, nq, idx.dim, true, 0, qscale.data());

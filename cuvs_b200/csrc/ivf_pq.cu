@@ -23,6 +23,9 @@
 //       the per-(query,probe) LUT build and the 4e11 shared-memory gathers altogether.
 // (B) is used when lut_dtype == internal_distance_dtype == fp32 and the index holds decoded rows
 // (conservative_memory_allocation == false); (A) otherwise or with CUVS_B200_PQ_PATH=lut.
+//
+// Cosine is inner product over unit vectors plus 1 (DESIGN.md §5): unit training rows and centres at build, x / |x| in the
+// encode path (encode_rows), unit rotated queries at search, and the +1 in the LUT kernel or in the per-pair offset `add`.
 #include "common.hpp"
 #include "exact.cuh"
 #include "ivf_common.cuh"
@@ -140,14 +143,16 @@ template <> struct lut_conv<uint8_t> {
 };
 
 // ------------------------------------------------------------------ build-side kernels
-__global__ void residual_kernel(const float* __restrict__ x_rot, const uint32_t* __restrict__ labels,
+// out = x_rot * inv_norm[row] - c_rot[label]; inv_norm is null (no scaling) except for cosine
+__global__ void residual_kernel(const float* __restrict__ x_rot, const uint32_t* __restrict__ labels, const float* __restrict__ inv_norm,
                                 const float* __restrict__ centers_rot, int64_t n, int rot_dim, float* __restrict__ out)
 {
   int64_t t = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x;
   if (t >= n * rot_dim) return;
   int64_t r = t / rot_dim;
   int c     = static_cast<int>(t % rot_dim);
-  out[t]    = x_rot[t] - centers_rot[static_cast<int64_t>(labels[r]) * rot_dim + c];
+  const float x = inv_norm ? __fmul_rn(x_rot[t], inv_norm[r]) : x_rot[t];
+  out[t]    = x - centers_rot[static_cast<int64_t>(labels[r]) * rot_dim + c];
 }
 
 // nearest code per (point, subspace).  grid (ceil(n/128), n_books); codebook of this book in smem.
@@ -317,12 +322,14 @@ __global__ void make_centers_ext_kernel(const float* __restrict__ centers, int64
 }
 
 // ------------------------------------------------------------------ search-side kernels
-// per pair: r = q_rot[query] - c_rot[list] (L2) or q_rot[query] (IP) as bf16 A rows; add[slot] = |r|^2 (L2) or 0 (IP)
+// per pair: r = q_rot[query] - c_rot[list] (L2) or q_rot[query] (IP) as bf16 A rows; add[slot] = |r|^2 (L2) or 0 (IP).
+// Cosine (q_rot already unit) adds the reference's +1 to the offset, so that every reader of `add` sees final distances:
+// 1 - q.c on code-only rows, 1 on decoded rows (c is inside y there).
 __global__ void pair_rows_kernel(const float* __restrict__ q_rot, const float* __restrict__ centers_rot,
                                  const uint32_t* __restrict__ pair_query, const uint32_t* __restrict__ pair_list,
                                  const int* __restrict__ n_live, int64_t rows_total, int rot_dim, int Kp, bool ip,
                                  __nv_bfloat16* __restrict__ a_hi,
-                                 __nv_bfloat16* __restrict__ a_lo, float* __restrict__ add, bool ip_center_in_add)
+                                 __nv_bfloat16* __restrict__ a_lo, float* __restrict__ add, bool ip_center_in_add, bool cosine)
 {
   int64_t r = (blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x) >> 5;
   int lane  = threadIdx.x & 31;
@@ -342,7 +349,11 @@ __global__ void pair_rows_kernel(const float* __restrict__ q_rot, const float* _
   }
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) nrm += __shfl_xor_sync(0xffffffffu, nrm, o);
-  if (lane == 0 && live) add[r] = (ip && !ip_center_in_add) ? 0.f : nrm;
+  if (lane == 0 && live) {
+    float a = (ip && !ip_center_in_add) ? 0.f : nrm;
+    if (cosine) a += 1.0f;
+    add[r] = a;
+  }
 }
 
 // out[q, p*KCW + c] = add[slot] + scale * s   (per-query concatenation of its probes' candidates)
@@ -557,6 +568,46 @@ void rotate_rows(cudaStream_t s, const float* x, int64_t n, int dim, const float
   }
 }
 
+// The one encode path of the index (codebook training in ivf_pq_build, ivf_pq_extend, cuvsIvfPqTransform), so that stored
+// codes and transform() output cannot diverge: nearest coarse centre of each row (unless `assign` is false and `labels`
+// already holds it), rotation, residual R x - c_rot[label] into `resid` [n, rot_dim], and, when `codes` is given, the
+// nearest codebook entry per subspace (row i written to row dst_rows[i], or i).  Cosine encodes x / |x|
+// (ivf_pq_build.cuh:159-174): R has orthonormal columns, so |R x| = |x| and the per-row 1 / |x| is applied inside the
+// residual step, without a normalised copy of the rows.
+void encode_rows(resources* res, const ivf_pq_index& idx, const float* x, int64_t n, uint32_t* labels, bool assign, float* resid,
+                 uint8_t* codes, const int64_t* dst_rows)
+{
+  auto s = res->stream;
+  if (n == 0) return;
+  if (assign) {
+    tc_rows_tmp xp;
+    xp.build(s, x, n, idx.dim, true);
+    assign_nearest(res, xp.hi.data(), xp.lo.data(), n, xp.rows_pad, xp.Kp, idx.centers_tc, labels, nullptr);
+  }
+  dbuf<float> inv;
+  if (idx.metric == CosineExpanded) {
+    inv.alloc(static_cast<size_t>(n), s);
+    row_norms(s, x, n, idx.dim, idx.dim, inv.data());
+    rsqrt_rows(s, inv.data(), n, inv.data());
+  }
+  {
+    dbuf<float> xr(static_cast<size_t>(n) * idx.rot_dim, s);
+    rotate_rows(s, x, n, idx.dim, idx.rotation.data(), idx.rot_dim, xr.data());
+    count_launch();
+    residual_kernel<<<blocks_for(n * idx.rot_dim, 256), 256, 0, s>>>(xr.data(), labels, inv.data(), idx.centers_rot.data(), n,
+                                                                     idx.rot_dim, resid);
+    B2_CUDA(cudaGetLastError());
+  }
+  if (codes) {
+    const size_t smem = static_cast<size_t>(idx.pq_len) * idx.book() * sizeof(float);
+    count_launch();
+    pq_assign_kernel<<<dim3(blocks_for(n, 128), idx.pq_dim), 128, smem, s>>>(
+      resid, n, idx.rot_dim, idx.pq_dim, idx.pq_len, idx.book(), idx.pq_centers.data(),
+      idx.codebook_kind == CUVS_IVF_PQ_CODEBOOK_GEN_PER_CLUSTER, labels, codes, dst_rows);
+    B2_CUDA(cudaGetLastError());
+  }
+}
+
 void refresh_centers(resources* res, ivf_pq_index& idx)
 {
   auto s = res->stream;
@@ -721,16 +772,9 @@ void ivf_pq_extend(resources* res, ivf_pq_index& idx, const DLTensor& t, const i
     place_rows(s, labels.data() + r0, rows, nl, fill, dst_new.data());
     for (uint32_t l = 0; l < idx.n_lists; ++l) fill[l] += chunk_add[ci][l];
     ++ci;
-    // encode: rotate, residual, nearest code per subspace
-    dbuf<float> xr(static_cast<size_t>(rows) * idx.rot_dim, s), rs(static_cast<size_t>(rows) * idx.rot_dim, s);
-    rotate_rows(s, x, rows, idx.dim, idx.rotation.data(), idx.rot_dim, xr.data());
-    count_launch(3);
-    residual_kernel<<<blocks_for(rows * idx.rot_dim, 256), 256, 0, s>>>(xr.data(), labels.data() + r0, idx.centers_rot.data(), rows,
-                                                                         idx.rot_dim, rs.data());
-    const size_t smem = static_cast<size_t>(idx.pq_len) * idx.book() * sizeof(float);
-    pq_assign_kernel<<<dim3(blocks_for(rows, 128), idx.pq_dim), 128, smem, s>>>(
-      rs.data(), rows, idx.rot_dim, idx.pq_dim, idx.pq_len, idx.book(), idx.pq_centers.data(),
-      idx.codebook_kind == CUVS_IVF_PQ_CODEBOOK_GEN_PER_CLUSTER, labels.data() + r0, ncodes.data(), dst_new.data());
+    dbuf<float> rs(static_cast<size_t>(rows) * idx.rot_dim, s);
+    encode_rows(res, idx, x, rows, labels.data() + r0, false, rs.data(), ncodes.data(), dst_new.data());
+    count_launch();
     set_ids_kernel<<<blocks_for(rows, 256), 256, 0, s>>>(dst_new.data(), new_ids ? new_ids + r0 : nullptr, id0 + r0, rows, nids.data());
     B2_CUDA(cudaGetLastError());
   });
@@ -758,7 +802,6 @@ void init_shape(ivf_pq_index& idx, const cuvsIvfPqIndexParams& p, int dim)
   B2_EXPECTS(idx.pq_bits >= 4 && idx.pq_bits <= 8, "pq_bits must be within [4, 8]");
   B2_EXPECTS(idx.pq_len >= 1 && idx.pq_len <= 32, "pq_len = ceil(dim / pq_dim) = %d is outside [1, 32] (dim %d, pq_dim %d)", idx.pq_len, dim, idx.pq_dim);
   B2_EXPECTS(is_l2(p.metric) || p.metric == InnerProduct || p.metric == CosineExpanded, "ivf_pq: unsupported metric %d", int(p.metric));
-  B2_EXPECTS(p.metric != CosineExpanded, "ivf_pq: cosine metric is not supported by this build yet");
 }
 
 ivf_pq_index* ivf_pq_build(resources* res, const cuvsIvfPqIndexParams& p, const DLTensor& ds)
@@ -785,7 +828,12 @@ ivf_pq_index* ivf_pq_build(resources* res, const cuvsIvfPqIndexParams& p, const 
   B2_CUDA(cudaMemcpy2DAsync(train.data(), sizeof(float) * d, dl_ptr<float>(ds), sizeof(float) * d * stride, sizeof(float) * d, n_train,
                             cudaMemcpyDefault, s));
   idx->centers.alloc(static_cast<size_t>(p.n_lists) * d);
+  // cosine (ivf_pq_build.cuh:1336-1348): fit on the unit training rows, then make the centres unit rows; the rows are
+  // labelled against the unit centres below.  `train` is a private copy, so it is normalised in place.
+  const bool cosine = idx->metric == CosineExpanded;
+  if (cosine) normalize_rows(s, train.data(), n_train, d, d);
   kmeans_train(res, train.data(), n_train, d, p.n_lists, std::max<uint32_t>(p.kmeans_n_iters, 1), idx->centers.data(), true, true, nullptr, nullptr);
+  if (cosine) normalize_rows(s, idx->centers.data(), p.n_lists, d, d);
   refresh_centers(res, *idx);
 
   // rotation and rotated centres
@@ -801,14 +849,9 @@ ivf_pq_index* ivf_pq_build(resources* res, const cuvsIvfPqIndexParams& p, const 
   if (idx->codebook_kind == CUVS_IVF_PQ_CODEBOOK_GEN_PER_CLUSTER) n_pq = n_train;
   n_pq = std::max<int64_t>(n_pq, std::min<int64_t>(n_train, idx->book()));
   {
-    tc_rows_tmp tp;
-    tp.build(s, train.data(), n_pq, d, true);
     dbuf<uint32_t> labels(static_cast<size_t>(n_pq), s);
-    assign_nearest(res, tp.hi.data(), tp.lo.data(), n_pq, tp.rows_pad, tp.Kp, idx->centers_tc, labels.data(), nullptr);
-    dbuf<float> xr(static_cast<size_t>(n_pq) * idx->rot_dim, s), rs(static_cast<size_t>(n_pq) * idx->rot_dim, s);
-    rotate_rows(s, train.data(), n_pq, d, idx->rotation.data(), idx->rot_dim, xr.data());
-    count_launch();
-    residual_kernel<<<blocks_for(n_pq * idx->rot_dim, 256), 256, 0, s>>>(xr.data(), labels.data(), idx->centers_rot.data(), n_pq, idx->rot_dim, rs.data());
+    dbuf<float> rs(static_cast<size_t>(n_pq) * idx->rot_dim, s);
+    encode_rows(res, *idx, train.data(), n_pq, labels.data(), true, rs.data(), nullptr, nullptr);
     train_codebooks(res, *idx, rs.data(), labels.data(), n_pq, std::max<uint32_t>(p.kmeans_n_iters, 1));
   }
   std::vector<int64_t> zero(p.n_lists, 0);
@@ -872,6 +915,10 @@ void ivf_pq_search(resources* res, const ivf_pq_index& idx, const cuvsIvfPqSearc
   coarse_select(res, qp, idx.centers_tc, static_cast<int>(n_probes), probes.data(), nullptr);
   dbuf<float> q_rot(static_cast<size_t>(nq) * idx.rot_dim, s);
   rotate_rows(s, q, nq, idx.dim, idx.rotation.data(), idx.rot_dim, q_rot.data());
+  // cosine: the fine scan scores unit queries (ivf_pq_search.cuh:1020-1025).  The coarse ranking -q.c over unit centres does
+  // not depend on |q|, so the probes above come from the raw queries, as in the reference.
+  const bool cosine = idx.metric == CosineExpanded;
+  if (cosine) normalize_rows(s, q_rot.data(), nq, idx.rot_dim, idx.rot_dim);
 
   // ---- bucket pairs by list
   // Decoded-row tensor-core scan whenever the index keeps decoded rows.  fp32 LUT + fp32 accumulation (the reference's
@@ -914,9 +961,9 @@ void ivf_pq_search(resources* res, const ivf_pq_index& idx, const cuvsIvfPqSearc
     count_launch();
     pair_rows_kernel<<<blocks_for(a_rows * 32, 256), 256, 0, s>>>(q_rot.data(), idx.centers_rot.data(), pb.pair_query.data(),
                                                                    pb.pair_list.data(), pb.n_items.data() + 1, a_rows, idx.rot_dim, idx.Kp, ip,
-                                                                   a_hi.data(), a_lo.data(), add.data(), use_stream);
+                                                                   a_hi.data(), a_lo.data(), add.data(), use_stream, cosine);
     B2_CUDA(cudaGetLastError());
-    scale = ip ? 1.0f : 2.0f;  // L2: |r|^2 + 2 (|y|^2/2 - r.y); IP: -(q.(c+y))
+    scale = ip ? 1.0f : 2.0f;  // L2: |r|^2 + 2 (|y|^2/2 - r.y); IP: -(q.(c+y)); cosine: 1 - q.(c+y)
     {
       // probes of one query share a running bound on its k'-th best DISTANCE: d = add[slot] + scale * s
       if (k <= KC) {  // the bound tracks a k-th best out of KC kept entries
@@ -947,7 +994,6 @@ void ivf_pq_search(resources* res, const ivf_pq_index& idx, const cuvsIvfPqSearc
     B2_EXPECTS(smem <= 227 * 1024, "ivf_pq: LUT (%zu bytes) does not fit in shared memory; use a smaller lut_dtype", smem);
     const bool half_out = sp.internal_distance_dtype == CUDA_R_16F;
     const bool per_cl   = idx.codebook_kind == CUVS_IVF_PQ_CODEBOOK_GEN_PER_CLUSTER;
-    const bool cosine   = idx.metric == CosineExpanded;
     // slots of dropped pairs hold garbage pair_query: only launch over the live prefix
     // (bucket_probes packs live pairs first; count is on the device -> launch over all slots, dead ones exit early)
 #define B2_LUT_LAUNCH(LUT_T, OUT_T)                                                                                         \
@@ -1211,6 +1257,9 @@ cuvsError_t cuvsIvfPqBuildPrecomputed(cuvsResources_t res, cuvsIvfPqIndexParams_
     B2_EXPECTS(ce.ndim == 2 && ce.shape[0] == idx->n_lists && (ce.shape[1] == idx->dim || ce.shape[1] == idx->dim_ext),
                "centers must have extent [n_lists, dim] or [n_lists, dim_ext]");
     copy_in(r, idx->pq_centers, pc, static_cast<size_t>(nb) * idx->pq_len * idx->book());
+    // Caller-supplied centres are used as given for every metric, cosine included: the reference's precomputed build
+    // (ivf_pq_build.cuh:1401-1470) wraps them in a view and normalises nothing.  A cosine index wants unit centres, as
+    // cuvsIvfPqIndexGetCenters returns them from a cosine build.
     idx->centers.alloc(static_cast<size_t>(idx->n_lists) * idx->dim);
     B2_CUDA(cudaMemcpy2DAsync(idx->centers.data(), sizeof(float) * idx->dim, dl_ptr<float>(ce), sizeof(float) * ce.shape[1],
                               sizeof(float) * idx->dim, idx->n_lists, cudaMemcpyDefault, r->stream));
@@ -1518,18 +1567,10 @@ cuvsError_t cuvsIvfPqTransform(cuvsResources_t res, cuvsIvfPqIndex_t index, DLMa
     B2_EXPECTS(dl_is(oc, kDLUInt, 8) && oc.ndim == 2 && oc.shape[0] == n && oc.shape[1] == out_ld && dl_is_device(oc), "output_dataset must be device uint8 [n, %d]", out_ld);
     if (n == 0) return;
     auto s = r->stream;
-    tc_rows_tmp xp;
-    xp.build(s, dl_ptr<float>(x), n, idx.dim, true);
     uint32_t* labels = dl_ptr<uint32_t>(ol);
-    assign_nearest(r, xp.hi.data(), xp.lo.data(), n, xp.rows_pad, xp.Kp, idx.centers_tc, labels, nullptr);
-    dbuf<float> xr(static_cast<size_t>(n) * idx.rot_dim, s), rs(static_cast<size_t>(n) * idx.rot_dim, s);
-    rotate_rows(s, dl_ptr<float>(x), n, idx.dim, idx.rotation.data(), idx.rot_dim, xr.data());
-    residual_kernel<<<blocks_for(n * idx.rot_dim, 256), 256, 0, s>>>(xr.data(), labels, idx.centers_rot.data(), n, idx.rot_dim, rs.data());
+    dbuf<float> rs(static_cast<size_t>(n) * idx.rot_dim, s);
     dbuf<uint8_t> codes(static_cast<size_t>(n) * idx.pq_dim, s);
-    const size_t smem = static_cast<size_t>(idx.pq_len) * idx.book() * sizeof(float);
-    pq_assign_kernel<<<dim3(blocks_for(n, 128), idx.pq_dim), 128, smem, s>>>(rs.data(), n, idx.rot_dim, idx.pq_dim, idx.pq_len, idx.book(),
-                                                                               idx.pq_centers.data(), idx.codebook_kind == CUVS_IVF_PQ_CODEBOOK_GEN_PER_CLUSTER,
-                                                                               labels, codes.data(), nullptr);
+    encode_rows(r, idx, dl_ptr<float>(x), n, labels, true, rs.data(), codes.data(), nullptr);
     pack_codes_kernel<<<blocks_for(n, 128), 128, 0, s>>>(codes.data(), n, idx.pq_dim, idx.pq_bits, out_ld, dl_ptr<uint8_t>(oc));
     B2_CUDA(cudaGetLastError());
   });
