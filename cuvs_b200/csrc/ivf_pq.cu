@@ -941,8 +941,8 @@ void ivf_pq_search(resources* res, const ivf_pq_index& idx, const cuvsIvfPqSearc
   const int KC    = k <= 16 ? 16 : (k <= 32 || (use_tc && !use_stream) ? 32 : 64);
   const int KCW   = KC * lists;
   B2_EXPECTS(KCW >= k, "ivf_pq search: k = %d > 64 needs an index with decoded rows (CUVS_B200_PQ_KEEP_DECODED=1) or the LUT path (CUVS_B200_PQ_PATH=lut)", k);
-  // queries per work item: 128 for the query-major kernels; the streamed kernel takes the list rows as the MMA's M side
-  // and 32 / 64 / 128 probing queries as N (picked from the average number of pairs per list)
+  // queries per work item: 128 for the query-major kernels; the streamed kernel takes 32 / 64 / 128 probing queries (picked
+  // from the average number of pairs per list), as the MMA's M side at 64 / 128 and as its N side at 32
   const int group = use_stream ? pq_stream_group(static_cast<double>(nq) * n_probes / std::max<uint32_t>(idx.n_lists, 1), KC, passes) : 128;
   probe_buckets pb;
   bucket_probes(res, probes.data(), nq, static_cast<int>(n_probes), idx.n_lists, idx.lists.d_offsets.data(), KCW, pb, 0, 0xffffffffu, group);

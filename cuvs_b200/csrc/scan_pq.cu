@@ -14,15 +14,19 @@
 //                          shared load; codebook words sit at [half][code][lane] (bank == lane), so a row's 64 entries are
 //                          fetched with two conflict-free LDS.32 per lane and written with two STS.32 into the 128-byte-
 //                          swizzled K-major operand tile (bf16 row = 256 B).
-//   warps 12-19 MMA +      two warpgroups, one per 64-row half of the tile: D[64 rows x NQ queries] (+)= Y_half . R^T on
-//               epilogue   wgmma m64nNQk16 (8 K-steps + 1 that adds -|y|^2/2: three bf16 pieces x ones), accumulator in
-//                          registers; each element is compared against its query's running threshold (shared memory), the
-//                          rare hits go into per-query candidate buffers; a buffer that overflows is compacted to its KC
-//                          best by one warp (rank by counting) and the threshold tightened; one named barrier per tile.
+//   warps 12-19 MMA +      two warpgroups.  NQ = 64 / 128: the queries are the MMA's M side, D[64 queries x 64 rows] (+)=
+//               epilogue   R . Y_half^T per 64-row half of the tile (NQ = 64), or D[64 queries x 128 rows] (+)= R_half . Y^T
+//                          per 64-query half of the item (NQ = 128), on wgmma m64nNQk16 (8 K-steps + 1 that adds -|y|^2/2:
+//                          ones x three bf16 pieces); a thread's fragment is 2 query rows x NQ / 4 list rows, so each query
+//                          row is tested with one max against one threshold and its hits reserve their buffer slots with one
+//                          atomic.  NQ = 32 (m64 would be half empty): the rows are the M side, D[64 rows x 32 queries] per
+//                          half, and each element is tested against its own query's threshold.  Hits go into per-query
+//                          candidate buffers; a buffer that overflows is compacted to its KC best by one warp (rank by
+//                          counting) and the threshold tightened; one named barrier per tile.
 //
 // With few probing queries per list (50M rows / 8192 lists / 10k-query batches at 48 probes: ~59) the accumulator is 128 x 32..64
-// instead of the 128 x 128 of the query-major kernel (scan_tc.cu), the rows fill the MMA's M side completely, and HBM
-// traffic per row is pq_dim + 4 bytes instead of a 2 * rot_dim + 32 byte decoded row.
+// instead of the 128 x 128 of the query-major kernel (scan_tc.cu), and HBM traffic per row is pq_dim + 4 bytes instead of a
+// 2 * rot_dim + 32 byte decoded row.
 #include "common.hpp"
 #include "ptx_sm90.cuh"
 #include "scan_pq.cuh"
@@ -129,9 +133,10 @@ __device__ __forceinline__ bool bar_red_or(uint32_t id, uint32_t nthreads, bool 
 __device__ __forceinline__ uint32_t okey(uint32_t fbits) { return (fbits & 0x80000000u) ? ~fbits : (fbits | 0x80000000u); }
 __device__ __forceinline__ uint32_t okey_inv(uint32_t k) { return (k & 0x80000000u) ? (k & 0x7fffffffu) : ~k; }
 
-// One tile's accumulator fragment (see ptx::wgmma_bf16: rows r0 and r0 + 8 of the tile, columns 8j + 2 * (lane % 4) + {0, 1})
-// against the query columns' running thresholds.  Only the elements flagged in `only` are looked at; returns the elements
-// whose candidate could not be stored (buffer full).
+// Rows-on-M fragment (NQ = 32; see ptx::wgmma_bf16: rows r0 and r0 + 8 of the tile, query columns 8j + 2 * (lane % 4) + {0, 1})
+// against the query columns' running thresholds: no two of a thread's elements share a query, so every element has its own
+// threshold and every hit its own slot-reserving atomic.  Only the elements flagged in `only` are looked at; returns the
+// elements whose candidate could not be stored (buffer full).
 template <int NQ>
 __device__ __forceinline__ uint64_t pq_filter_frag(const float (&d)[NQ / 2], uint64_t only, int lane, uint32_t pos0, uint32_t pos1,
                                                    const float* __restrict__ thr, int* cnt, unsigned long long* cand, int cap)
@@ -160,6 +165,63 @@ __device__ __forceinline__ uint64_t pq_filter_frag(const float (&d)[NQ / 2], uin
           if (at < cap) cand[col * cap + at] = (static_cast<unsigned long long>(okey(__float_as_uint(d[i]))) << 32) | (~pos);
           else left |= 1ull << i;
         }
+      }
+    }
+  }
+  return left;
+}
+
+// Queries-on-M fragment (NQ = 64 / 128; see ptx::wgmma_bf16: query rows q0 and q0 + 8, list rows 8j + 2 * (lane % 4) + {0, 1}
+// of the warpgroup's N side) against the two query rows' running thresholds.  Element k < NQ / 4 of query row q0 + 8h is
+// d[4 * (k / 2) + 2h + k % 2], list row pos0 + 8 * (k / 2) + k % 2; bit 32h + k of `only` and of the result stands for it.
+// A query row is tested with one max over its elements against one threshold (a candidate iff > threshold); a row with hits
+// reserves all its buffer slots with one atomic and then stores one hit per pass (constant register indices only: the
+// fragment stays in registers).  Returns the elements whose candidate could not be stored (buffer full).
+template <int NQ>
+__device__ __forceinline__ uint64_t pq_filter_rows(const float (&d)[NQ / 2], uint64_t only, int q0, uint32_t pos0,
+                                                   const float* __restrict__ thr, int* cnt, unsigned long long* cand, int cap)
+{
+  constexpr int NE = NQ / 4;
+  uint64_t left    = 0;
+  // (thresholds change only in compaction, between the per-tile barriers: read once per filter pass)
+  const float th[2] = {thr[q0], thr[q0 + 8]};
+  // four interleaved max chains per query row: short dependence chains, and few registers beside the fragment
+  float mx[2];
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    float v[4];
+#pragma unroll
+    for (int k = 0; k < 4; ++k) v[k] = d[4 * (k >> 1) + 2 * h + (k & 1)];
+#pragma unroll
+    for (int k = 4; k < NE; ++k) v[k & 3] = fmaxf(v[k & 3], d[4 * (k >> 1) + 2 * h + (k & 1)]);
+    mx[h] = fmaxf(fmaxf(v[0], v[1]), fmaxf(v[2], v[3]));
+  }
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    if (mx[h] > th[h]) {
+      uint32_t m = 0;
+#pragma unroll
+      for (int k = 0; k < NE; ++k) m |= (d[4 * (k >> 1) + 2 * h + (k & 1)] > th[h] ? 1u : 0u) << k;
+      m &= static_cast<uint32_t>(only >> (32 * h));
+      const int q = q0 + 8 * h;
+      int at      = m != 0u ? atomicAdd(&cnt[q], __popc(m)) : 0;
+      // one pass per hit: the hit's value is picked from the registers by a select tree on the bits of its index, so the
+      // warp runs as many passes as its lane with the most hits in this row, not one per element
+      while (m != 0u) {
+        const int k = __ffs(m) - 1;
+        m &= m - 1u;
+        float v[NE / 2];
+#pragma unroll
+        for (int j = 0; j < NE / 2; ++j) v[j] = (k & 1) ? d[4 * j + 2 * h + 1] : d[4 * j + 2 * h];
+#pragma unroll
+        for (int lv = 1; (NE >> lv) > 1; ++lv)
+#pragma unroll
+          for (int j = 0; j < NE / 4; ++j)  // (fixed inner trip count: both loops unroll, v stays in registers)
+            if (j < (NE >> (lv + 1))) v[j] = ((k >> lv) & 1) ? v[2 * j + 1] : v[2 * j];
+        const uint32_t pos = pos0 + 8 * (k >> 1) + (k & 1);
+        if (at < cap) cand[q * cap + at] = (static_cast<unsigned long long>(okey(__float_as_uint(v[0]))) << 32) | (~pos);
+        else left |= 1ull << (32 * h + k);
+        ++at;
       }
     }
   }
@@ -392,18 +454,24 @@ pq_stream_scan_kernel(const __grid_constant__ CUtensorMap tmQ_hi, const __grid_c
     }
   } else {
     ptx::setmaxnreg_inc<136>();  // 40 + 2 x 80 + 2 x 136 <= 5 x 96: only registers the other warpgroups gave back
-    // ------------------------------------------------------------------ MMA + epilogue: two warpgroups, one per 64-row half
-    // D[64 rows x NQ queries] (+)= Y_half . R^T on wgmma (8 K-steps + 1 that adds -|y|^2/2), then every accumulator element of
-    // the thread's fragment is compared against its query column's running threshold (shared memory); the rare hits go into
-    // per-query candidate buffers; a buffer that overflows is compacted to its KC best by one warp (rank by counting) and the
-    // threshold tightened, and the elements that did not fit are re-tested from the registers.
+    // ------------------------------------------------------------------ MMA + epilogue: two warpgroups
+    // NQ = 64: one per 64-row half of the tile, D[64 queries x 64 rows] (+)= R . Y_half^T; NQ = 128: one per 64-query half of
+    // the item, D[64 queries x 128 rows] (+)= R_half . Y^T; NQ = 32: one per 64-row half, D[64 rows x 32 queries] (+)=
+    // Y_half . R^T.  wgmma: 8 K-steps + 1 that adds -|y|^2/2.  Then the fragment is tested against the running thresholds
+    // (shared memory); the hits go into per-query candidate buffers; a buffer that overflows is compacted to its KC best
+    // by one warp (rank by counting) and the threshold tightened, and the elements that did not fit are re-tested from the
+    // registers.
+    constexpr bool kQM = NQ >= 64;                                   // queries on the MMA's M side
     const int ew = warp - kEpiWarp0;                                 // 0..7
     const int wg = ew >> 2;
     const int te = static_cast<int>(threadIdx.x) - 32 * kEpiWarp0;  // 0..255
-    const int r0 = 64 * wg + 16 * (ew & 3) + (lane >> 2);            // fragment rows r0 and r0 + 8 of the tile
-    const uint32_t q_lo0   = ptx::smem_desc_lo(ptx::smem_u32(sQ));
-    const uint32_t d_lo0   = ptx::smem_desc_lo(ptx::smem_u32(sDec)) + wg * 512;                  // + 64 rows of 128 B
-    const uint32_t x_lo0   = ptx::smem_desc_lo(ptx::smem_u32(sDec + NKB * kDecTile)) + wg * 128;  // + 64 rows of 32 B
+    // rows-on-M: fragment rows r0 and r0 + 8 of the tile; queries-on-M: query rows q0 and q0 + 8, list rows from rb on
+    const int r0 = 64 * wg + 16 * (ew & 3) + (lane >> 2);
+    const int q0 = (NQ == 128 ? 64 * wg : 0) + 16 * (ew & 3) + (lane >> 2);
+    const int rb = (NQ == 128 ? 0 : 64 * wg) + 2 * (lane & 3);
+    const uint32_t q_lo0   = ptx::smem_desc_lo(ptx::smem_u32(sQ)) + (NQ == 128 ? wg * 512 : 0);  // + 64 rows of 128 B
+    const uint32_t d_lo0   = ptx::smem_desc_lo(ptx::smem_u32(sDec)) + (NQ == 128 ? 0 : wg * 512);
+    const uint32_t x_lo0   = ptx::smem_desc_lo(ptx::smem_u32(sDec + NKB * kDecTile)) + (NQ == 128 ? 0 : wg * 128);  // 32 B rows
     const uint32_t ones_lo = ptx::smem_desc_lo(ptx::smem_u32(sOnes));
     const int cap = P.cap, KC = P.KC;
     const int kth = (P.kth > 0 && P.kth < KC) ? P.kth : KC;
@@ -464,15 +532,22 @@ pq_stream_scan_kernel(const __grid_constant__ CUtensorMap tmQ_hi, const __grid_c
         for (int kb = 0; kb < NKB; ++kb) {
 #pragma unroll
           for (int k = 0; k < 4; ++k) {
-            const uint32_t a = a0 + kb * (kDecTile >> 4) + k * 2;  // decoded rows: the M side
-            const uint32_t b = q_lo0 + kb * (L::q_tile >> 4) + k * 2;
-            ptx::wgmma_bf16<NQ>(d, ptx::desc(a, ptx::kDescHiSw128), ptx::desc(b, ptx::kDescHiSw128), (kb | k) != 0 ? 1u : 0u);
-            if (PASSES == 2)
-              ptx::wgmma_bf16<NQ>(d, ptx::desc(a, ptx::kDescHiSw128), ptx::desc(b + NKB * (L::q_tile >> 4), ptx::kDescHiSw128), 1u);
+            const uint64_t y  = ptx::desc(a0 + kb * (kDecTile >> 4) + k * 2, ptx::kDescHiSw128);  // decoded rows
+            const uint32_t qd = q_lo0 + kb * (L::q_tile >> 4) + k * 2;                          // residual rows
+            const uint64_t r  = ptx::desc(qd, ptx::kDescHiSw128);
+            if (kQM) ptx::wgmma_bf16<NQ>(d, r, y, (kb | k) != 0 ? 1u : 0u);
+            else ptx::wgmma_bf16<NQ>(d, y, r, (kb | k) != 0 ? 1u : 0u);
+            if (PASSES == 2) {
+              const uint64_t rl = ptx::desc(qd + NKB * (L::q_tile >> 4), ptx::kDescHiSw128);
+              if (kQM) ptx::wgmma_bf16<NQ>(d, rl, y, 1u);
+              else ptx::wgmma_bf16<NQ>(d, y, rl, 1u);
+            }
           }
         }
         // -= |y|^2/2 : ext rows hold the three bf16 pieces of -hn/2 in both chunks, ones rows three 1s in both chunks
-        ptx::wgmma_bf16<NQ>(d, ptx::desc(x_lo0 + ds * (L::dec_stage >> 4), ptx::kDescHiSw32), ptx::desc(ones_lo, ptx::kDescHiSw32), 1u);
+        const uint64_t xd = ptx::desc(x_lo0 + ds * (L::dec_stage >> 4), ptx::kDescHiSw32), od = ptx::desc(ones_lo, ptx::kDescHiSw32);
+        if (kQM) ptx::wgmma_bf16<NQ>(d, od, xd, 1u);
+        else ptx::wgmma_bf16<NQ>(d, xd, od, 1u);
         ptx::wgmma_commit();
         ptx::wgmma_wait<0>();
         __syncwarp();
@@ -482,14 +557,18 @@ pq_stream_scan_kernel(const __grid_constant__ CUtensorMap tmQ_hi, const __grid_c
         }
         if (++ds == kDecStages) { ds = 0; dph ^= 1; }
 
-        const uint32_t pos0 = item.b_row0 + t * 128 + r0;
-        uint64_t left = pq_filter_frag<NQ>(d, ~0ull, lane, pos0, pos0 + 8, sThr, sCnt, sCand, cap);
+        const uint32_t pos0 = item.b_row0 + t * 128 + (kQM ? rb : r0);
+        auto filter = [&](uint64_t only) -> uint64_t {
+          if constexpr (kQM) return pq_filter_rows<NQ>(d, only, q0, pos0, sThr, sCnt, sCand, cap);
+          else return pq_filter_frag<NQ>(d, only, lane, pos0, pos0 + 8, sThr, sCnt, sCand, cap);
+        };
+        uint64_t left = filter(~0ull);
         // ONE barrier per tile decides whether any buffer overflowed
         while (bar_red_or(1, kEpiThreads, left != 0)) {
           for (int col = ew; col < NQ; col += kEpiWarps)
             if (sCnt[col] > cap) compact(col);  // (warp-uniform: every lane reads the same counter)
           ptx::named_bar_sync(1, kEpiThreads);
-          if (left != 0) left = pq_filter_frag<NQ>(d, left, lane, pos0, pos0 + 8, sThr, sCnt, sCand, cap);
+          if (left != 0) left = filter(left);
         }
       }
       qph ^= 1;
