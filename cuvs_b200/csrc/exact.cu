@@ -140,7 +140,8 @@ __global__ void __launch_bounds__(256) exact_tile_kernel(const float* __restrict
   }
 }
 
-constexpr int kMaxCand = 256;
+constexpr int kMaxCand      = 256;   // one warp per query
+constexpr int kMaxCandBlock = 2048;  // one CTA per query
 
 // one warp per query
 __global__ void __launch_bounds__(128) rescore_kernel(const float* __restrict__ q, int64_t nq, int64_t ldq,
@@ -272,6 +273,96 @@ __global__ void __launch_bounds__(128) rescore_kernel(const float* __restrict__ 
   }
 }
 
+// More candidates than one warp's shared memory holds (refine with 257..2048 candidates): one CTA per query.  Every candidate
+// is scored by one thread with rescore_kernel's arithmetic (same fmaf order, same vec4 rule), then the kc entries are sorted by
+// rescore_kernel's ranking rule, (distance, id, slot), with a bitonic sort over kpow2 entries; the padding entries (slot >= kc)
+// rank last.
+__global__ void __launch_bounds__(256) rescore_block_kernel(const float* __restrict__ q, int64_t ldq, const float* __restrict__ x,
+                                                             int64_t ldx, int d, const float* __restrict__ qn,
+                                                             const float* __restrict__ xn, int metric,
+                                                             const uint32_t* __restrict__ cand_pos, int kc, int kpow2,
+                                                             const int64_t* __restrict__ src_ids, int k,
+                                                             int64_t* __restrict__ out_idx, float* __restrict__ out_dist, int64_t pad_id)
+{
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  int64_t* si = reinterpret_cast<int64_t*>(smem_raw);
+  float* sd   = reinterpret_cast<float*>(si + kpow2);
+  int* sc     = reinterpret_cast<int*>(sd + kpow2);
+  const int64_t qi      = blockIdx.x;
+  const bool select_min = metric != InnerProduct;
+  const float* qr       = q + qi * ldq;
+  const float qnv       = qn ? qn[qi] : 0.f;
+  const bool sqdiff     = (metric == L2Unexpanded || metric == L2SqrtUnexpanded);
+  const bool vec4       = ((d & 3) == 0) && ((ldx & 3) == 0) && ((ldq & 3) == 0) &&
+                    ((reinterpret_cast<uintptr_t>(x) & 15) == 0) && ((reinterpret_cast<uintptr_t>(q) & 15) == 0);
+  for (int c = threadIdx.x; c < kpow2; c += blockDim.x) {
+    float dist = select_min ? FLT_MAX : -FLT_MAX;
+    int64_t id = INT64_MAX;
+    const uint32_t pos = c < kc ? cand_pos[qi * kc + c] : 0xffffffffu;
+    if (pos != 0xffffffffu) {
+      const float* xr = x + static_cast<int64_t>(pos) * ldx;
+      float acc       = 0.f;
+      if (vec4) {
+        const float4* x4 = reinterpret_cast<const float4*>(xr);
+        const float4* q4 = reinterpret_cast<const float4*>(qr);
+        for (int kk = 0; kk < d / 4; ++kk) {
+          float4 a = q4[kk], b = x4[kk];
+          if (sqdiff) {
+            float t;
+            t = a.x - b.x; acc = fmaf(t, t, acc);
+            t = a.y - b.y; acc = fmaf(t, t, acc);
+            t = a.z - b.z; acc = fmaf(t, t, acc);
+            t = a.w - b.w; acc = fmaf(t, t, acc);
+          } else {
+            acc = fmaf(a.x, b.x, acc);
+            acc = fmaf(a.y, b.y, acc);
+            acc = fmaf(a.z, b.z, acc);
+            acc = fmaf(a.w, b.w, acc);
+          }
+        }
+      } else {
+        for (int kk = 0; kk < d; ++kk) {
+          if (sqdiff) { float t = qr[kk] - xr[kk]; acc = fmaf(t, t, acc); }
+          else acc = fmaf(qr[kk], xr[kk], acc);
+        }
+      }
+      dist = finish_distance(acc, qnv, xn ? xn[pos] : 0.f, metric);
+      id   = src_ids ? src_ids[pos] : static_cast<int64_t>(pos);
+    }
+    sd[c] = dist;
+    si[c] = id;
+    sc[c] = c;
+  }
+  __syncthreads();
+  // a before b in the ranking (slots are unique, so this is a strict total order)
+  auto before = [&](float da, int64_t ia, int ca, float db, int64_t ib, int cb) {
+    const bool pa = ca >= kc, pb = cb >= kc;
+    if (pa != pb) return pb;
+    if (da != db) return select_min ? da < db : da > db;
+    return ia != ib ? ia < ib : ca < cb;
+  };
+  for (int size = 2; size <= kpow2; size <<= 1) {
+    for (int stride = size >> 1; stride > 0; stride >>= 1) {
+      for (int i = threadIdx.x; i < (kpow2 >> 1); i += blockDim.x) {
+        const int lo = (i / stride) * (stride << 1) + (i % stride), hi = lo + stride;
+        const bool up = (lo & size) == 0;
+        const bool swap = before(sd[hi], si[hi], sc[hi], sd[lo], si[lo], sc[lo]) == up;
+        if (swap) {
+          const float td = sd[lo]; sd[lo] = sd[hi]; sd[hi] = td;
+          const int64_t ti = si[lo]; si[lo] = si[hi]; si[hi] = ti;
+          const int tc = sc[lo]; sc[lo] = sc[hi]; sc[hi] = tc;
+        }
+      }
+      __syncthreads();
+    }
+  }
+  for (int j = threadIdx.x; j < k; j += blockDim.x) {
+    const int64_t iv = si[j];
+    out_idx[qi * k + j]  = iv != INT64_MAX ? iv : pad_id;
+    out_dist[qi * k + j] = sd[j];
+  }
+}
+
 __global__ void postprocess_kernel(float* dist, int64_t count, int metric)
 {
   int64_t i = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x;
@@ -334,6 +425,18 @@ void rescore_topk(cudaStream_t stream, const float* q, int64_t nq, int64_t ldq, 
                   int64_t pad_id, const approx_map& amap, int* flags, int* n_flagged, const float* approx_floor)
 {
   if (nq == 0) return;
+  if (kc > kMaxCand) {
+    B2_EXPECTS(kc <= kMaxCandBlock && k <= kc, "rescore_topk: candidate count %d out of range", kc);
+    B2_EXPECTS(cand_score == nullptr && flags == nullptr, "rescore_topk: the certificate takes at most %d candidates", kMaxCand);
+    int kpow2 = 1;
+    while (kpow2 < kc) kpow2 <<= 1;
+    const size_t smem = static_cast<size_t>(kpow2) * (sizeof(int64_t) + sizeof(float) + sizeof(int));
+    count_launch();
+    rescore_block_kernel<<<static_cast<unsigned>(nq), 256, smem, stream>>>(q, ldq, x, ldx, d, qn, xn, int(metric), cand_pos, kc, kpow2,
+                                                                          src_ids, k, out_idx, out_dist, pad_id);
+    B2_CUDA(cudaGetLastError());
+    return;
+  }
   B2_EXPECTS(kc >= 1 && kc <= kMaxCand, "rescore_topk: candidate count %d out of range", kc);
   const int warps = 4;
   size_t smem     = static_cast<size_t>(warps) * kc * (sizeof(float) + sizeof(int64_t));

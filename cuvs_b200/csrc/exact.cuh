@@ -55,6 +55,8 @@ struct approx_map {
  * k-th exact distance is strictly better than (worst candidate approx score -/+ eps_i), where
  * eps_i comes from `amap` (for L2: eps_rel * (|q_i|^2 + max_j |x_j|^2)): the certificate that no non-candidate can
  * belong to the exact top-k (DESIGN.md §3).
+ * kc <= 256 runs one warp per query; 256 < kc <= 2048 (no certificate: cand_score and flags null, k <= kc) one CTA per
+ * query with the same arithmetic and ranking.
  */
 void rescore_topk(cudaStream_t stream, const float* q, int64_t nq, int64_t ldq, const float* x, int64_t ldx, int d,
                   const float* qn, const float* xn, cuvsDistanceType metric, const uint32_t* cand_pos,

@@ -46,6 +46,7 @@
 #include <cstdlib>
 #include <cstring>
 #include <fstream>
+#include <functional>
 #include <memory>
 #include <random>
 #include <vector>
@@ -395,17 +396,66 @@ __global__ void finish_ids_kernel(const uint32_t* __restrict__ pos, const int64_
   dist[i] = d;
 }
 
+// ---- k > 64: dense per-pair score segments (DESIGN.md §5 "k > 64")
+// Slot i (a live pair of list l) owns scores[seg_off[i] .. + padded size of l): its list's rows in list order.  seg_len is the
+// list's real size (the padding rows at its end are never selected) and seg_base its first index row, so that a column c of
+// the segment is index row seg_base + c.  Slots are few (nq * n_probes): one CTA scans them, each thread a contiguous chunk.
+__global__ void __launch_bounds__(1024) pair_segments_kernel(const uint32_t* __restrict__ pair_list, const int* __restrict__ n_live,
+                                                             int64_t n_pairs, const int64_t* __restrict__ list_offsets,
+                                                             const uint32_t* __restrict__ list_sizes, int64_t* __restrict__ seg_off,
+                                                             uint32_t* __restrict__ seg_len, uint32_t* __restrict__ seg_base)
+{
+  __shared__ int64_t part[1024];
+  const int tid      = threadIdx.x;
+  const int64_t live = *n_live;
+  const int64_t per  = (n_pairs + 1023) / 1024;
+  const int64_t b = min(n_pairs, tid * per), e = min(n_pairs, b + per);
+  int64_t sum = 0;
+  for (int64_t i = b; i < min(e, live); ++i) sum += list_offsets[pair_list[i] + 1] - list_offsets[pair_list[i]];
+  part[tid] = sum;
+  __syncthreads();
+  for (int o = 1; o < 1024; o <<= 1) {
+    const int64_t v = tid >= o ? part[tid - o] : 0;
+    __syncthreads();
+    part[tid] += v;
+    __syncthreads();
+  }
+  int64_t run = part[tid] - sum;
+  for (int64_t i = b; i < e; ++i) {
+    seg_off[i] = run;
+    if (i < live) {
+      const uint32_t l = pair_list[i];
+      seg_len[i]       = list_sizes[l];
+      seg_base[i]      = static_cast<uint32_t>(list_offsets[l]);
+      run += list_offsets[l + 1] - list_offsets[l];
+    } else {
+      seg_len[i]  = 0;
+      seg_base[i] = 0;
+    }
+  }
+}
+
+// the stream kernel's store epilogue writes an item's pairs from the segment of its first slot on
+__global__ void item_segments_kernel(tc_item* __restrict__ items, const int* __restrict__ n_items, const int64_t* __restrict__ seg_off)
+{
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < *n_items) items[i].out_off = static_cast<uint64_t>(seg_off[items[i].a_row0]);
+}
+
 // ---- (A) LUT scan: one CTA per (query, probe) slot ------------------------------------------------
 constexpr int kLutThreads = 128;
 constexpr int kLutBuf     = 256;  // candidate buffer (entries) per CTA
 
-template <typename LutT, typename OutT>
+// Store mode (k > 64, Store = true): no selection in the kernel.  The CTA writes the score of every row of its list, in list
+// order, to the pair's segment out_score[seg_off[slot] ...] (padding rows +inf); KC, out_pos and KCW are unused.
+template <typename LutT, typename OutT, bool Store = false>
 __global__ void __launch_bounds__(kLutThreads)
 pq_lut_scan_kernel(const float* __restrict__ q_rot, const float* __restrict__ centers_rot, const float* __restrict__ pq_centers,
                    int per_cluster, const uint8_t* __restrict__ codes, const int64_t* __restrict__ list_offsets,
                    const uint32_t* __restrict__ list_sizes, const uint32_t* __restrict__ pair_query,
                    const uint32_t* __restrict__ pair_list, const int* __restrict__ n_live, int rot_dim, int pq_dim, int pq_len, int pq_bits, bool ip, bool cosine,
-                   int KC, float* __restrict__ out_score, uint32_t* __restrict__ out_pos, int KCW)
+                   int KC, float* __restrict__ out_score, uint32_t* __restrict__ out_pos, int KCW,
+                   const int64_t* __restrict__ seg_off)
 {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   const int book     = 1 << pq_bits;
@@ -457,6 +507,35 @@ pq_lut_scan_kernel(const float* __restrict__ q_rot, const float* __restrict__ ce
   const uint32_t n   = list_sizes[l];
   const int vec16    = pq_dim / 16;  // uint4 loads per row when pq_dim % 16 == 0
   const bool aligned = (pq_dim % 16 == 0);
+
+  if constexpr (Store) {
+    float* seg         = out_score + seg_off[slot];
+    const uint32_t pad = static_cast<uint32_t>(list_offsets[l + 1] - row0);
+    for (uint32_t i = threadIdx.x; i < pad; i += blockDim.x) {
+      float fs = INFINITY;
+      if (i < n) {
+        const uint8_t* code = codes + (row0 + i) * pq_dim;
+        OutT score = OutT(0.f);
+        if (aligned) {
+          for (int v = 0; v < vec16; ++v) {
+            const uint4 w = reinterpret_cast<const uint4*>(code)[v];
+            const uint32_t ws[4] = {w.x, w.y, w.z, w.w};
+#pragma unroll
+            for (int b = 0; b < 16; ++b) {
+              const uint32_t cdx = (ws[b >> 2] >> ((b & 3) * 8)) & 0xffu;
+              score += OutT(lut_conv<LutT>::dec(lut[((v * 16 + b) << pq_bits) + cdx], ip));
+            }
+          }
+        } else {
+          for (int s = 0; s < pq_dim; ++s) score += OutT(lut_conv<LutT>::dec(lut[(s << pq_bits) + code[s]], ip));
+        }
+        fs = float(score);
+        if (cosine) fs += 1.0f;
+      }
+      seg[i] = fs;
+    }
+    return;
+  }
 
   auto compact = [&](int keep) {
     // rank compaction: keep the `keep` best of the buffer, sorted, at the front
@@ -872,6 +951,114 @@ int env_path()  // read on every search: tests switch paths inside one process
   return strcmp(e, "lut") == 0 ? 1 : (strcmp(e, "tc") == 0 ? 2 : (strcmp(e, "stream") == 0 ? 3 : 0));  // stream: never the decoded-row cache
 }
 
+// k > 64: upper bound on the dense score rows of one query, the sum of the n_probes largest padded lists
+int64_t large_k_rows_per_query(const ivf_pq_index& idx, uint32_t n_probes)
+{
+  std::vector<int64_t> pad(idx.n_lists);
+  for (uint32_t l = 0; l < idx.n_lists; ++l) pad[l] = idx.lists.h_offsets[l + 1] - idx.lists.h_offsets[l];
+  const uint32_t m = std::min<uint32_t>(n_probes, idx.n_lists);
+  std::partial_sort(pad.begin(), pad.begin() + m, pad.end(), std::greater<int64_t>());
+  int64_t rows = 0;
+  for (uint32_t i = 0; i < m; ++i) rows += pad[i];
+  return rows;
+}
+
+// k > 64: bytes of workspace one query batch may take (dense scores + per-pair top-k + merge buffers).  Default min(8 GiB, half
+// of the free device memory); CUVS_B200_PQ_LARGE_K_BUDGET_MB overrides it (read per call).
+int64_t large_k_budget()
+{
+  if (const char* e = getenv("CUVS_B200_PQ_LARGE_K_BUDGET_MB")) return std::max<int64_t>(1, atoll(e)) << 20;
+  size_t free_b = 0, total_b = 0;
+  B2_CUDA(cudaMemGetInfo(&free_b, &total_b));
+  return std::min<int64_t>(int64_t(8) << 30, static_cast<int64_t>(free_b / 2));
+}
+
+// k > 64 (DESIGN.md §5 "k > 64"): the scan writes every (pair, list row) score to the pair's dense segment (store epilogue of
+// the code-stream kernel for stream indexes, store mode of the LUT kernel for every other index), a segmented select takes each
+// pair's k best with their index rows, and the probes of a query are merged as on the k <= 64 path with KCW = k.  Scores of
+// one pair differ from its distances only by the pair's `add` and a positive `scale`, so the per-pair order is the final one.
+void search_large_k(resources* res, const ivf_pq_index& idx, const cuvsIvfPqSearchParams& sp, const float* q_rot, const uint32_t* probes,
+                    int64_t nq, uint32_t n_probes, int k, int64_t* out_idx, float* out_dist)
+{
+  auto s            = res->stream;
+  const bool ip     = is_ip(idx.metric);
+  const bool cosine = idx.metric == CosineExpanded;
+  const bool reduced    = !(sp.lut_dtype == CUDA_R_32F && sp.internal_distance_dtype == CUDA_R_32F);
+  const bool use_stream = env_path() != 1 && idx.cstream.data() != nullptr;
+  const int passes      = reduced ? 1 : 2;
+  const int group = use_stream ? pq_stream_group(static_cast<double>(nq) * n_probes / std::max<uint32_t>(idx.n_lists, 1), 0, passes) : 128;
+  probe_buckets pb;
+  bucket_probes(res, probes, nq, static_cast<int>(n_probes), idx.n_lists, idx.lists.d_offsets.data(), 0, pb, 0, 0xffffffffu, group);
+  const int64_t n_pairs = pb.n_pairs;
+  dbuf<int64_t> seg_off(static_cast<size_t>(n_pairs), s);
+  dbuf<uint32_t> seg_len(static_cast<size_t>(n_pairs), s), seg_base(static_cast<size_t>(n_pairs), s);
+  count_launch();
+  pair_segments_kernel<<<1, 1024, 0, s>>>(pb.pair_list.data(), pb.n_items.data() + 1, n_pairs, idx.lists.d_offsets.data(),
+                                          idx.lists.d_sizes.data(), seg_off.data(), seg_len.data(), seg_base.data());
+  B2_CUDA(cudaGetLastError());
+  dbuf<float> scores(static_cast<size_t>(std::max<int64_t>(1, nq * large_k_rows_per_query(idx, n_probes))), s);
+  dbuf<float> add;
+  float scale = 1.0f;
+  if (use_stream) {
+    const int64_t a_rows = n_pairs + 128;
+    dbuf<__nv_bfloat16> a_hi(static_cast<size_t>(a_rows) * idx.Kp, s), a_lo;
+    if (passes == 2) a_lo.alloc(static_cast<size_t>(a_rows) * idx.Kp, s);
+    add.alloc(static_cast<size_t>(n_pairs), s);
+    count_launch(2);
+    pair_rows_kernel<<<blocks_for(a_rows * 32, 256), 256, 0, s>>>(q_rot, idx.centers_rot.data(), pb.pair_query.data(), pb.pair_list.data(),
+                                                                   pb.n_items.data() + 1, a_rows, idx.rot_dim, idx.Kp, ip, a_hi.data(),
+                                                                   a_lo.data(), add.data(), true, cosine);
+    item_segments_kernel<<<blocks_for(pb.max_items, 256), 256, 0, s>>>(pb.items.data(), pb.n_items.data(), seg_off.data());
+    B2_CUDA(cudaGetLastError());
+    scale = ip ? 1.0f : 2.0f;
+    timed_section ts("pq_scan", s);
+    pq_stream_scan(s, res->device, a_hi.data(), a_lo.data(), a_rows, idx.Kp, idx.cstream.data(), idx.cb_words.data(), idx.pq_dim,
+                   pb.items.data(), pb.max_items, pb.n_items.data(), group, 0, passes, scores.data(), nullptr, 0, nullptr);
+  } else {
+    ensure_flat_codes(res, idx);
+    const size_t lut_b = sp.lut_dtype == CUDA_R_32F ? 4 : (sp.lut_dtype == CUDA_R_16F ? 2 : 1);
+    const size_t smem  = ((static_cast<size_t>(idx.pq_dim) * idx.book() * lut_b + 15) & ~size_t(15)) + 2 * idx.rot_dim * sizeof(float);
+    B2_EXPECTS(smem <= 227 * 1024, "ivf_pq: LUT (%zu bytes) does not fit in shared memory; use a smaller lut_dtype", smem);
+    const bool half_out = sp.internal_distance_dtype == CUDA_R_16F;
+    const bool per_cl   = idx.codebook_kind == CUVS_IVF_PQ_CODEBOOK_GEN_PER_CLUSTER;
+#define B2_LUT_STORE(LUT_T, OUT_T)                                                                                          \
+  {                                                                                                                         \
+    auto kern = pq_lut_scan_kernel<LUT_T, OUT_T, true>;                                                                     \
+    B2_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));               \
+    timed_section ts("pq_scan", s);                                                                                         \
+    count_launch();                                                                                                         \
+    kern<<<static_cast<unsigned>(n_pairs), kLutThreads, smem, s>>>(                                                         \
+      q_rot, idx.centers_rot.data(), idx.pq_centers.data(), per_cl, idx.codes.data(), idx.lists.d_offsets.data(),          \
+      idx.lists.d_sizes.data(), pb.pair_query.data(), pb.pair_list.data(), pb.n_items.data() + 1, idx.rot_dim, idx.pq_dim, \
+      idx.pq_len, idx.pq_bits, ip, cosine, 0, scores.data(), nullptr, 0, seg_off.data());                                  \
+  }
+    if (sp.lut_dtype == CUDA_R_32F) B2_LUT_STORE(float, float)
+    else if (sp.lut_dtype == CUDA_R_16F && !half_out) B2_LUT_STORE(__half, float)
+    else if (sp.lut_dtype == CUDA_R_16F && half_out) B2_LUT_STORE(__half, __half)
+    else if (!half_out) B2_LUT_STORE(uint8_t, float)
+    else B2_LUT_STORE(uint8_t, __half)
+#undef B2_LUT_STORE
+    B2_CUDA(cudaGetLastError());
+  }
+  // per pair: its k best rows (positions are index rows); ties go to the smaller row
+  int64_t max_len = 0;
+  for (int64_t v : idx.lists.h_sizes) max_len = std::max(max_len, v);
+  dbuf<float> cs(static_cast<size_t>(n_pairs) * k, s);
+  dbuf<uint32_t> cp(static_cast<size_t>(n_pairs) * k, s);
+  select_k_segments(s, scores.data(), seg_off.data(), seg_len.data(), seg_base.data(), n_pairs, max_len, k, cs.data(), cp.data(), true);
+  scores.release();
+  // per query: its probes' k best, in distance units, then the k best of those
+  const int64_t cand_w = static_cast<int64_t>(n_probes) * k;
+  dbuf<float> gs(static_cast<size_t>(nq * cand_w), s);
+  dbuf<uint32_t> gp(static_cast<size_t>(nq * cand_w), s), mp(static_cast<size_t>(nq) * k, s);
+  count_launch(2);
+  gather_pq_cands_kernel<<<blocks_for(nq * cand_w, 256), 256, 0, s>>>(cs.data(), cp.data(), pb.slot_of.data(), use_stream ? add.data() : nullptr,
+                                                                       scale, nq * cand_w, k, gs.data(), gp.data());
+  select_k(s, gs.data(), gp.data(), IDX_U32, nq, cand_w, cand_w, k, out_dist, mp.data(), IDX_U32, true);
+  finish_ids_kernel<<<blocks_for(nq * k, 256), 256, 0, s>>>(mp.data(), idx.ids.data(), out_dist, nq * k, int(idx.metric), out_idx);
+  B2_CUDA(cudaGetLastError());
+}
+
 void ivf_pq_search(resources* res, const ivf_pq_index& idx, const cuvsIvfPqSearchParams& sp, const DLTensor& qt, const DLTensor& nt,
                    const DLTensor& dt)
 {
@@ -880,7 +1067,7 @@ void ivf_pq_search(resources* res, const ivf_pq_index& idx, const cuvsIvfPqSearc
   const int k      = static_cast<int>(nt.shape[1]);
   B2_EXPECTS(qt.shape[1] == idx.dim, "queries dim (%lld) != index dim (%d)", (long long)qt.shape[1], idx.dim);
   B2_EXPECTS(nt.shape[0] == nq && dt.shape[0] == nq && dt.shape[1] == k, "neighbors/distances shape mismatch");
-  B2_EXPECTS(k >= 1 && k <= 64, "ivf_pq search: k must be in [1, 64] in this build (got %d)", k);
+  B2_EXPECTS(k >= 1 && k <= kSelectMaxK, "ivf_pq search: k must be in [1, %d] (got %d)", kSelectMaxK, k);
   B2_EXPECTS(sp.n_probes >= 1, "n_probes must be >= 1");
   B2_EXPECTS(sp.lut_dtype == CUDA_R_32F || sp.lut_dtype == CUDA_R_16F || sp.lut_dtype == CUDA_R_8U, "unsupported lut_dtype");
   B2_EXPECTS(sp.internal_distance_dtype == CUDA_R_32F || sp.internal_distance_dtype == CUDA_R_16F, "unsupported internal_distance_dtype");
@@ -894,6 +1081,12 @@ void ivf_pq_search(resources* res, const ivf_pq_index& idx, const cuvsIvfPqSearc
     int64_t batch = std::max<int64_t>(1, (int64_t(3) << 30) / per_query);
     batch         = std::min<int64_t>(batch, (int64_t(1) << 31) / std::max<uint32_t>(n_probes, 1));
     if (sp.max_internal_batch_size > 0 && n_probes > 256) batch = std::min<int64_t>(batch, std::max<uint32_t>(sp.max_internal_batch_size, 128));
+    if (k > 64) {
+      // k > 64: dense scores (bounded per query by its n_probes largest lists), per-pair top-k and the merge's gathered
+      // candidates (8 bytes each), residual rows and slot bookkeeping, under the workspace budget
+      const int64_t per_q = large_k_rows_per_query(idx, n_probes) * 4 + static_cast<int64_t>(n_probes) * (16 * k + 4 * idx.Kp + 48);
+      batch = std::min<int64_t>(batch, std::max<int64_t>(1, large_k_budget() / per_q));
+    }
     if (nq > batch) {
       for (int64_t q0 = 0; q0 < nq; q0 += batch) {
         const int64_t rows = std::min(batch, nq - q0);
@@ -919,6 +1112,7 @@ void ivf_pq_search(resources* res, const ivf_pq_index& idx, const cuvsIvfPqSearc
   // not depend on |q|, so the probes above come from the raw queries, as in the reference.
   const bool cosine = idx.metric == CosineExpanded;
   if (cosine) normalize_rows(s, q_rot.data(), nq, idx.rot_dim, idx.rot_dim);
+  if (k > 64) return search_large_k(res, idx, sp, q_rot.data(), probes.data(), nq, n_probes, k, out_idx, out_dist);
 
   // ---- bucket pairs by list
   // Decoded-row tensor-core scan whenever the index keeps decoded rows.  fp32 LUT + fp32 accumulation (the reference's
@@ -940,7 +1134,6 @@ void ivf_pq_search(resources* res, const ivf_pq_index& idx, const cuvsIvfPqSearc
   // them fall into one half — an approximation only the k > 32 candidate-generation use case can see)
   const int KC    = k <= 16 ? 16 : (k <= 32 || (use_tc && !use_stream) ? 32 : 64);
   const int KCW   = KC * lists;
-  B2_EXPECTS(KCW >= k, "ivf_pq search: k = %d > 64 needs an index with decoded rows (CUVS_B200_PQ_KEEP_DECODED=1) or the LUT path (CUVS_B200_PQ_PATH=lut)", k);
   // queries per work item: 128 for the query-major kernels; the streamed kernel takes 32 / 64 / 128 probing queries (picked
   // from the average number of pairs per list), as the MMA's M side at 64 / 128 and as its N side at 32
   const int group = use_stream ? pq_stream_group(static_cast<double>(nq) * n_probes / std::max<uint32_t>(idx.n_lists, 1), KC, passes) : 128;
@@ -1005,7 +1198,7 @@ void ivf_pq_search(resources* res, const ivf_pq_index& idx, const cuvsIvfPqSearc
     kern<<<static_cast<unsigned>(pb.n_pairs), kLutThreads, smem, s>>>(                                                      \
       q_rot.data(), idx.centers_rot.data(), idx.pq_centers.data(), per_cl, idx.codes.data(), idx.lists.d_offsets.data(),   \
       idx.lists.d_sizes.data(), pb.pair_query.data(), pb.pair_list.data(), pb.n_items.data() + 1, idx.rot_dim, idx.pq_dim, idx.pq_len, idx.pq_bits, ip,  \
-      cosine, KC, cs.data(), cp.data(), KCW);                                                                               \
+      cosine, KC, cs.data(), cp.data(), KCW, nullptr);                                                                      \
   }
     if (sp.lut_dtype == CUDA_R_32F) B2_LUT_LAUNCH(float, float)
     else if (sp.lut_dtype == CUDA_R_16F && !half_out) B2_LUT_LAUNCH(__half, float)

@@ -1,7 +1,8 @@
 // Exact re-ranking of ANN candidates (cuvsRefine).
 // Reference: cpp/src/neighbors/refine/refine_device.cuh:30-130 (re-uses the IVF-Flat scan over a fake
-// one-list-per-query index), c/src/neighbors/refine.cpp.  Here: one warp per query gathers its
-// candidates' rows and scores them in fp32 (oracle arithmetic), then ranks by (distance, id) — exact.cu.
+// one-list-per-query index), c/src/neighbors/refine.cpp.  Here: one warp per query (up to 256 candidates; one CTA per query
+// up to 2048) gathers its candidates' rows and scores them in fp32 (oracle arithmetic), then ranks by (distance, id) —
+// exact.cu.
 #include "common.hpp"
 #include "exact.cuh"
 #include "timing.hpp"
@@ -46,7 +47,7 @@ extern "C" cuvsError_t cuvsRefine(cuvsResources_t res, DLManagedTensor* dataset_
     const int d = static_cast<int>(ds.shape[1]), n_cand = static_cast<int>(c.shape[1]), k = static_cast<int>(oi.shape[1]);
     B2_EXPECTS(q.shape[1] == d && c.shape[0] == nq && oi.shape[0] == nq && od.shape[0] == nq && od.shape[1] == k, "refine: shape mismatch");
     B2_EXPECTS(k <= n_cand, "refine: k (%d) must not exceed the number of candidates (%d)", k, n_cand);
-    B2_EXPECTS(n_cand <= 256, "refine: at most 256 candidates per query are supported (got %d)", n_cand);
+    B2_EXPECTS(n_cand <= 2048, "refine: at most 2048 candidates per query are supported (got %d)", n_cand);
     B2_EXPECTS(n < (int64_t(1) << 32) - 1, "refine: dataset too large");
     if (nq == 0) return;
     auto s = r->stream;

@@ -275,7 +275,12 @@ struct layout {
   static_assert(q_tile % 1024 == 0 && dec_stage % 1024 == 0, "operand tiles need 1024-byte alignment");
 };
 
-template <int NQ, int NKB, int PASSES>
+// (STORE ends its item with `continue`: the filtering epilogue after it is then unreachable, which is intended)
+#pragma nv_diag_suppress 128
+// STORE (KC = 0, k > 64): no threshold filter, candidate buffers, compaction or bound.  The consumers write the score of every
+// (query column, list row) of the item to out_score[out_off + col * n_tiles * 128 + row]: one dense segment per pair, its
+// list's padded rows in list order (padding rows +inf).
+template <int NQ, int NKB, int PASSES, bool STORE = false>
 __global__ void __launch_bounds__(kThreads, 1)
 pq_stream_scan_kernel(const __grid_constant__ CUtensorMap tmQ_hi, const __grid_constant__ CUtensorMap tmQ_lo, const pq_args P)
 {
@@ -505,6 +510,69 @@ pq_stream_scan_kernel(const __grid_constant__ CUtensorMap tmQ_hi, const __grid_c
       if (++ss == kSched) { ss = 0; sp ^= 1; }
       if (it < 0) break;
       const tc_item item = P.items[it];
+      if constexpr (STORE) {
+        wait_dbg(P.dbg, q_full, qph, 0x202, static_cast<uint32_t>(it), 0);
+        const int64_t seg = static_cast<int64_t>(item.n_tiles) * 128;  // a pair's segment: its list's padded rows
+        float* out        = P.out_score + item.out_off;
+        for (uint32_t t = 0; t < item.n_tiles; ++t) {
+          wait_dbg(P.dbg, &d_full[ds], dph, 0x204, static_cast<uint32_t>(it), t);
+          float d[NQ / 2];
+          ptx::wgmma_fence();
+          const uint32_t a0 = d_lo0 + ds * (L::dec_stage >> 4);
+#pragma unroll
+          for (int kb = 0; kb < NKB; ++kb) {
+#pragma unroll
+            for (int k = 0; k < 4; ++k) {
+              const uint64_t y  = ptx::desc(a0 + kb * (kDecTile >> 4) + k * 2, ptx::kDescHiSw128);
+              const uint32_t qd = q_lo0 + kb * (L::q_tile >> 4) + k * 2;
+              const uint64_t r  = ptx::desc(qd, ptx::kDescHiSw128);
+              if (kQM) ptx::wgmma_bf16<NQ>(d, r, y, (kb | k) != 0 ? 1u : 0u);
+              else ptx::wgmma_bf16<NQ>(d, y, r, (kb | k) != 0 ? 1u : 0u);
+              if (PASSES == 2) {
+                const uint64_t rl = ptx::desc(qd + NKB * (L::q_tile >> 4), ptx::kDescHiSw128);
+                if (kQM) ptx::wgmma_bf16<NQ>(d, rl, y, 1u);
+                else ptx::wgmma_bf16<NQ>(d, y, rl, 1u);
+              }
+            }
+          }
+          const uint64_t xd = ptx::desc(x_lo0 + ds * (L::dec_stage >> 4), ptx::kDescHiSw32), od = ptx::desc(ones_lo, ptx::kDescHiSw32);
+          if (kQM) ptx::wgmma_bf16<NQ>(d, od, xd, 1u);
+          else ptx::wgmma_bf16<NQ>(d, xd, od, 1u);
+          ptx::wgmma_commit();
+          ptx::wgmma_wait<0>();
+          __syncwarp();
+          if (lane == 0) {
+            ptx::mbar_arrive(&d_empty[ds]);
+            if (t + 1 == item.n_tiles) ptx::mbar_arrive(q_empty);
+          }
+          if (++ds == kDecStages) { ds = 0; dph ^= 1; }
+          // score = -accumulator, as the filtering epilogue reports it
+          if constexpr (kQM) {
+            // query rows q0, q0 + 8; list rows rb + 8j + {0, 1}: one float2 per lane, a quad writes 8 consecutive rows (32 B)
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+              const int q = q0 + 8 * h;
+              if (static_cast<uint32_t>(q) < item.valid_rows) {
+                float* o = out + q * seg + t * 128 + rb;
+#pragma unroll
+                for (int j = 0; j < NQ / 8; ++j)
+                  *reinterpret_cast<float2*>(o + 8 * j) = make_float2(-d[4 * j + 2 * h], -d[4 * j + 2 * h + 1]);
+              }
+            }
+          } else {
+            // list rows r0, r0 + 8; query columns 8j + 2 (lane % 4) + {0, 1}: the 8 lanes of one column write 8 consecutive rows
+#pragma unroll
+            for (int j = 0; j < NQ / 8; ++j)
+#pragma unroll
+              for (int e = 0; e < 4; ++e) {
+                const int col = 8 * j + 2 * (lane & 3) + (e & 1);
+                if (static_cast<uint32_t>(col) < item.valid_rows) out[col * seg + t * 128 + r0 + 8 * (e >> 1)] = -d[4 * j + e];
+              }
+          }
+        }
+        qph ^= 1;
+        continue;
+      }
       // per-column state: running threshold in t = -(score) units (a row is a candidate iff t > thr), empty buffer
       for (int col = te; col < NQ; col += kEpiThreads) {
         float thr = INFINITY;  // columns past the item's queries never collect anything
@@ -600,6 +668,8 @@ pq_stream_scan_kernel(const __grid_constant__ CUtensorMap tmQ_hi, const __grid_c
     }
   }
 }
+
+#pragma nv_diag_default 128
 
 // ------------------------------------------------------------------------------------ build-side kernels
 // one CTA per 128-row tile: codes [128, pq_dim] -> lane-transposed 16-byte chunks + half norms
@@ -706,13 +776,14 @@ int env_int(const char* name, int dflt)
   return v ? atoi(v) : dflt;
 }
 
-template <int NQ, int NKB, int PASSES>
+template <int NQ, int NKB, int PASSES, bool STORE = false>
 void launch(cudaStream_t stream, int sms, const CUtensorMap& mq_hi, const CUtensorMap& mq_lo, pq_args a, int n_items)
 {
   using L   = layout<NQ, NKB, PASSES>;
-  auto kern = pq_stream_scan_kernel<NQ, NKB, PASSES>;
+  auto kern = pq_stream_scan_kernel<NQ, NKB, PASSES, STORE>;
   a.cap     = a.KC <= 16 ? (NQ == 128 ? 32 : 64) : (a.KC <= 32 ? 64 : 128);  // free slots between compactions: cap - KC
   if (const int cap_env = env_int("CUVS_B200_PQ_CAP", 0)) a.cap = std::max(a.KC + 8, std::min(128, cap_env));  // bisection knob
+  if (STORE) a.cap = 0;  // no candidate buffers
   const int fixed = L::off_cand + NQ * a.cap * 8 + 1024 /*alignment slack of the dynamic segment*/;
   a.cstages = std::min(kMaxCStages, (kSmemLimit - fixed) / a.blk);
   const int forced = env_int("CUVS_B200_PQ_CSTAGES", 0);  // limiter experiments only
@@ -795,6 +866,7 @@ int pq_stream_group(double pairs_per_list, int KC, int passes)
   const int forced = env_int("CUVS_B200_PQ_GROUP", 0);  // tests and limiter experiments (read per call)
   int g = pairs_per_list <= 20.0 ? 32 : (pairs_per_list <= 80.0 ? 64 : 128);
   if (forced == 32 || forced == 64 || forced == 128) g = forced;
+  if (KC == 0) return g;                           // store epilogue: no candidate buffers, every width fits
   if ((KC > 16 || passes == 2) && g > 64) g = 64;  // shared-memory budget: wide candidate buffers / two residual planes
   if (KC > 32) g = 32;                             // 128-entry buffers (k in 33..64): 32 query columns per item
   return g;
@@ -807,9 +879,10 @@ void pq_stream_scan(cudaStream_t stream, int device, const __nv_bfloat16* q_hi, 
 {
   if (n_items == 0) return;
   B2_EXPECTS(Kp == 2 * pq_dim && (pq_dim == 32 || pq_dim == 64), "pq_stream_scan: pq_dim must be 32 or 64 with pq_len 2 (Kp=%d)", Kp);
-  B2_EXPECTS(KC == 16 || KC == 32 || KC == 64, "pq_stream_scan: KC must be 16, 32 or 64");
+  B2_EXPECTS(KC == 0 || KC == 16 || KC == 32 || KC == 64, "pq_stream_scan: KC must be 0 (store), 16, 32 or 64");
   B2_EXPECTS(passes == 1 || (passes == 2 && q_lo != nullptr), "pq_stream_scan: passes must be 1, or 2 with a lo plane");
-  B2_EXPECTS(group == 32 || (group == 64 && KC <= 32) || (group == 128 && KC == 16 && passes == 1), "pq_stream_scan: unsupported group %d", group);
+  B2_EXPECTS(group == 32 || (group == 64 && KC <= 32) || (group == 128 && (KC == 0 || (KC == 16 && passes == 1))),
+             "pq_stream_scan: unsupported group %d", group);
   B2_EXPECTS(a_rows >= group, "pq_stream_scan: the residual plane must hold at least one group of rows");
   pq_args a{};
   a.stream = code_stream;
@@ -819,7 +892,7 @@ void pq_stream_scan(cudaStream_t stream, int device, const __nv_bfloat16* q_hi, 
   a.out_score = out_score;
   a.out_pos = out_pos;
   a.out_row_stride = out_row_stride;
-  if (bound != nullptr && bound->keys != nullptr && !env_int("CUVS_B200_PQ_NO_BOUND", 0)) {
+  if (KC > 0 && bound != nullptr && bound->keys != nullptr && !env_int("CUVS_B200_PQ_NO_BOUND", 0)) {
     a.b_keys = bound->keys;
     a.b_idx = bound->idx;
     a.b_add = bound->add;
@@ -839,10 +912,15 @@ void pq_stream_scan(cudaStream_t stream, int device, const __nv_bfloat16* q_hi, 
   const int sms = sm_count_of(device);
   const int nkb = Kp / 64;
 #define B2_PQ_CASE(NQ_, NKB_, P_) \
-  if (group == NQ_ && nkb == NKB_ && passes == P_) return launch<NQ_, NKB_, P_>(stream, sms, mq, mql, a, n_items);
+  if (KC > 0 && group == NQ_ && nkb == NKB_ && passes == P_) return launch<NQ_, NKB_, P_>(stream, sms, mq, mql, a, n_items);
   B2_PQ_CASE(32, 1, 1) B2_PQ_CASE(64, 1, 1) B2_PQ_CASE(128, 1, 1) B2_PQ_CASE(32, 2, 1) B2_PQ_CASE(64, 2, 1) B2_PQ_CASE(128, 2, 1)
   B2_PQ_CASE(32, 1, 2) B2_PQ_CASE(64, 1, 2) B2_PQ_CASE(32, 2, 2) B2_PQ_CASE(64, 2, 2)
 #undef B2_PQ_CASE
+#define B2_PQ_STORE(NQ_, NKB_, P_) \
+  if (KC == 0 && group == NQ_ && nkb == NKB_ && passes == P_) return launch<NQ_, NKB_, P_, true>(stream, sms, mq, mql, a, n_items);
+  B2_PQ_STORE(32, 1, 1) B2_PQ_STORE(64, 1, 1) B2_PQ_STORE(128, 1, 1) B2_PQ_STORE(32, 2, 1) B2_PQ_STORE(64, 2, 1) B2_PQ_STORE(128, 2, 1)
+  B2_PQ_STORE(32, 1, 2) B2_PQ_STORE(64, 1, 2) B2_PQ_STORE(128, 1, 2) B2_PQ_STORE(32, 2, 2) B2_PQ_STORE(64, 2, 2) B2_PQ_STORE(128, 2, 2)
+#undef B2_PQ_STORE
   B2_FAIL("pq_stream_scan: no kernel for group=%d Kp=%d passes=%d", group, Kp, passes);
 }
 

@@ -43,7 +43,8 @@ void pq_stream_build(cudaStream_t s, const uint8_t* codes, const int64_t* ids, i
 /** The flat form back from the stream: codes [rows_total, pq_dim], one code per byte (getters, extend, serialize, LUT path). */
 void pq_stream_to_flat(cudaStream_t s, const uint8_t* stream, int64_t rows_total, int pq_dim, uint8_t* codes);
 
-/** Queries per work item the scan wants for an average of `pairs_per_list` probing queries per list (32, 64 or 128). */
+/** Queries per work item the scan wants for an average of `pairs_per_list` probing queries per list (32, 64 or 128);
+ *  KC = 0 (store epilogue) is not limited by candidate buffers. */
 int pq_stream_group(double pairs_per_list, int KC, int passes);
 
 /**
@@ -51,6 +52,8 @@ int pq_stream_group(double pairs_per_list, int KC, int passes);
  * A rows = per-(query, probe) residual rows [a_rows, Kp] bf16 (q_lo: second plane for passes == 2, else null), B = the code
  * stream.  For every item and valid A row the kernel writes KC (score, position) candidates (unsorted, empty slots
  * (+inf, 0xffffffff)) at out_off + row * out_row_stride; score = hn - r.y as in tc_scan_topk; `bound` as in tc_scan_topk.
+ * KC = 0 is the store epilogue (k > 64): the score of every list row goes to out_score[out_off + row * n_tiles * 128 + j],
+ * j = row of the item's list (padding rows +inf); out_pos, out_row_stride and `bound` are unused, any group is accepted.
  */
 void pq_stream_scan(cudaStream_t stream, int device, const __nv_bfloat16* q_hi, const __nv_bfloat16* q_lo, int64_t a_rows, int Kp,
                     const uint8_t* code_stream, const uint32_t* cb_words, int pq_dim, const tc_item* items_dev, int n_items,

@@ -44,10 +44,20 @@ __device__ __forceinline__ int32_t all_ones<int32_t>()
   return -1;
 }
 
-constexpr int kMaxK = 2048;
+constexpr int kMaxK = kSelectMaxK;
 
-// smem: hist[256] | scalars[8] | warp_tot[32] | skeys[kpow2] (u64)
-template <typename IdxIn, typename IdxOut, bool HasIdx>
+// Rows given as segments of one array (CSR): row r is in_val[off[r] .. off[r] + len[r]), and the position reported for its
+// column c is base[r] + c.  `stage`: segments up to this many floats are first copied into shared memory, so the four radix
+// passes, the gathers and the read-out read global memory once.
+struct seg_rows {
+  const int64_t* off   = nullptr;
+  const uint32_t* len  = nullptr;
+  const uint32_t* base = nullptr;
+  int stage            = 0;
+};
+
+// smem: hist[256] | scalars[8] | warp_tot[32] | skeys[kpow2] (u64) | (Seg) staged segment [seg.stage] (f32)
+template <typename IdxIn, typename IdxOut, bool HasIdx, bool Seg = false>
 __global__ void __launch_bounds__(1024) select_k_kernel(const float* __restrict__ in_val,
                                                           const IdxIn* __restrict__ in_idx,
                                                           int64_t len,
@@ -56,7 +66,8 @@ __global__ void __launch_bounds__(1024) select_k_kernel(const float* __restrict_
                                                           int kpow2,
                                                           float* __restrict__ out_val,
                                                           IdxOut* __restrict__ out_idx,
-                                                          bool select_min)
+                                                          bool select_min,
+                                                          seg_rows seg = seg_rows{})
 {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   uint32_t* hist     = reinterpret_cast<uint32_t*>(smem_raw);
@@ -68,6 +79,15 @@ __global__ void __launch_bounds__(1024) select_k_kernel(const float* __restrict_
   const float* v    = in_val + row * in_ld;
   const int tid     = threadIdx.x;
   const int bs      = blockDim.x;
+  if constexpr (Seg) {
+    v   = in_val + seg.off[row];
+    len = seg.len[row];
+    if (len <= seg.stage) {
+      float* st = reinterpret_cast<float*>(skeys + kpow2);
+      for (int64_t i = tid; i < len; i += bs) st[i] = v[i];
+      v = st;  // (made visible by the barrier below)
+    }
+  }
   const int k_eff   = len < k ? static_cast<int>(len) : k;
 
   for (int i = tid; i < kpow2; i += bs) skeys[i] = ~0ull;
@@ -183,6 +203,8 @@ __global__ void __launch_bounds__(1024) select_k_kernel(const float* __restrict_
       ov           = v[pos];
       if constexpr (HasIdx) {
         oi = static_cast<IdxOut>(in_idx[row * in_ld + pos]);
+      } else if constexpr (Seg) {
+        oi = static_cast<IdxOut>(seg.base[row] + pos);
       } else {
         oi = static_cast<IdxOut>(pos);
       }
@@ -436,6 +458,35 @@ void select_k(cudaStream_t stream, const float* in_val, const void* in_idx, idx_
   if (in_kind == IDX_U32 && out_kind == IDX_I64) return launch<uint32_t, int64_t, true>(stream, in_val, in_idx, batch, len, in_ld, k, out_val, out_idx, select_min);
   if (in_kind == IDX_I32 && out_kind == IDX_I32) return launch<int32_t, int32_t, true>(stream, in_val, in_idx, batch, len, in_ld, k, out_val, out_idx, select_min);
   B2_FAIL("select_k: unsupported index dtype combination (%d -> %d)", int(in_kind), int(out_kind));
+}
+
+void select_k_segments(cudaStream_t stream, const float* in_val, const int64_t* seg_off, const uint32_t* seg_len,
+                       const uint32_t* pos_base, int64_t batch, int64_t max_len, int k, float* out_val, uint32_t* out_pos,
+                       bool select_min)
+{
+  B2_EXPECTS(k >= 1 && k <= kMaxK, "select_k: k must be in [1, %d] (got %d)", kMaxK, k);
+  B2_EXPECTS(max_len >= 0 && max_len < (int64_t(1) << 32), "select_k: segment length out of range");
+  B2_EXPECTS(batch < (int64_t(1) << 31), "select_k: batch too large");
+  if (batch == 0) return;
+  int kpow2 = 1;
+  while (kpow2 < k) kpow2 <<= 1;
+  if (kpow2 < 2) kpow2 = 2;
+  int threads = max_len <= 2048 ? 128 : (max_len <= 32768 ? 256 : 1024);
+  if (kpow2 / 2 > threads && threads < 1024) threads = kpow2 / 2 > 1024 ? 1024 : kpow2 / 2;
+  const size_t base = (256 + 8 + 32) * sizeof(uint32_t) + static_cast<size_t>(kpow2) * sizeof(uint64_t);
+  seg_rows seg;
+  seg.off  = seg_off;
+  seg.len  = seg_len;
+  seg.base = pos_base;
+  // stage segments of up to 96 KiB (24k rows, two CTAs per SM); a longer segment is read from global memory in every pass
+  seg.stage = max_len * sizeof(float) <= (96u << 10) ? static_cast<int>(max_len) : 0;
+  const size_t smem = base + static_cast<size_t>(seg.stage) * sizeof(float);
+  auto kern         = select_k_kernel<uint32_t, uint32_t, false, true>;
+  B2_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
+  count_launch();
+  timed_section ts("select_k_segments", stream);
+  kern<<<static_cast<unsigned>(batch), threads, smem, stream>>>(in_val, nullptr, 0, 0, k, kpow2, out_val, out_pos, select_min, seg);
+  B2_CUDA(cudaGetLastError());
 }
 
 void knn_merge_parts(cudaStream_t stream, const float* in_keys, const int64_t* in_vals, float* out_keys,

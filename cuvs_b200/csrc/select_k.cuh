@@ -21,6 +21,18 @@ enum idx_kind : int { IDX_NONE = 0, IDX_I64 = 1, IDX_U32 = 2, IDX_I32 = 3 };
 void select_k(cudaStream_t stream, const float* in_val, const void* in_idx, idx_kind in_kind, int64_t batch,
               int64_t len, int64_t in_ld, int k, float* out_val, void* out_idx, idx_kind out_kind, bool select_min);
 
+/** Largest k of select_k and select_k_segments. */
+constexpr int kSelectMaxK = 2048;
+
+/**
+ * select_k over rows that are segments of one array: row r is in_val[seg_off[r] .. seg_off[r] + seg_len[r]) (device arrays,
+ * seg_len[r] <= max_len), and its column c is reported as position pos_base[r] + c.  Same order, tie rule and padding as
+ * select_k; out_* are [batch, k].
+ */
+void select_k_segments(cudaStream_t stream, const float* in_val, const int64_t* seg_off, const uint32_t* seg_len,
+                       const uint32_t* pos_base, int64_t batch, int64_t max_len, int k, float* out_val, uint32_t* out_pos,
+                       bool select_min);
+
 /**
  * Merge per-part top-k lists: in_* are [n_parts * n_rows, k] (part-major), out_* [n_rows, k].
  * `translations` (device int64[n_parts] or null) is added to the ids of each part.
