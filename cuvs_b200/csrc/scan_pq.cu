@@ -14,15 +14,17 @@
 //                          shared load; codebook words sit at [half][code][lane] (bank == lane), so a row's 64 entries are
 //                          fetched with two conflict-free LDS.32 per lane and written with two STS.32 into the 128-byte-
 //                          swizzled K-major operand tile (bf16 row = 256 B).
-//   warps 12-19 MMA +      two warpgroups.  NQ = 64 / 128: the queries are the MMA's M side, D[64 queries x 64 rows] (+)=
-//               epilogue   R . Y_half^T per 64-row half of the tile (NQ = 64), or D[64 queries x 128 rows] (+)= R_half . Y^T
-//                          per 64-query half of the item (NQ = 128), on wgmma m64nNQk16 (8 K-steps + 1 that adds -|y|^2/2:
-//                          ones x three bf16 pieces); a thread's fragment is 2 query rows x NQ / 4 list rows, so each query
-//                          row is tested with one max against one threshold and its hits reserve their buffer slots with one
-//                          atomic.  NQ = 32 (m64 would be half empty): the rows are the M side, D[64 rows x 32 queries] per
-//                          half, and each element is tested against its own query's threshold.  Hits go into per-query
-//                          candidate buffers; a buffer that overflows is compacted to its KC best by one warp (rank by
-//                          counting) and the threshold tightened; one named barrier per tile.
+//   warps 12-19 MMA +      two warpgroups.  NQ = 64 / 128: the queries are the MMA's M side.  NQ = 64, one pass: the
+//               epilogue   warpgroups take whole tiles in turn (ping-pong), D[64 queries x 128 rows] (+)= R . Y^T; NQ = 64,
+//                          two passes: D[64 queries x 64 rows] (+)= R . Y_half^T per 64-row half of the tile; NQ = 128:
+//                          D[64 queries x 128 rows] (+)= R_half . Y^T per 64-query half of the item (wgmma, 8 K-steps + 1 that
+//                          adds -|y|^2/2: ones x three bf16 pieces); a thread's fragment is 2 query rows x 16 | 32 list rows,
+//                          so each query row is tested with one max against one threshold and its hits reserve their buffer
+//                          slots with one atomic.  NQ = 32 (m64 would be half empty): the rows are the M side, D[64 rows x
+//                          32 queries] per half, and each element is tested against its own query's threshold.  Hits go
+//                          into per-query candidate buffers; a buffer that overflows is compacted to its KC best by one
+//                          warp (rank by counting) and the threshold tightened; one named barrier per tile (ping-pong: per
+//                          tile of the warpgroup, over its own buffers).
 //
 // With few probing queries per list (50M rows / 8192 lists / 10k-query batches at 48 probes: ~59) the accumulator is 128 x 32..64
 // instead of the 128 x 128 of the query-major kernel (scan_tc.cu), and HBM traffic per row is pq_dim + 4 bytes instead of a
@@ -171,20 +173,19 @@ __device__ __forceinline__ uint64_t pq_filter_frag(const float (&d)[NQ / 2], uin
   return left;
 }
 
-// Queries-on-M fragment (NQ = 64 / 128; see ptx::wgmma_bf16: query rows q0 and q0 + 8, list rows 8j + 2 * (lane % 4) + {0, 1}
-// of the warpgroup's N side) against the two query rows' running thresholds.  Element k < NQ / 4 of query row q0 + 8h is
-// d[4 * (k / 2) + 2h + k % 2], list row pos0 + 8 * (k / 2) + k % 2; bit 32h + k of `only` and of the result stands for it.
-// A query row is tested with one max over its elements against one threshold (a candidate iff > threshold); a row with hits
-// reserves all its buffer slots with one atomic and then stores one hit per pass (constant register indices only: the
-// fragment stays in registers).  Returns the elements whose candidate could not be stored (buffer full).
-template <int NQ>
-__device__ __forceinline__ uint64_t pq_filter_rows(const float (&d)[NQ / 2], uint64_t only, int q0, uint32_t pos0,
-                                                   const float* __restrict__ thr, int* cnt, unsigned long long* cand, int cap)
+// Queries-on-M fragment (MMA N = 64 / 128 list rows; see ptx::wgmma_bf16: query rows q0 and q0 + 8, list rows
+// 8j + 2 * (lane % 4) + {0, 1} of the warpgroup's N side) against the two query rows' thresholds th[0], th[1].  Element
+// k < N / 4 of query row q0 + 8h is d[4 * (k / 2) + 2h + k % 2], list row pos0 + 8 * (k / 2) + k % 2; bit 32h + k of `only` and
+// of the result stands for it.  A query row is tested with one max over its elements against one threshold (a candidate iff
+// > threshold); a row with hits reserves all its buffer slots with one atomic and then stores one hit per pass (constant
+// register indices only: the fragment stays in registers).  Returns the elements whose candidate could not be stored (buffer
+// full).
+template <int N>
+__device__ __forceinline__ uint64_t pq_filter_rows(const float (&d)[N / 2], uint64_t only, int q0, uint32_t pos0,
+                                                   const float (&th)[2], int* cnt, unsigned long long* cand, int cap)
 {
-  constexpr int NE = NQ / 4;
+  constexpr int NE = N / 4;
   uint64_t left    = 0;
-  // (thresholds change only in compaction, between the per-tile barriers: read once per filter pass)
-  const float th[2] = {thr[q0], thr[q0 + 8]};
   // four interleaved max chains per query row: short dependence chains, and few registers beside the fragment
   float mx[2];
 #pragma unroll
@@ -230,18 +231,26 @@ __device__ __forceinline__ uint64_t pq_filter_rows(const float (&d)[NQ / 2], uin
 
 // Selection inside one column's buffer by one warp, rank by counting: lane l holds entries l, l + 32, l + 64, l + 96 (64-bit keys
 // order(t) << 32 | ~pos, unique, 0 = none; n <= 128); every entry is broadcast from shared memory and each lane counts how
-// many beat its own.  rank 0 = best.  No dependent chain: n iterations of one LDS.64 + four compare-adds.
-__device__ __forceinline__ void pq_rank_select(const unsigned long long* buf, int n, int lane, unsigned long long (&k)[4], int (&r)[4])
+// many beat its own.  rank 0 = best.  No dependent chain: n iterations of one LDS.64 + four compare-adds.  The entries are
+// buf[0 .. n) followed by buf2[0 .. n2) (the two warpgroups' buffers of one column at NQ = 64 / one pass; n2 = 0 otherwise).
+__device__ __forceinline__ void pq_rank_select(const unsigned long long* buf, int n, const unsigned long long* buf2, int n2, int lane,
+                                               unsigned long long (&k)[4], int (&r)[4])
 {
 #pragma unroll
   for (int e = 0; e < 4; ++e) {
-    k[e] = lane + 32 * e < n ? buf[lane + 32 * e] : 0ull;
-    r[e] = 0;
+    const int i = lane + 32 * e;
+    k[e]        = i < n ? buf[i] : (i < n + n2 ? buf2[i - n] : 0ull);
+    r[e]        = 0;
   }
-  if (n <= 64) {  // (warp-uniform) the common case: buffers of <= 64 entries
+  if (n + n2 <= 64) {  // (warp-uniform) the common case: buffers of <= 64 entries
 #pragma unroll 4
     for (int i = 0; i < n; ++i) {
       const unsigned long long ki = buf[i];
+      r[0] += ki > k[0] ? 1 : 0;
+      r[1] += ki > k[1] ? 1 : 0;
+    }
+    for (int i = 0; i < n2; ++i) {
+      const unsigned long long ki = buf2[i];
       r[0] += ki > k[0] ? 1 : 0;
       r[1] += ki > k[1] ? 1 : 0;
     }
@@ -252,11 +261,22 @@ __device__ __forceinline__ void pq_rank_select(const unsigned long long* buf, in
 #pragma unroll
       for (int e = 0; e < 4; ++e) r[e] += ki > k[e] ? 1 : 0;
     }
+    for (int i = 0; i < n2; ++i) {
+      const unsigned long long ki = buf2[i];
+#pragma unroll
+      for (int e = 0; e < 4; ++e) r[e] += ki > k[e] ? 1 : 0;
+    }
   }
 }
 
+// Ping-pong consumers (NQ = 64, one pass): each warpgroup owns whole tiles, alternately, and keeps its own thresholds,
+// counters and candidate buffers.  With two residual planes (PASSES = 2) two buffer sets leave fewer than two code stages in
+// shared memory at pq_dim 64 and KC = 32, so the two-pass consumers keep both warpgroups on every tile (one 64-row half each).
+constexpr bool pq_pingpong(int NQ, int PASSES) { return NQ == 64 && PASSES == 1; }
+
 template <int NQ, int NKB, int PASSES>
 struct layout {
+  static constexpr int n_sets     = pq_pingpong(NQ, PASSES) ? 2 : 1;  // per-warpgroup threshold / counter / buffer sets
   static constexpr int q_tile     = NQ * 128;                       // one k-block of the residual rows
   static constexpr int q_bytes    = PASSES * NKB * q_tile;
   static constexpr int dec_stage  = NKB * kDecTile + kExtTile;
@@ -267,11 +287,11 @@ struct layout {
   static constexpr int off_ones   = off_dec + kDecStages * dec_stage;
   static constexpr int off_cb     = off_ones + ones_bytes;
   static constexpr int off_thr    = off_cb + cb_bytes;
-  static constexpr int off_cnt    = off_thr + NQ * 4;
-  static constexpr int off_bars   = off_cnt + NQ * 4;
+  static constexpr int off_cnt    = off_thr + n_sets * NQ * 4;
+  static constexpr int off_bars   = off_cnt + n_sets * NQ * 4;
   static constexpr int n_bars     = 2 * kMaxCStages + 2 * kDecStages + 2 + 2 * kSched;
   static constexpr int off_item   = off_bars + n_bars * 8;
-  static constexpr int off_cand   = (off_item + kSched * 4 + 15) / 16 * 16;   // [NQ][cap] uint2, then the code ring
+  static constexpr int off_cand   = (off_item + kSched * 4 + 15) / 16 * 16;   // [n_sets][NQ][cap] uint2, then the code ring
   static_assert(q_tile % 1024 == 0 && dec_stage % 1024 == 0, "operand tiles need 1024-byte alignment");
 };
 
@@ -285,6 +305,8 @@ __global__ void __launch_bounds__(kThreads, 1)
 pq_stream_scan_kernel(const __grid_constant__ CUtensorMap tmQ_hi, const __grid_constant__ CUtensorMap tmQ_lo, const pq_args P)
 {
   using L = layout<NQ, NKB, PASSES>;
+  constexpr bool kPP = pq_pingpong(NQ, PASSES) && !STORE;
+  static_assert(!kPP || kDecStages == 2, "ping-pong: warpgroup w owns decode stage w and flips its phase once per owned tile");
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   if (threadIdx.x == 0 && (ptx::smem_u32(smem_raw) & 1023u) != 0) __trap();
   uint8_t* sQ     = smem_raw + L::off_q;
@@ -304,7 +326,7 @@ pq_stream_scan_kernel(const __grid_constant__ CUtensorMap tmQ_hi, const __grid_c
   uint64_t* s_empty = s_full + kSched;
   int* s_item       = reinterpret_cast<int*>(smem_raw + L::off_item);
   unsigned long long* sCand = reinterpret_cast<unsigned long long*>(smem_raw + L::off_cand);  // okey(t) << 32 | ~pos
-  uint8_t* sCode  = smem_raw + L::off_cand + NQ * P.cap * 8;
+  uint8_t* sCode  = smem_raw + L::off_cand + L::n_sets * NQ * P.cap * 8;
 
   const int warp = __shfl_sync(0xffffffffu, static_cast<int>(threadIdx.x >> 5), 0), lane = threadIdx.x & 31;
   const int n_items = P.n_items_dev ? *P.n_items_dev : P.n_items_host;
@@ -321,7 +343,7 @@ pq_stream_scan_kernel(const __grid_constant__ CUtensorMap tmQ_hi, const __grid_c
     }
     for (int s = 0; s < kDecStages; ++s) {
       ptx::mbar_init(&d_full[s], kDecWarps);
-      ptx::mbar_init(&d_empty[s], kEpiWarps);
+      ptx::mbar_init(&d_empty[s], kPP ? kEpiWarps / 2 : kEpiWarps);  // ping-pong: stage s is warpgroup s's
     }
     ptx::mbar_init(q_full, 1);
     ptx::mbar_init(q_empty, kEpiWarps);
@@ -460,46 +482,56 @@ pq_stream_scan_kernel(const __grid_constant__ CUtensorMap tmQ_hi, const __grid_c
   } else {
     ptx::setmaxnreg_inc<136>();  // 40 + 2 x 80 + 2 x 136 <= 5 x 96: only registers the other warpgroups gave back
     // ------------------------------------------------------------------ MMA + epilogue: two warpgroups
-    // NQ = 64: one per 64-row half of the tile, D[64 queries x 64 rows] (+)= R . Y_half^T; NQ = 128: one per 64-query half of
-    // the item, D[64 queries x 128 rows] (+)= R_half . Y^T; NQ = 32: one per 64-row half, D[64 rows x 32 queries] (+)=
-    // Y_half . R^T.  wgmma: 8 K-steps + 1 that adds -|y|^2/2.  Then the fragment is tested against the running thresholds
-    // (shared memory); the hits go into per-query candidate buffers; a buffer that overflows is compacted to its KC best
-    // by one warp (rank by counting) and the threshold tightened, and the elements that did not fit are re-tested from the
-    // registers.
-    constexpr bool kQM = NQ >= 64;                                   // queries on the MMA's M side
+    // NQ = 64, one pass (ping-pong, kPP): warpgroup w owns every tile g (counted across items, as the decode ring counts) with
+    // g % 2 == w, i.e. decode stage w, and computes D[64 queries x 128 rows] (+)= R . Y^T over the whole tile, so one
+    // warpgroup's MMAs run while the other filters.  NQ = 64, two passes: one per 64-row half of the tile, D[64 queries x 64
+    // rows] (+)= R . Y_half^T; NQ = 128: one per 64-query half of the item, D[64 queries x 128 rows] (+)= R_half . Y^T; NQ = 32:
+    // one per 64-row half, D[64 rows x 32 queries] (+)= Y_half . R^T.  wgmma: 8 K-steps + 1 that adds -|y|^2/2.  Then the
+    // fragment is tested against the running thresholds (shared memory); the hits go into per-query candidate buffers; a
+    // buffer that overflows is compacted to its KC best by one warp (rank by counting) and the threshold tightened, and the
+    // elements that did not fit are re-tested from the registers.
+    constexpr bool kQM    = NQ >= 64;                              // queries on the MMA's M side
+    constexpr bool kWhole = NQ == 128 || kPP;                      // each MMA covers all 128 rows of the tile
+    constexpr int MN      = kPP ? 128 : NQ;                        // the MMA's N width
     const int ew = warp - kEpiWarp0;                                 // 0..7
     const int wg = ew >> 2;
     const int te = static_cast<int>(threadIdx.x) - 32 * kEpiWarp0;  // 0..255
     // rows-on-M: fragment rows r0 and r0 + 8 of the tile; queries-on-M: query rows q0 and q0 + 8, list rows from rb on
     const int r0 = 64 * wg + 16 * (ew & 3) + (lane >> 2);
     const int q0 = (NQ == 128 ? 64 * wg : 0) + 16 * (ew & 3) + (lane >> 2);
-    const int rb = (NQ == 128 ? 0 : 64 * wg) + 2 * (lane & 3);
+    const int rb = (kWhole ? 0 : 64 * wg) + 2 * (lane & 3);
     const uint32_t q_lo0   = ptx::smem_desc_lo(ptx::smem_u32(sQ)) + (NQ == 128 ? wg * 512 : 0);  // + 64 rows of 128 B
-    const uint32_t d_lo0   = ptx::smem_desc_lo(ptx::smem_u32(sDec)) + (NQ == 128 ? 0 : wg * 512);
-    const uint32_t x_lo0   = ptx::smem_desc_lo(ptx::smem_u32(sDec + NKB * kDecTile)) + (NQ == 128 ? 0 : wg * 128);  // 32 B rows
+    const uint32_t d_lo0   = ptx::smem_desc_lo(ptx::smem_u32(sDec)) + (kWhole ? 0 : wg * 512);
+    const uint32_t x_lo0   = ptx::smem_desc_lo(ptx::smem_u32(sDec + NKB * kDecTile)) + (kWhole ? 0 : wg * 128);  // 32 B rows
     const uint32_t ones_lo = ptx::smem_desc_lo(ptx::smem_u32(sOnes));
     const int cap = P.cap, KC = P.KC;
     const int kth = (P.kth > 0 && P.kth < KC) ? P.kth : KC;
-    uint32_t ds = 0, dph = 0, qph = 0, ss = 0, sp = 0;
+    // this warpgroup's threshold / counter / buffer set (ping-pong: one per warpgroup) and the other warpgroup's thresholds
+    float* thr_w = sThr + (kPP ? wg * NQ : 0);
+    const float* thr_x = sThr + (kPP ? (wg ^ 1) * NQ : 0);
+    int* cnt_w = sCnt + (kPP ? wg * NQ : 0);
+    unsigned long long* cand_w = sCand + (kPP ? wg * NQ * cap : 0);
+    // the barrier of the overflow loop and the warps that compact: the warpgroup's own (ping-pong), or both warpgroups.
+    // (A run-time barrier id makes ptxas reserve all 16 named barriers, which is harmless at one CTA per SM.)
+    const uint32_t bar_id = kPP ? 2 + wg : 1, bar_n = kPP ? 128 : kEpiThreads;
+    const int cw0 = kPP ? (ew & 3) : ew, cwn = kPP ? 4 : kEpiWarps;
+    uint32_t ds = kPP ? wg : 0, dph = 0, qph = 0, ss = 0, sp = 0;
+    uint32_t g0 = 0;  // ping-pong: running tile number of the item's first tile
 
-    auto rank_select = [&](int col, unsigned long long (&k)[4], int (&r)[4]) -> int {
-      const int n = min(sCnt[col], cap);
-      pq_rank_select(sCand + col * cap, n, lane, k, r);
-      return n;
-    };
     // compaction: keep the KC best at the front, tighten the column's threshold to its kth best
     auto compact = [&](int col) {
       unsigned long long k[4];
       int r[4];
-      const int n = rank_select(col, k, r);
+      unsigned long long* buf = cand_w + col * cap;
+      const int n = min(cnt_w[col], cap);
+      pq_rank_select(buf, n, nullptr, 0, lane, k, r);
       __syncwarp();
-      unsigned long long* buf = sCand + col * cap;
 #pragma unroll
       for (int e = 0; e < 4; ++e) {
         if (k[e] != 0ull && r[e] < KC) buf[r[e]] = k[e];
-        if (n >= kth && k[e] != 0ull && r[e] == kth - 1) sThr[col] = fmaxf(sThr[col], __uint_as_float(okey_inv(static_cast<uint32_t>(k[e] >> 32))));
+        if (n >= kth && k[e] != 0ull && r[e] == kth - 1) thr_w[col] = fmaxf(thr_w[col], __uint_as_float(okey_inv(static_cast<uint32_t>(k[e] >> 32))));
       }
-      if (lane == 0) sCnt[col] = min(n, KC);
+      if (lane == 0) cnt_w[col] = min(n, KC);
       __syncwarp();
     };
 
@@ -573,9 +605,11 @@ pq_stream_scan_kernel(const __grid_constant__ CUtensorMap tmQ_hi, const __grid_c
         qph ^= 1;
         continue;
       }
-      // per-column state: running threshold in t = -(score) units (a row is a candidate iff t > thr), empty buffer
-      for (int col = te; col < NQ; col += kEpiThreads) {
-        float thr = INFINITY;  // columns past the item's queries never collect anything
+      // per-column state: running threshold in t = -(score) units (a row is a candidate iff t > thr), empty buffer; one set
+      // per warpgroup in ping-pong
+      for (int i = te; i < L::n_sets * NQ; i += kEpiThreads) {
+        const int col = i % NQ;
+        float thr     = INFINITY;  // columns past the item's queries never collect anything
         if (static_cast<uint32_t>(col) < item.valid_rows) {
           thr = -INFINITY;
           if (P.b_keys != nullptr) {
@@ -585,15 +619,18 @@ pq_stream_scan_kernel(const __grid_constant__ CUtensorMap tmQ_hi, const __grid_c
             thr                 = -((bv - (P.b_add ? P.b_add[arow] : 0.f)) / P.b_scale);
           }
         }
-        sThr[col] = thr;
-        sCnt[col] = 0;
+        sThr[i] = thr;
+        sCnt[i] = 0;
       }
       ptx::named_bar_sync(1, kEpiThreads);
       wait_dbg(P.dbg, q_full, qph, 0x202, static_cast<uint32_t>(it), 0);
 
-      for (uint32_t t = 0; t < item.n_tiles; ++t) {
+      // ping-pong: this warpgroup's tiles of the item are t0, t0 + 2, ...; it may have none (an item of one tile)
+      const uint32_t t0 = kPP ? (wg ^ (g0 & 1u)) : 0, tstep = kPP ? 2 : 1;
+      if (kPP && t0 >= item.n_tiles && lane == 0) ptx::mbar_arrive(q_empty);
+      for (uint32_t t = t0; t < item.n_tiles; t += tstep) {
         wait_dbg(P.dbg, &d_full[ds], dph, 0x204, static_cast<uint32_t>(it), t);
-        float d[NQ / 2];
+        float d[MN / 2];
         ptx::wgmma_fence();
         const uint32_t a0 = d_lo0 + ds * (L::dec_stage >> 4);
 #pragma unroll
@@ -603,49 +640,72 @@ pq_stream_scan_kernel(const __grid_constant__ CUtensorMap tmQ_hi, const __grid_c
             const uint64_t y  = ptx::desc(a0 + kb * (kDecTile >> 4) + k * 2, ptx::kDescHiSw128);  // decoded rows
             const uint32_t qd = q_lo0 + kb * (L::q_tile >> 4) + k * 2;                          // residual rows
             const uint64_t r  = ptx::desc(qd, ptx::kDescHiSw128);
-            if (kQM) ptx::wgmma_bf16<NQ>(d, r, y, (kb | k) != 0 ? 1u : 0u);
-            else ptx::wgmma_bf16<NQ>(d, y, r, (kb | k) != 0 ? 1u : 0u);
+            if (kQM) ptx::wgmma_bf16<MN>(d, r, y, (kb | k) != 0 ? 1u : 0u);
+            else ptx::wgmma_bf16<MN>(d, y, r, (kb | k) != 0 ? 1u : 0u);
             if (PASSES == 2) {
               const uint64_t rl = ptx::desc(qd + NKB * (L::q_tile >> 4), ptx::kDescHiSw128);
-              if (kQM) ptx::wgmma_bf16<NQ>(d, rl, y, 1u);
-              else ptx::wgmma_bf16<NQ>(d, y, rl, 1u);
+              if (kQM) ptx::wgmma_bf16<MN>(d, rl, y, 1u);
+              else ptx::wgmma_bf16<MN>(d, y, rl, 1u);
             }
           }
         }
         // -= |y|^2/2 : ext rows hold the three bf16 pieces of -hn/2 in both chunks, ones rows three 1s in both chunks
         const uint64_t xd = ptx::desc(x_lo0 + ds * (L::dec_stage >> 4), ptx::kDescHiSw32), od = ptx::desc(ones_lo, ptx::kDescHiSw32);
-        if (kQM) ptx::wgmma_bf16<NQ>(d, od, xd, 1u);
-        else ptx::wgmma_bf16<NQ>(d, xd, od, 1u);
+        if (kQM) ptx::wgmma_bf16<MN>(d, od, xd, 1u);
+        else ptx::wgmma_bf16<MN>(d, xd, od, 1u);
         ptx::wgmma_commit();
         ptx::wgmma_wait<0>();
         __syncwarp();
         if (lane == 0) {
           ptx::mbar_arrive(&d_empty[ds]);
-          if (t + 1 == item.n_tiles) ptx::mbar_arrive(q_empty);  // the item's residual rows may be replaced
+          if (t + tstep >= item.n_tiles) ptx::mbar_arrive(q_empty);  // the item's residual rows may be replaced
         }
-        if (++ds == kDecStages) { ds = 0; dph ^= 1; }
+        if (kPP) dph ^= 1;  // (the warpgroup's own stage)
+        else if (++ds == kDecStages) { ds = 0; dph ^= 1; }
 
         const uint32_t pos0 = item.b_row0 + t * 128 + (kQM ? rb : r0);
         auto filter = [&](uint64_t only) -> uint64_t {
-          if constexpr (kQM) return pq_filter_rows<NQ>(d, only, q0, pos0, sThr, sCnt, sCand, cap);
-          else return pq_filter_frag<NQ>(d, only, lane, pos0, pos0 + 8, sThr, sCnt, sCand, cap);
+          if constexpr (kQM) {
+            // (a warpgroup's thresholds change only in its own compaction, between its overflow barriers: read once per pass)
+            float th[2] = {thr_w[q0], thr_w[q0 + 8]};
+            if constexpr (kPP) {
+              // The other warpgroup's buffer may hold rows of LATER tiles, which lose exact ties to this tile's rows: against
+              // its threshold a row is kept iff t >= thr_x, not t > thr_x.  (Its own buffer holds only earlier rows, which
+              // win ties, so t > thr_w is exact.)  thr_x can rise while this runs: a stale value only keeps more rows.
+#pragma unroll
+              for (int h = 0; h < 2; ++h) {
+                const float tx = thr_x[q0 + 8 * h];
+                if (tx > th[h]) th[h] = nextafterf(tx, -INFINITY);
+              }
+            }
+            return pq_filter_rows<MN>(d, only, q0, pos0, th, cnt_w, cand_w, cap);
+          } else {
+            return pq_filter_frag<NQ>(d, only, lane, pos0, pos0 + 8, sThr, sCnt, sCand, cap);
+          }
         };
         uint64_t left = filter(~0ull);
-        // ONE barrier per tile decides whether any buffer overflowed
-        while (bar_red_or(1, kEpiThreads, left != 0)) {
-          for (int col = ew; col < NQ; col += kEpiWarps)
-            if (sCnt[col] > cap) compact(col);  // (warp-uniform: every lane reads the same counter)
-          ptx::named_bar_sync(1, kEpiThreads);
+        // ONE barrier per tile (of the warpgroup in ping-pong, else of both) decides whether any buffer overflowed
+        while (bar_red_or(bar_id, bar_n, left != 0)) {
+          for (int col = cw0; col < NQ; col += cwn)
+            if (cnt_w[col] > cap) compact(col);  // (warp-uniform: every lane reads the same counter)
+          ptx::named_bar_sync(bar_id, bar_n);
           if (left != 0) left = filter(left);
         }
       }
       qph ^= 1;
+      if constexpr (kPP) {
+        g0 += item.n_tiles;
+        // both warpgroups' buffers are final; the read-out ranks their union (<= 2 cap <= 128 entries, see launch())
+        ptx::named_bar_sync(1, kEpiThreads);
+      }
 
       // item done: every column's KC best -> global; publish the query's k-th best for the other items of the same query
       for (int col = ew; col < static_cast<int>(min(item.valid_rows, static_cast<uint32_t>(NQ))); col += kEpiWarps) {
         unsigned long long k[4];
         int r[4];
-        const int n  = rank_select(col, k, r);
+        const int n0 = min(sCnt[col], cap), n1 = kPP ? min(sCnt[NQ + col], cap) : 0;  // (ping-pong: the union of both sets)
+        pq_rank_select(sCand + col * cap, n0, sCand + (NQ + col) * cap, n1, lane, k, r);
+        const int n  = n0 + n1;
         const int nk = min(n, KC);
         const uint32_t arow = item.a_row0 + col;
         const int64_t o     = static_cast<int64_t>(item.out_off) + static_cast<int64_t>(col) * P.out_row_stride;
@@ -781,10 +841,12 @@ void launch(cudaStream_t stream, int sms, const CUtensorMap& mq_hi, const CUtens
 {
   using L   = layout<NQ, NKB, PASSES>;
   auto kern = pq_stream_scan_kernel<NQ, NKB, PASSES, STORE>;
-  a.cap     = a.KC <= 16 ? (NQ == 128 ? 32 : 64) : (a.KC <= 32 ? 64 : 128);  // free slots between compactions: cap - KC
+  // free slots between compactions: cap - KC.  Ping-pong keeps one buffer set per warpgroup (L::n_sets), each with KC + 16.
+  a.cap = pq_pingpong(NQ, PASSES) ? a.KC + 16 : (a.KC <= 16 ? (NQ == 128 ? 32 : 64) : (a.KC <= 32 ? 64 : 128));
   if (const int cap_env = env_int("CUVS_B200_PQ_CAP", 0)) a.cap = std::max(a.KC + 8, std::min(128, cap_env));  // bisection knob
   if (STORE) a.cap = 0;  // no candidate buffers
-  const int fixed = L::off_cand + NQ * a.cap * 8 + 1024 /*alignment slack of the dynamic segment*/;
+  B2_EXPECTS(L::n_sets * a.cap <= 128, "pq_stream_scan: %d candidate buffer entries per query exceed the read-out's 128", L::n_sets * a.cap);
+  const int fixed = L::off_cand + L::n_sets * NQ * a.cap * 8 + 1024 /*alignment slack of the dynamic segment*/;
   a.cstages = std::min(kMaxCStages, (kSmemLimit - fixed) / a.blk);
   const int forced = env_int("CUVS_B200_PQ_CSTAGES", 0);  // limiter experiments only
   if (forced > 0) a.cstages = std::min(a.cstages, forced);
