@@ -9,20 +9,22 @@
 //   fp_8bit               cpp/src/neighbors/ivf_pq/ivf_pq_fp_8bit.cuh:31-100
 //   C wrapper             c/src/neighbors/ivf_pq.cpp
 //
-// Two fine-scan kernels sit behind cuvsIvfPqSearch (DESIGN.md §5):
-//   (A) pq_lut_scan_kernel — the reference's formulation restated for H100: one CTA per (query, probe),
-//       LUT[pq_dim x 2^bits] in shared memory (fp32 / fp16 / fp_8bit<5>), codes streamed with 128-bit
-//       loads, scores accumulated in subspace order (bit-identical to oracle/oracle.c for fp32), block-level
-//       threshold filter + rank compaction for the top-k'.  Work is bound by shared-memory LUT gathers
-//       (one 4-byte bank access per code) — 4.0e11 gathers per 10k-query batch at config C2.
-//   (B) decoded-tile scan on wgmma — score(x) = sum_i lut[i, code_i] is algebraically
-//       |r - y(x)|^2 with r = R q - c_rot[list] and y(x) the concatenation of the PQ centres selected by
-//       the codes; the index keeps y(x) as bf16 rows (codebook entries are rounded to bf16 at training
-//       time so the rows are exact), pairs are bucketed by list and each list tile is contracted against
-//       up to 128 probing queries at once on the tensor cores (ivf_common.cu + scan_tc.cu).  This removes
-//       the per-(query,probe) LUT build and the 4e11 shared-memory gathers altogether.
-// (B) is used when lut_dtype == internal_distance_dtype == fp32 and the index holds decoded rows
-// (conservative_memory_allocation == false); (A) otherwise or with CUVS_B200_PQ_PATH=lut.
+// Three fine scans sit behind cuvsIvfPqSearch (DESIGN.md §5); plan_scan picks one per search:
+//   stream   pq_stream_scan (scan_pq.cu) — score(x) = sum_i lut[i, code_i] is algebraically |r - y(x)|^2 with
+//            r = R q - c_rot[list] and y(x) the concatenation of the PQ centres selected by the codes (codebook entries
+//            are rounded to bf16 at training time, so y(x) is exact in bf16).  The index keeps each list as a stream of
+//            code tiles; pairs are bucketed by list, and the kernel decodes every tile on the SM and contracts it against
+//            the list's probing queries on wgmma.  This removes the per-(query, probe) LUT build and its shared-memory
+//            gathers (one per code: 4.0e11 per 10k-query batch at config C2), which bound the LUT kernel.
+//   decoded  tc_scan_topk (scan_tc.cu) over y(x) kept as bf16 rows: a small index caches them as well, for batches that
+//            send >= 128 queries to the average list.
+//   lut      pq_lut_scan_kernel — the reference's formulation restated for H100: one CTA per (query, probe),
+//            LUT[pq_dim x 2^bits] in shared memory (fp32 / fp16 / fp_8bit<5>), codes read with 128-bit loads, scores
+//            accumulated in subspace order (bit-identical to oracle/oracle.c for fp32).  It serves the searches the other
+//            two do not (an index with neither, k > 64 without a code stream) and CUVS_B200_PQ_PATH=lut.
+// Each keeps the k' best per (query, probe) in its epilogue for k <= 64.  For k > 64 the stream and LUT kernels store every
+// score to a dense per-pair segment instead, and a segmented select takes each pair's k best.  Either way the probes of a
+// query are then merged into its k best.
 //
 // Cosine is inner product over unit vectors plus 1 (DESIGN.md §5): unit training rows and centres at build, x / |x| in the
 // encode path (encode_rows), unit rotated queries at search, and the +1 in the LUT kernel or in the per-pair offset `add`.
@@ -74,11 +76,11 @@ struct ivf_pq_index {
   // want rows (getters, extend, serialize, the LUT kernel).
   mutable owned<uint8_t> codes;
   owned<int64_t> ids;    // [rows_total], kPadId on padding rows
-  // decoded side (path B)
+  // decoded side (the decoded scan)
   int Kp = 0;
   owned<__nv_bfloat16> yhat;  // [rows_total, Kp]
   owned<__nv_bfloat16> hx;    // [rows_total, 16] half-norm plane: |y|^2/2 (0 for inner product), +inf on padding rows
-  // streamed side (path C, scan_pq.cu): lane-transposed code tiles + half norms, bank-transposed bf16x2 codebook words.
+  // streamed side (the stream scan, scan_pq.cu): lane-transposed code tiles + half norms, bank-transposed bf16x2 codebook words.
   // When the shape is served by the code-streaming kernel the decoded rows above are NOT kept (pq_dim + 4 bytes per
   // vector instead of 2 * rot_dim + 32).
   owned<uint8_t> cstream;    // [rows_total / 128, pq_stream_tile_bytes(pq_dim)]
@@ -241,7 +243,7 @@ __global__ void pq_init_kernel(float* __restrict__ pq_centers, int64_t n_books, 
   for (int j = 0; j < pq_len; ++j) pq_centers[(b * pq_len + j) * book + code] = resid[row * rot_dim + sub * pq_len + j];
 }
 
-// decoded bf16 rows + half norms from codes (path B).  one warp per row.
+// decoded bf16 rows + half norms from codes (the decoded scan).  one warp per row.
 __global__ void pq_decode_kernel(const uint8_t* __restrict__ codes, const int64_t* __restrict__ ids, int64_t rows, int pq_dim,
                                  int pq_len, int book, int Kp, const float* __restrict__ pq_centers, int per_cluster,
                                  const int64_t* __restrict__ list_offsets, int64_t n_lists, bool ip,
@@ -442,7 +444,7 @@ __global__ void item_segments_kernel(tc_item* __restrict__ items, const int* __r
   if (i < *n_items) items[i].out_off = static_cast<uint64_t>(seg_off[items[i].a_row0]);
 }
 
-// ---- (A) LUT scan: one CTA per (query, probe) slot ------------------------------------------------
+// ---- LUT scan: one CTA per (query, probe) slot ------------------------------------------------
 constexpr int kLutThreads = 128;
 constexpr int kLutBuf     = 256;  // candidate buffer (entries) per CTA
 
@@ -507,33 +509,32 @@ pq_lut_scan_kernel(const float* __restrict__ q_rot, const float* __restrict__ ce
   const uint32_t n   = list_sizes[l];
   const int vec16    = pq_dim / 16;  // uint4 loads per row when pq_dim % 16 == 0
   const bool aligned = (pq_dim % 16 == 0);
+  // score of list row i: its codes' LUT entries summed in subspace order in OutT, plus cosine's 1
+  auto row_score = [&](uint32_t i) -> float {
+    const uint8_t* code = codes + (row0 + i) * pq_dim;
+    OutT score = OutT(0.f);
+    if (aligned) {
+      for (int v = 0; v < vec16; ++v) {
+        const uint4 w = reinterpret_cast<const uint4*>(code)[v];
+        const uint32_t ws[4] = {w.x, w.y, w.z, w.w};
+#pragma unroll
+        for (int b = 0; b < 16; ++b) {
+          const uint32_t cdx = (ws[b >> 2] >> ((b & 3) * 8)) & 0xffu;
+          score += OutT(lut_conv<LutT>::dec(lut[((v * 16 + b) << pq_bits) + cdx], ip));
+        }
+      }
+    } else {
+      for (int s = 0; s < pq_dim; ++s) score += OutT(lut_conv<LutT>::dec(lut[(s << pq_bits) + code[s]], ip));
+    }
+    float fs = float(score);
+    if (cosine) fs += 1.0f;
+    return fs;
+  };
 
   if constexpr (Store) {
     float* seg         = out_score + seg_off[slot];
     const uint32_t pad = static_cast<uint32_t>(list_offsets[l + 1] - row0);
-    for (uint32_t i = threadIdx.x; i < pad; i += blockDim.x) {
-      float fs = INFINITY;
-      if (i < n) {
-        const uint8_t* code = codes + (row0 + i) * pq_dim;
-        OutT score = OutT(0.f);
-        if (aligned) {
-          for (int v = 0; v < vec16; ++v) {
-            const uint4 w = reinterpret_cast<const uint4*>(code)[v];
-            const uint32_t ws[4] = {w.x, w.y, w.z, w.w};
-#pragma unroll
-            for (int b = 0; b < 16; ++b) {
-              const uint32_t cdx = (ws[b >> 2] >> ((b & 3) * 8)) & 0xffu;
-              score += OutT(lut_conv<LutT>::dec(lut[((v * 16 + b) << pq_bits) + cdx], ip));
-            }
-          }
-        } else {
-          for (int s = 0; s < pq_dim; ++s) score += OutT(lut_conv<LutT>::dec(lut[(s << pq_bits) + code[s]], ip));
-        }
-        fs = float(score);
-        if (cosine) fs += 1.0f;
-      }
-      seg[i] = fs;
-    }
+    for (uint32_t i = threadIdx.x; i < pad; i += blockDim.x) seg[i] = i < n ? row_score(i) : INFINITY;
     return;
   }
 
@@ -561,23 +562,7 @@ pq_lut_scan_kernel(const float* __restrict__ q_rot, const float* __restrict__ ce
   for (uint32_t base = 0; base < n; base += blockDim.x) {
     const uint32_t i = base + threadIdx.x;
     if (i < n) {
-      const uint8_t* code = codes + (row0 + i) * pq_dim;
-      OutT score = OutT(0.f);
-      if (aligned) {
-        for (int v = 0; v < vec16; ++v) {
-          const uint4 w = reinterpret_cast<const uint4*>(code)[v];
-          const uint32_t ws[4] = {w.x, w.y, w.z, w.w};
-#pragma unroll
-          for (int b = 0; b < 16; ++b) {
-            const uint32_t cdx = (ws[b >> 2] >> ((b & 3) * 8)) & 0xffu;
-            score += OutT(lut_conv<LutT>::dec(lut[((v * 16 + b) << pq_bits) + cdx], ip));
-          }
-        }
-      } else {
-        for (int s = 0; s < pq_dim; ++s) score += OutT(lut_conv<LutT>::dec(lut[(s << pq_bits) + code[s]], ip));
-      }
-      float fs = float(score);
-      if (cosine) fs += 1.0f;
+      const float fs = row_score(i);
       if (fs < s_thr) {
         int at = atomicAdd(&s_cnt, 1);
         if (at < kLutBuf) { bv[at] = fs; bp[at] = static_cast<uint32_t>(row0 + i); }
@@ -707,8 +692,7 @@ void refresh_decoded(resources* res, ivf_pq_index& idx)
   idx.cstream.release();
   idx.cb_words.release();
   if (idx.conservative || !tc_supported(res->device, idx.rot_dim)) { idx.yhat.release(); idx.hx.release(); return; }
-  static const bool keep_decoded = getenv("CUVS_B200_PQ_KEEP_DECODED") != nullptr;  // A/B experiments against path (B)
-  if (!keep_decoded && idx.Kp == idx.rot_dim &&
+  if (idx.Kp == idx.rot_dim &&
       pq_stream_supported(res->device, idx.pq_dim, idx.pq_len, idx.pq_bits, idx.codebook_kind == CUVS_IVF_PQ_CODEBOOK_GEN_PER_SUBSPACE)) {
     idx.cstream.alloc(static_cast<size_t>(std::max<int64_t>(R / 128, 1)) * pq_stream_tile_bytes(idx.pq_dim));
     idx.cb_words.alloc(static_cast<size_t>(idx.pq_dim / 32) * 256 * 32);
@@ -717,7 +701,7 @@ void refresh_decoded(resources* res, ivf_pq_index& idx)
     // A SMALL index additionally caches its decoded rows (2 * rot_dim bytes per vector, derived data): when a batch sends
     // hundreds of queries to every list (10M vectors / 1024 lists / 10k x 64 probes = 625 per list) the stream kernel would
     // decode each list once per 64 probing queries, and reading rows decoded once at build time is the better trade.  The
-    // search picks per call (dense_probing below).  Budget: CUVS_B200_PQ_DECODED_BUDGET_MB (default 4096, 0 = never).
+    // search picks per call (`dense` in plan_scan).  Budget: CUVS_B200_PQ_DECODED_BUDGET_MB (default 4096, 0 = never).
     const char* bm        = getenv("CUVS_B200_PQ_DECODED_BUDGET_MB");
     const int64_t budget  = (bm ? atoll(bm) : 4096) << 20;
     const bool also_rows  = R > 0 && static_cast<int64_t>(R) * idx.Kp * 2 <= budget;
@@ -736,8 +720,7 @@ void refresh_decoded(resources* res, ivf_pq_index& idx)
       idx.yhat.release();
       idx.hx.release();
     }
-    static const bool keep_flat = getenv("CUVS_B200_PQ_KEEP_FLAT") != nullptr;
-    if (!keep_flat && R > 0) {  // the stream is the index: pq_dim + 4 bytes per vector (+ 8 for the id)
+    if (R > 0) {  // the stream is the index: pq_dim + 4 bytes per vector (+ 8 for the id)
       B2_CUDA(cudaStreamSynchronize(s));
       idx.codes.release();
     }
@@ -944,13 +927,6 @@ ivf_pq_index* ivf_pq_build(resources* res, const cuvsIvfPqIndexParams& p, const 
   return idx.release();
 }
 
-int env_path()  // read on every search: tests switch paths inside one process
-{
-  const char* e = getenv("CUVS_B200_PQ_PATH");
-  if (!e) return 0;
-  return strcmp(e, "lut") == 0 ? 1 : (strcmp(e, "tc") == 0 ? 2 : (strcmp(e, "stream") == 0 ? 3 : 0));  // stream: never the decoded-row cache
-}
-
 // k > 64: upper bound on the dense score rows of one query, the sum of the n_probes largest padded lists
 int64_t large_k_rows_per_query(const ivf_pq_index& idx, uint32_t n_probes)
 {
@@ -973,89 +949,111 @@ int64_t large_k_budget()
   return std::min<int64_t>(int64_t(8) << 30, static_cast<int64_t>(free_b / 2));
 }
 
-// k > 64 (DESIGN.md §5 "k > 64"): the scan writes every (pair, list row) score to the pair's dense segment (store epilogue of
-// the code-stream kernel for stream indexes, store mode of the LUT kernel for every other index), a segmented select takes each
-// pair's k best with their index rows, and the probes of a query are merged as on the k <= 64 path with KCW = k.  Scores of
-// one pair differ from its distances only by the pair's `add` and a positive `scale`, so the per-pair order is the final one.
-void search_large_k(resources* res, const ivf_pq_index& idx, const cuvsIvfPqSearchParams& sp, const float* q_rot, const uint32_t* probes,
-                    int64_t nq, uint32_t n_probes, int k, int64_t* out_idx, float* out_dist)
+// The fine scan of one search (DESIGN.md §5), decided in one place before any work is queued.  env is CUVS_B200_PQ_PATH: lut,
+// tc (the default choice) or stream, read on every search because tests switch paths inside one process.  reduced: lut_dtype or
+// internal_distance_dtype is not fp32.  dense: the index also caches decoded rows, k <= 32, env != stream and the batch sends
+// >= 128 queries to the average list (the stream kernel would decode each list more than twice per batch).
+//
+//                  k <= 64                                         k > 64 (store)
+//   stream         env != lut && code stream && !dense             env != lut && code stream
+//   decoded        not stream, env != lut && decoded rows          never
+//   lut            otherwise                                       otherwise
+//   passes         reduced ? 1 : 2                                 same
+//   KC             k <= 16 ? 16 : (k <= 32 or decoded ? 32 : 64)   0
+//   KCW            KC x (decoded ? tc_lists_per_item() : 1)        0 to bucket_probes, k after the segment select
+//   group          stream ? pq_stream_group(pairs per list, KC, passes) : 128   same, with KC = 0
+//   pruning bound  tensor-core paths with k <= KC                  none
+//
+// passes: fp32 LUT + fp32 accumulation (the reference's exact formulation) splits the residual into two bf16 planes; the decoded
+// rows ARE bf16, so the scores equal the LUT sums to fp32 rounding.  A reduced-precision request takes one pass over the residual
+// rounded to bf16, the same class of approximation at tensor-core speed; lut forces the faithful LUT kernel (bit-level
+// emulation of the fp16 / fp_8bit<5> entries).  KCW: the decoded-row epilogue keeps one sorted list of KC per column half of
+// the tile; for k > KC the union of the two stands in for the pair's top-k (exact whenever no more than KC of them fall into
+// one half).  group: queries per work item, 128 for the query-major kernels; the stream kernel takes 32 / 64 / 128 from the
+// average pairs per list.  store (k > 64, DESIGN.md §5 "k > 64"): the scan writes every (pair, list row) score to the pair's
+// dense segment and a segmented select takes each pair's k best; scores of one pair differ from its distances only by the
+// pair's `add` and a positive `scale`, so the per-pair order is the final one.
+enum class scan_path { stream, decoded, lut };
+struct scan_plan {
+  scan_path path;
+  bool store;
+  int passes, group, KC, KCW;
+};
+
+scan_plan plan_scan(const ivf_pq_index& idx, const cuvsIvfPqSearchParams& sp, int64_t nq, uint32_t n_probes, int k)
 {
-  auto s            = res->stream;
-  const bool ip     = is_ip(idx.metric);
-  const bool cosine = idx.metric == CosineExpanded;
+  const char* e         = getenv("CUVS_B200_PQ_PATH");
+  const bool env_lut    = e != nullptr && strcmp(e, "lut") == 0;
+  const bool env_stream = e != nullptr && strcmp(e, "stream") == 0;
   const bool reduced    = !(sp.lut_dtype == CUDA_R_32F && sp.internal_distance_dtype == CUDA_R_32F);
-  const bool use_stream = env_path() != 1 && idx.cstream.data() != nullptr;
-  const int passes      = reduced ? 1 : 2;
-  const int group = use_stream ? pq_stream_group(static_cast<double>(nq) * n_probes / std::max<uint32_t>(idx.n_lists, 1), 0, passes) : 128;
-  probe_buckets pb;
-  bucket_probes(res, probes, nq, static_cast<int>(n_probes), idx.n_lists, idx.lists.d_offsets.data(), 0, pb, 0, 0xffffffffu, group);
-  const int64_t n_pairs = pb.n_pairs;
-  dbuf<int64_t> seg_off(static_cast<size_t>(n_pairs), s);
-  dbuf<uint32_t> seg_len(static_cast<size_t>(n_pairs), s), seg_base(static_cast<size_t>(n_pairs), s);
+  const bool dense      = idx.yhat.data() != nullptr && k <= 32 && !env_stream &&
+                     static_cast<double>(nq) * n_probes >= 128.0 * std::max<uint32_t>(idx.n_lists, 1);
+  scan_plan p{};
+  p.store = k > 64;
+  if (!env_lut && idx.cstream.data() != nullptr && (p.store || !dense)) p.path = scan_path::stream;
+  else if (!env_lut && !p.store && idx.yhat.data() != nullptr) p.path = scan_path::decoded;
+  else p.path = scan_path::lut;
+  const bool decoded = p.path == scan_path::decoded;
+  p.passes = reduced ? 1 : 2;
+  p.KC     = p.store ? 0 : (k <= 16 ? 16 : (k <= 32 || decoded ? 32 : 64));
+  p.KCW    = p.KC * (decoded ? tc_lists_per_item() : 1);
+  p.group  = p.path == scan_path::stream
+               ? pq_stream_group(static_cast<double>(nq) * n_probes / std::max<uint32_t>(idx.n_lists, 1), p.KC, p.passes)
+               : 128;
+  return p;
+}
+
+// Residual rows of the tensor-core scans, one per pair slot (slots of dropped pairs are never read; the 128 rows past the pairs
+// are zero): bf16 planes of q_rot - c_rot (L2) or q_rot (IP), hi and, with two passes, lo; add[slot] is the pair's offset (see
+// pair_rows_kernel).  Returns `scale`: a distance is add[slot] + scale * score (L2: |r|^2 + 2 (|y|^2/2 - r.y); IP: -(q.(c+y));
+// cosine: 1 - q.(c+y)).
+struct residual_rows {
+  int64_t rows = 0;
+  dbuf<__nv_bfloat16> hi, lo;
+};
+float pair_residual_rows(cudaStream_t s, const ivf_pq_index& idx, const float* q_rot, const probe_buckets& pb, const scan_plan& plan,
+                         residual_rows& a, dbuf<float>& add)
+{
+  const bool ip = is_ip(idx.metric);
+  a.rows        = pb.n_pairs + 128;
+  a.hi.alloc(static_cast<size_t>(a.rows) * idx.Kp, s);
+  if (plan.passes == 2) a.lo.alloc(static_cast<size_t>(a.rows) * idx.Kp, s);
+  add.alloc(static_cast<size_t>(pb.n_pairs), s);
   count_launch();
-  pair_segments_kernel<<<1, 1024, 0, s>>>(pb.pair_list.data(), pb.n_items.data() + 1, n_pairs, idx.lists.d_offsets.data(),
-                                          idx.lists.d_sizes.data(), seg_off.data(), seg_len.data(), seg_base.data());
+  pair_rows_kernel<<<blocks_for(a.rows * 32, 256), 256, 0, s>>>(q_rot, idx.centers_rot.data(), pb.pair_query.data(), pb.pair_list.data(),
+                                                                 pb.n_items.data() + 1, a.rows, idx.rot_dim, idx.Kp, ip, a.hi.data(),
+                                                                 a.lo.data(), add.data(), plan.path == scan_path::stream,
+                                                                 idx.metric == CosineExpanded);
   B2_CUDA(cudaGetLastError());
-  dbuf<float> scores(static_cast<size_t>(std::max<int64_t>(1, nq * large_k_rows_per_query(idx, n_probes))), s);
-  dbuf<float> add;
-  float scale = 1.0f;
-  if (use_stream) {
-    const int64_t a_rows = n_pairs + 128;
-    dbuf<__nv_bfloat16> a_hi(static_cast<size_t>(a_rows) * idx.Kp, s), a_lo;
-    if (passes == 2) a_lo.alloc(static_cast<size_t>(a_rows) * idx.Kp, s);
-    add.alloc(static_cast<size_t>(n_pairs), s);
-    count_launch(2);
-    pair_rows_kernel<<<blocks_for(a_rows * 32, 256), 256, 0, s>>>(q_rot, idx.centers_rot.data(), pb.pair_query.data(), pb.pair_list.data(),
-                                                                   pb.n_items.data() + 1, a_rows, idx.rot_dim, idx.Kp, ip, a_hi.data(),
-                                                                   a_lo.data(), add.data(), true, cosine);
-    item_segments_kernel<<<blocks_for(pb.max_items, 256), 256, 0, s>>>(pb.items.data(), pb.n_items.data(), seg_off.data());
-    B2_CUDA(cudaGetLastError());
-    scale = ip ? 1.0f : 2.0f;
+  return ip ? 1.0f : 2.0f;
+}
+
+// The LUT kernel for the search's LUT and distance dtypes, one CTA per pair slot.  The grid covers every slot: the live count
+// is on the device, and the slots past it (dropped pairs, garbage pair_query) exit at once.
+template <bool Store>
+void launch_lut_scan(cudaStream_t s, const ivf_pq_index& idx, const cuvsIvfPqSearchParams& sp, const float* q_rot, const probe_buckets& pb,
+                     int KC, float* out_score, uint32_t* out_pos, int KCW, const int64_t* seg_off)
+{
+  const size_t lut_b = sp.lut_dtype == CUDA_R_32F ? 4 : (sp.lut_dtype == CUDA_R_16F ? 2 : 1);
+  const size_t smem  = ((static_cast<size_t>(idx.pq_dim) * idx.book() * lut_b + 15) & ~size_t(15)) + 2 * idx.rot_dim * sizeof(float) +
+                      (Store ? 0 : 4 * kLutBuf * sizeof(float));  // select mode: candidate and compaction buffers
+  B2_EXPECTS(smem <= 227 * 1024, "ivf_pq: LUT (%zu bytes) does not fit in shared memory; use a smaller lut_dtype", smem);
+  const bool per_cl = idx.codebook_kind == CUVS_IVF_PQ_CODEBOOK_GEN_PER_CLUSTER;
+  auto run = [&](auto kern) {
+    B2_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
     timed_section ts("pq_scan", s);
-    pq_stream_scan(s, res->device, a_hi.data(), a_lo.data(), a_rows, idx.Kp, idx.cstream.data(), idx.cb_words.data(), idx.pq_dim,
-                   pb.items.data(), pb.max_items, pb.n_items.data(), group, 0, passes, scores.data(), nullptr, 0, nullptr);
-  } else {
-    ensure_flat_codes(res, idx);
-    const size_t lut_b = sp.lut_dtype == CUDA_R_32F ? 4 : (sp.lut_dtype == CUDA_R_16F ? 2 : 1);
-    const size_t smem  = ((static_cast<size_t>(idx.pq_dim) * idx.book() * lut_b + 15) & ~size_t(15)) + 2 * idx.rot_dim * sizeof(float);
-    B2_EXPECTS(smem <= 227 * 1024, "ivf_pq: LUT (%zu bytes) does not fit in shared memory; use a smaller lut_dtype", smem);
-    const bool half_out = sp.internal_distance_dtype == CUDA_R_16F;
-    const bool per_cl   = idx.codebook_kind == CUVS_IVF_PQ_CODEBOOK_GEN_PER_CLUSTER;
-#define B2_LUT_STORE(LUT_T, OUT_T)                                                                                          \
-  {                                                                                                                         \
-    auto kern = pq_lut_scan_kernel<LUT_T, OUT_T, true>;                                                                     \
-    B2_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));               \
-    timed_section ts("pq_scan", s);                                                                                         \
-    count_launch();                                                                                                         \
-    kern<<<static_cast<unsigned>(n_pairs), kLutThreads, smem, s>>>(                                                         \
-      q_rot, idx.centers_rot.data(), idx.pq_centers.data(), per_cl, idx.codes.data(), idx.lists.d_offsets.data(),          \
-      idx.lists.d_sizes.data(), pb.pair_query.data(), pb.pair_list.data(), pb.n_items.data() + 1, idx.rot_dim, idx.pq_dim, \
-      idx.pq_len, idx.pq_bits, ip, cosine, 0, scores.data(), nullptr, 0, seg_off.data());                                  \
-  }
-    if (sp.lut_dtype == CUDA_R_32F) B2_LUT_STORE(float, float)
-    else if (sp.lut_dtype == CUDA_R_16F && !half_out) B2_LUT_STORE(__half, float)
-    else if (sp.lut_dtype == CUDA_R_16F && half_out) B2_LUT_STORE(__half, __half)
-    else if (!half_out) B2_LUT_STORE(uint8_t, float)
-    else B2_LUT_STORE(uint8_t, __half)
-#undef B2_LUT_STORE
-    B2_CUDA(cudaGetLastError());
-  }
-  // per pair: its k best rows (positions are index rows); ties go to the smaller row
-  int64_t max_len = 0;
-  for (int64_t v : idx.lists.h_sizes) max_len = std::max(max_len, v);
-  dbuf<float> cs(static_cast<size_t>(n_pairs) * k, s);
-  dbuf<uint32_t> cp(static_cast<size_t>(n_pairs) * k, s);
-  select_k_segments(s, scores.data(), seg_off.data(), seg_len.data(), seg_base.data(), n_pairs, max_len, k, cs.data(), cp.data(), true);
-  scores.release();
-  // per query: its probes' k best, in distance units, then the k best of those
-  const int64_t cand_w = static_cast<int64_t>(n_probes) * k;
-  dbuf<float> gs(static_cast<size_t>(nq * cand_w), s);
-  dbuf<uint32_t> gp(static_cast<size_t>(nq * cand_w), s), mp(static_cast<size_t>(nq) * k, s);
-  count_launch(2);
-  gather_pq_cands_kernel<<<blocks_for(nq * cand_w, 256), 256, 0, s>>>(cs.data(), cp.data(), pb.slot_of.data(), use_stream ? add.data() : nullptr,
-                                                                       scale, nq * cand_w, k, gs.data(), gp.data());
-  select_k(s, gs.data(), gp.data(), IDX_U32, nq, cand_w, cand_w, k, out_dist, mp.data(), IDX_U32, true);
-  finish_ids_kernel<<<blocks_for(nq * k, 256), 256, 0, s>>>(mp.data(), idx.ids.data(), out_dist, nq * k, int(idx.metric), out_idx);
+    count_launch();
+    kern<<<static_cast<unsigned>(pb.n_pairs), kLutThreads, smem, s>>>(
+      q_rot, idx.centers_rot.data(), idx.pq_centers.data(), per_cl, idx.codes.data(), idx.lists.d_offsets.data(), idx.lists.d_sizes.data(),
+      pb.pair_query.data(), pb.pair_list.data(), pb.n_items.data() + 1, idx.rot_dim, idx.pq_dim, idx.pq_len, idx.pq_bits,
+      is_ip(idx.metric), idx.metric == CosineExpanded, KC, out_score, out_pos, KCW, seg_off);
+  };
+  const bool half_out = sp.internal_distance_dtype == CUDA_R_16F;
+  if (sp.lut_dtype == CUDA_R_32F) run(pq_lut_scan_kernel<float, float, Store>);
+  else if (sp.lut_dtype == CUDA_R_16F && !half_out) run(pq_lut_scan_kernel<__half, float, Store>);
+  else if (sp.lut_dtype == CUDA_R_16F && half_out) run(pq_lut_scan_kernel<__half, __half, Store>);
+  else if (!half_out) run(pq_lut_scan_kernel<uint8_t, float, Store>);
+  else run(pq_lut_scan_kernel<uint8_t, __half, Store>);
   B2_CUDA(cudaGetLastError());
 }
 
@@ -1099,7 +1097,6 @@ void ivf_pq_search(resources* res, const ivf_pq_index& idx, const cuvsIvfPqSearc
   const float* q   = dl_ptr<float>(qt);
   int64_t* out_idx = dl_ptr<int64_t>(nt);
   float* out_dist  = dl_ptr<float>(dt);
-  const bool ip    = is_ip(idx.metric);
 
   // ---- coarse + rotation
   tc_rows_tmp qp;
@@ -1110,123 +1107,84 @@ void ivf_pq_search(resources* res, const ivf_pq_index& idx, const cuvsIvfPqSearc
   rotate_rows(s, q, nq, idx.dim, idx.rotation.data(), idx.rot_dim, q_rot.data());
   // cosine: the fine scan scores unit queries (ivf_pq_search.cuh:1020-1025).  The coarse ranking -q.c over unit centres does
   // not depend on |q|, so the probes above come from the raw queries, as in the reference.
-  const bool cosine = idx.metric == CosineExpanded;
-  if (cosine) normalize_rows(s, q_rot.data(), nq, idx.rot_dim, idx.rot_dim);
-  if (k > 64) return search_large_k(res, idx, sp, q_rot.data(), probes.data(), nq, n_probes, k, out_idx, out_dist);
+  if (idx.metric == CosineExpanded) normalize_rows(s, q_rot.data(), nq, idx.rot_dim, idx.rot_dim);
 
-  // ---- bucket pairs by list
-  // Decoded-row tensor-core scan whenever the index keeps decoded rows.  fp32 LUT + fp32 accumulation (the reference's
-  // exact formulation) -> 2-pass scan: the residual is split into two bf16 planes, the decoded rows ARE bf16, so the scores
-  // equal the LUT sums to fp32 rounding.  A reduced-precision LUT / accumulator request (fp16, fp8) -> 1-pass scan with the
-  // residual rounded to bf16: the same class of approximation, at tensor-core speed.  CUVS_B200_PQ_PATH=lut forces the
-  // faithful LUT kernel (bit-level emulation of the fp16 / fp_8bit<5> LUT entries).
-  const bool reduced = !(sp.lut_dtype == CUDA_R_32F && sp.internal_distance_dtype == CUDA_R_32F);
-  // (C) codes streamed + decoded on the SM — unless the index is small enough to also hold decoded rows AND this batch probes
-  // densely (>= 128 queries per list on average: the per-group decode would be repeated more than twice per list)
-  const bool dense_probing = idx.yhat.data() != nullptr && k <= 32 && env_path() != 3 &&
-                             static_cast<double>(nq) * n_probes >= 128.0 * std::max<uint32_t>(idx.n_lists, 1);
-  const bool use_stream = env_path() != 1 && idx.cstream.data() != nullptr && k <= 64 && !dense_probing;
-  const bool use_tc     = use_stream || (env_path() == 1 ? false : idx.yhat.data() != nullptr);
-  const int passes   = reduced ? 1 : 2;
-  const int lists = use_stream ? 1 : (use_tc ? tc_lists_per_item() : 1);
-  // candidates kept per (query, probe): the tensor-core epilogue keeps `lists` sorted lists of KC (one per column half of
-  // the tile); for k > KC the union of the two half lists stands in for the pair's top-k (exact whenever no more than KC of
-  // them fall into one half — an approximation only the k > 32 candidate-generation use case can see)
-  const int KC    = k <= 16 ? 16 : (k <= 32 || (use_tc && !use_stream) ? 32 : 64);
-  const int KCW   = KC * lists;
-  // queries per work item: 128 for the query-major kernels; the streamed kernel takes 32 / 64 / 128 probing queries (picked
-  // from the average number of pairs per list), as the MMA's M side at 64 / 128 and as its N side at 32
-  const int group = use_stream ? pq_stream_group(static_cast<double>(nq) * n_probes / std::max<uint32_t>(idx.n_lists, 1), KC, passes) : 128;
+  // ---- bucket pairs by list, fine scan
+  const scan_plan plan = plan_scan(idx, sp, nq, n_probes, k);
   probe_buckets pb;
-  bucket_probes(res, probes.data(), nq, static_cast<int>(n_probes), idx.n_lists, idx.lists.d_offsets.data(), KCW, pb, 0, 0xffffffffu, group);
-  dbuf<float> cs(static_cast<size_t>(pb.n_pairs) * KCW, s);
-  dbuf<uint32_t> cp(static_cast<size_t>(pb.n_pairs) * KCW, s);
+  bucket_probes(res, probes.data(), nq, static_cast<int>(n_probes), idx.n_lists, idx.lists.d_offsets.data(), plan.KCW, pb, 0, 0xffffffffu,
+                plan.group);
+  const int64_t n_pairs = pb.n_pairs;
+  dbuf<int64_t> seg_off;
+  dbuf<uint32_t> seg_len, seg_base;
+  dbuf<float> scores;  // store: the dense segments
+  if (plan.store) {
+    seg_off.alloc(static_cast<size_t>(n_pairs), s);
+    seg_len.alloc(static_cast<size_t>(n_pairs), s);
+    seg_base.alloc(static_cast<size_t>(n_pairs), s);
+    count_launch();
+    pair_segments_kernel<<<1, 1024, 0, s>>>(pb.pair_list.data(), pb.n_items.data() + 1, n_pairs, idx.lists.d_offsets.data(),
+                                            idx.lists.d_sizes.data(), seg_off.data(), seg_len.data(), seg_base.data());
+    B2_CUDA(cudaGetLastError());
+    scores.alloc(static_cast<size_t>(std::max<int64_t>(1, nq * large_k_rows_per_query(idx, n_probes))), s);
+  }
+  // per pair: its KCW candidates (store: its k best, from the segmented select below)
+  dbuf<float> cs;
+  dbuf<uint32_t> cp;
+  if (!plan.store) {
+    cs.alloc(static_cast<size_t>(n_pairs) * plan.KCW, s);
+    cp.alloc(static_cast<size_t>(n_pairs) * plan.KCW, s);
+  }
+  float* const scan_out = plan.store ? scores.data() : cs.data();
   dbuf<float> add;
   dbuf<int> bkeys;  // per-query pruning bound of the tensor-core scan (tc_bound), reused by the merge
   float scale = 1.0f;
-
-  if (use_tc) {
-    const int64_t a_rows = pb.n_pairs + 128;
-    dbuf<__nv_bfloat16> a_hi(static_cast<size_t>(a_rows) * idx.Kp, s), a_lo;
-    if (passes == 2) a_lo.alloc(static_cast<size_t>(a_rows) * idx.Kp, s);
-    add.alloc(static_cast<size_t>(pb.n_pairs), s);
-    // slots that were dropped (empty lists) are never read; slots beyond the live pairs are zero rows
-    count_launch();
-    pair_rows_kernel<<<blocks_for(a_rows * 32, 256), 256, 0, s>>>(q_rot.data(), idx.centers_rot.data(), pb.pair_query.data(),
-                                                                   pb.pair_list.data(), pb.n_items.data() + 1, a_rows, idx.rot_dim, idx.Kp, ip,
-                                                                   a_hi.data(), a_lo.data(), add.data(), use_stream, cosine);
-    B2_CUDA(cudaGetLastError());
-    scale = ip ? 1.0f : 2.0f;  // L2: |r|^2 + 2 (|y|^2/2 - r.y); IP: -(q.(c+y)); cosine: 1 - q.(c+y)
-    {
-      // probes of one query share a running bound on its k'-th best DISTANCE: d = add[slot] + scale * s
-      if (k <= KC) {  // the bound tracks a k-th best out of KC kept entries
-        bkeys.alloc(static_cast<size_t>(nq), s);
-        B2_CUDA(cudaMemsetAsync(bkeys.data(), tc_bound_init_byte, sizeof(int) * nq, s));
-      }
-      tc_bound bnd;
-      bnd.keys  = bkeys.data();
-      bnd.idx   = pb.pair_query.data();
-      bnd.add   = add.data();
-      bnd.scale = scale;
-      bnd.kth   = k;  // only the query's k best survive the merge below
-      timed_section ts("pq_scan", s);
-      if (use_stream)
-        pq_stream_scan(s, res->device, a_hi.data(), a_lo.data(), a_rows, idx.Kp, idx.cstream.data(), idx.cb_words.data(), idx.pq_dim,
-                       pb.items.data(), pb.max_items, pb.n_items.data(), group, KC, passes, cs.data(), cp.data(), KCW,
-                       bkeys.data() ? &bnd : nullptr);
-      else
-        tc_scan_topk(s, res->device, a_hi.data(), a_lo.data(), a_rows, idx.yhat.data(), nullptr, std::max<int64_t>(idx.lists.rows_total, 128),
-                     idx.Kp, idx.hx.data(), pb.items.data(), pb.max_items, pb.n_items.data(), KC, passes, cs.data(), cp.data(), KCW, bkeys.data() ? &bnd : nullptr);
-    }
-  } else {
+  if (plan.path == scan_path::lut) {
     ensure_flat_codes(res, idx);
-    const int book      = idx.book();
-    const size_t lut_b  = sp.lut_dtype == CUDA_R_32F ? 4 : (sp.lut_dtype == CUDA_R_16F ? 2 : 1);
-    const size_t smem   = ((static_cast<size_t>(idx.pq_dim) * book * lut_b + 15) & ~size_t(15)) + 2 * idx.rot_dim * sizeof(float) +
-                        4 * kLutBuf * sizeof(float);
-    B2_EXPECTS(smem <= 227 * 1024, "ivf_pq: LUT (%zu bytes) does not fit in shared memory; use a smaller lut_dtype", smem);
-    const bool half_out = sp.internal_distance_dtype == CUDA_R_16F;
-    const bool per_cl   = idx.codebook_kind == CUVS_IVF_PQ_CODEBOOK_GEN_PER_CLUSTER;
-    // slots of dropped pairs hold garbage pair_query: only launch over the live prefix
-    // (bucket_probes packs live pairs first; count is on the device -> launch over all slots, dead ones exit early)
-#define B2_LUT_LAUNCH(LUT_T, OUT_T)                                                                                         \
-  {                                                                                                                         \
-    auto kern = pq_lut_scan_kernel<LUT_T, OUT_T>;                                                                           \
-    B2_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));               \
-    timed_section ts("pq_scan", s);                                                                                         \
-    count_launch();                                                                                                         \
-    kern<<<static_cast<unsigned>(pb.n_pairs), kLutThreads, smem, s>>>(                                                      \
-      q_rot.data(), idx.centers_rot.data(), idx.pq_centers.data(), per_cl, idx.codes.data(), idx.lists.d_offsets.data(),   \
-      idx.lists.d_sizes.data(), pb.pair_query.data(), pb.pair_list.data(), pb.n_items.data() + 1, idx.rot_dim, idx.pq_dim, idx.pq_len, idx.pq_bits, ip,  \
-      cosine, KC, cs.data(), cp.data(), KCW, nullptr);                                                                      \
+    (plan.store ? launch_lut_scan<true> : launch_lut_scan<false>)(s, idx, sp, q_rot.data(), pb, plan.KC, scan_out, cp.data(), plan.KCW,
+                                                                  seg_off.data());
+  } else {
+    residual_rows a;
+    scale = pair_residual_rows(s, idx, q_rot.data(), pb, plan, a, add);
+    if (plan.store) {
+      count_launch();
+      item_segments_kernel<<<blocks_for(pb.max_items, 256), 256, 0, s>>>(pb.items.data(), pb.n_items.data(), seg_off.data());
+      B2_CUDA(cudaGetLastError());
+    }
+    // probes of one query share a running bound on its k'-th best DISTANCE: d = add[slot] + scale * s
+    if (k <= plan.KC) {  // the bound tracks a k-th best out of KC kept entries
+      bkeys.alloc(static_cast<size_t>(nq), s);
+      B2_CUDA(cudaMemsetAsync(bkeys.data(), tc_bound_init_byte, sizeof(int) * nq, s));
+    }
+    tc_bound bnd;
+    bnd.keys  = bkeys.data();
+    bnd.idx   = pb.pair_query.data();
+    bnd.add   = add.data();
+    bnd.scale = scale;
+    bnd.kth   = k;  // only the query's k best survive the merge below
+    timed_section ts("pq_scan", s);
+    if (plan.path == scan_path::stream)
+      pq_stream_scan(s, res->device, a.hi.data(), a.lo.data(), a.rows, idx.Kp, idx.cstream.data(), idx.cb_words.data(), idx.pq_dim,
+                     pb.items.data(), pb.max_items, pb.n_items.data(), plan.group, plan.KC, plan.passes, scan_out, cp.data(), plan.KCW,
+                     bkeys.data() ? &bnd : nullptr);
+    else
+      tc_scan_topk(s, res->device, a.hi.data(), a.lo.data(), a.rows, idx.yhat.data(), nullptr, std::max<int64_t>(idx.lists.rows_total, 128),
+                   idx.Kp, idx.hx.data(), pb.items.data(), pb.max_items, pb.n_items.data(), plan.KC, plan.passes, cs.data(), cp.data(),
+                   plan.KCW, bkeys.data() ? &bnd : nullptr);
   }
-    if (sp.lut_dtype == CUDA_R_32F) B2_LUT_LAUNCH(float, float)
-    else if (sp.lut_dtype == CUDA_R_16F && !half_out) B2_LUT_LAUNCH(__half, float)
-    else if (sp.lut_dtype == CUDA_R_16F && half_out) B2_LUT_LAUNCH(__half, __half)
-    else if (!half_out) B2_LUT_LAUNCH(uint8_t, float)
-    else B2_LUT_LAUNCH(uint8_t, __half)
-#undef B2_LUT_LAUNCH
-    B2_CUDA(cudaGetLastError());
+  int KCW = plan.KCW;
+  if (plan.store) {
+    // per pair: its k best rows (positions are index rows); ties go to the smaller row
+    int64_t max_len = 0;
+    for (int64_t v : idx.lists.h_sizes) max_len = std::max(max_len, v);
+    cs.alloc(static_cast<size_t>(n_pairs) * k, s);
+    cp.alloc(static_cast<size_t>(n_pairs) * k, s);
+    select_k_segments(s, scores.data(), seg_off.data(), seg_len.data(), seg_base.data(), n_pairs, max_len, k, cs.data(), cp.data(), true);
+    scores.release();
+    KCW = k;
   }
 
-  if (const char* dump = getenv("CUVS_B200_PQ_DUMP")) {
-    // debug: raw per-(query, probe) candidate lists of the fine scan -> file (slot_of [nq*n_probes] u32, cs / cp [n_pairs*KCW])
-    B2_CUDA(cudaStreamSynchronize(s));
-    std::vector<uint32_t> h_slot(static_cast<size_t>(nq) * n_probes), h_cp(static_cast<size_t>(pb.n_pairs) * KCW), h_probes(static_cast<size_t>(nq) * n_probes);
-    std::vector<float> h_cs(static_cast<size_t>(pb.n_pairs) * KCW);
-    B2_CUDA(cudaMemcpy(h_slot.data(), pb.slot_of.data(), h_slot.size() * 4, cudaMemcpyDeviceToHost));
-    B2_CUDA(cudaMemcpy(h_probes.data(), probes.data(), h_probes.size() * 4, cudaMemcpyDeviceToHost));
-    B2_CUDA(cudaMemcpy(h_cp.data(), cp.data(), h_cp.size() * 4, cudaMemcpyDeviceToHost));
-    B2_CUDA(cudaMemcpy(h_cs.data(), cs.data(), h_cs.size() * 4, cudaMemcpyDeviceToHost));
-    std::ofstream os(dump, std::ios::binary);
-    const int64_t hdr[4] = {nq, static_cast<int64_t>(n_probes), KCW, pb.n_pairs};
-    os.write(reinterpret_cast<const char*>(hdr), sizeof(hdr));
-    os.write(reinterpret_cast<const char*>(h_slot.data()), h_slot.size() * 4);
-    os.write(reinterpret_cast<const char*>(h_probes.data()), h_probes.size() * 4);
-    os.write(reinterpret_cast<const char*>(h_cs.data()), h_cs.size() * 4);
-    os.write(reinterpret_cast<const char*>(h_cp.data()), h_cp.size() * 4);
-  }
-  // ---- per query: concatenate its probes' candidates (already in final distance units), top-k, ids
+  // ---- per query: concatenate its probes' candidates (in final distance units), top-k, ids
   const int64_t cand_w = static_cast<int64_t>(n_probes) * KCW;
   dbuf<uint32_t> mp(static_cast<size_t>(nq) * k, s);
   if (!(bkeys.data() != nullptr &&
@@ -1235,8 +1193,8 @@ void ivf_pq_search(resources* res, const ivf_pq_index& idx, const cuvsIvfPqSearc
     dbuf<float> gs(static_cast<size_t>(nq) * cand_w, s);
     dbuf<uint32_t> gp(static_cast<size_t>(nq) * cand_w, s);
     count_launch();
-    gather_pq_cands_kernel<<<blocks_for(nq * cand_w, 256), 256, 0, s>>>(cs.data(), cp.data(), pb.slot_of.data(), use_tc ? add.data() : nullptr,
-                                                                         scale, nq * cand_w, KCW, gs.data(), gp.data());
+    gather_pq_cands_kernel<<<blocks_for(nq * cand_w, 256), 256, 0, s>>>(cs.data(), cp.data(), pb.slot_of.data(), add.data(), scale,
+                                                                         nq * cand_w, KCW, gs.data(), gp.data());
     select_k(s, gs.data(), gp.data(), IDX_U32, nq, cand_w, cand_w, k, out_dist, mp.data(), IDX_U32, true);
   }
   count_launch();

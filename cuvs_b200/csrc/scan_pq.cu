@@ -295,8 +295,39 @@ struct layout {
   static_assert(q_tile % 1024 == 0 && dec_stage % 1024 == 0, "operand tiles need 1024-byte alignment");
 };
 
-// (STORE ends its item with `continue`: the filtering epilogue after it is then unreachable, which is intended)
-#pragma nv_diag_suppress 128
+// One tile's MMA into the N-wide fragment d, from decode stage ds (descriptor bases d_lo / x_lo, stages `stage` apart): queries
+// on M (QM) D (+)= R . Y^T, else D (+)= Y . R^T.  8 K-steps over the decoded rows and the residual rows (q_lo, k-blocks q_kb
+// apart; with two passes the lo plane follows the NKB hi k-blocks), then the step that adds -|y|^2/2: the ext rows hold the
+// three bf16 pieces of -hn/2 in both chunks, the ones rows three 1s in both chunks.  Waits for the result.
+template <int N, bool QM, int NKB, int PASSES>
+__device__ __forceinline__ void pq_tile_mma(float (&d)[N / 2], uint32_t ds, uint32_t stage, uint32_t d_lo, uint32_t x_lo, uint32_t q_lo,
+                                            uint32_t q_kb, uint32_t ones_lo)
+{
+  ptx::wgmma_fence();
+  const uint32_t a0 = d_lo + ds * stage;
+#pragma unroll
+  for (int kb = 0; kb < NKB; ++kb) {
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      const uint64_t y  = ptx::desc(a0 + kb * (kDecTile >> 4) + k * 2, ptx::kDescHiSw128);
+      const uint32_t qd = q_lo + kb * q_kb + k * 2;
+      const uint64_t r  = ptx::desc(qd, ptx::kDescHiSw128);
+      if (QM) ptx::wgmma_bf16<N>(d, r, y, (kb | k) != 0 ? 1u : 0u);
+      else ptx::wgmma_bf16<N>(d, y, r, (kb | k) != 0 ? 1u : 0u);
+      if (PASSES == 2) {
+        const uint64_t rl = ptx::desc(qd + NKB * q_kb, ptx::kDescHiSw128);
+        if (QM) ptx::wgmma_bf16<N>(d, rl, y, 1u);
+        else ptx::wgmma_bf16<N>(d, y, rl, 1u);
+      }
+    }
+  }
+  const uint64_t xd = ptx::desc(x_lo + ds * stage, ptx::kDescHiSw32), od = ptx::desc(ones_lo, ptx::kDescHiSw32);
+  if (QM) ptx::wgmma_bf16<N>(d, od, xd, 1u);
+  else ptx::wgmma_bf16<N>(d, xd, od, 1u);
+  ptx::wgmma_commit();
+  ptx::wgmma_wait<0>();
+}
+
 // STORE (KC = 0, k > 64): no threshold filter, candidate buffers, compaction or bound.  The consumers write the score of every
 // (query column, list row) of the item to out_score[out_off + col * n_tiles * 128 + row]: one dense segment per pair, its
 // list's padded rows in list order (padding rows +inf).
@@ -548,30 +579,8 @@ pq_stream_scan_kernel(const __grid_constant__ CUtensorMap tmQ_hi, const __grid_c
         float* out        = P.out_score + item.out_off;
         for (uint32_t t = 0; t < item.n_tiles; ++t) {
           wait_dbg(P.dbg, &d_full[ds], dph, 0x204, static_cast<uint32_t>(it), t);
-          float d[NQ / 2];
-          ptx::wgmma_fence();
-          const uint32_t a0 = d_lo0 + ds * (L::dec_stage >> 4);
-#pragma unroll
-          for (int kb = 0; kb < NKB; ++kb) {
-#pragma unroll
-            for (int k = 0; k < 4; ++k) {
-              const uint64_t y  = ptx::desc(a0 + kb * (kDecTile >> 4) + k * 2, ptx::kDescHiSw128);
-              const uint32_t qd = q_lo0 + kb * (L::q_tile >> 4) + k * 2;
-              const uint64_t r  = ptx::desc(qd, ptx::kDescHiSw128);
-              if (kQM) ptx::wgmma_bf16<NQ>(d, r, y, (kb | k) != 0 ? 1u : 0u);
-              else ptx::wgmma_bf16<NQ>(d, y, r, (kb | k) != 0 ? 1u : 0u);
-              if (PASSES == 2) {
-                const uint64_t rl = ptx::desc(qd + NKB * (L::q_tile >> 4), ptx::kDescHiSw128);
-                if (kQM) ptx::wgmma_bf16<NQ>(d, rl, y, 1u);
-                else ptx::wgmma_bf16<NQ>(d, y, rl, 1u);
-              }
-            }
-          }
-          const uint64_t xd = ptx::desc(x_lo0 + ds * (L::dec_stage >> 4), ptx::kDescHiSw32), od = ptx::desc(ones_lo, ptx::kDescHiSw32);
-          if (kQM) ptx::wgmma_bf16<NQ>(d, od, xd, 1u);
-          else ptx::wgmma_bf16<NQ>(d, xd, od, 1u);
-          ptx::wgmma_commit();
-          ptx::wgmma_wait<0>();
+          float d[MN / 2];
+          pq_tile_mma<MN, kQM, NKB, PASSES>(d, ds, L::dec_stage >> 4, d_lo0, x_lo0, q_lo0, L::q_tile >> 4, ones_lo);
           __syncwarp();
           if (lane == 0) {
             ptx::mbar_arrive(&d_empty[ds]);
@@ -603,133 +612,108 @@ pq_stream_scan_kernel(const __grid_constant__ CUtensorMap tmQ_hi, const __grid_c
           }
         }
         qph ^= 1;
-        continue;
-      }
-      // per-column state: running threshold in t = -(score) units (a row is a candidate iff t > thr), empty buffer; one set
-      // per warpgroup in ping-pong
-      for (int i = te; i < L::n_sets * NQ; i += kEpiThreads) {
-        const int col = i % NQ;
-        float thr     = INFINITY;  // columns past the item's queries never collect anything
-        if (static_cast<uint32_t>(col) < item.valid_rows) {
-          thr = -INFINITY;
-          if (P.b_keys != nullptr) {
-            const uint32_t arow = item.a_row0 + col;
-            const int kb        = *reinterpret_cast<volatile int*>(P.b_keys + (P.b_idx ? P.b_idx[arow] : arow));
-            const float bv      = __int_as_float(kb >= 0 ? kb : kb ^ 0x7fffffff);
-            thr                 = -((bv - (P.b_add ? P.b_add[arow] : 0.f)) / P.b_scale);
-          }
-        }
-        sThr[i] = thr;
-        sCnt[i] = 0;
-      }
-      ptx::named_bar_sync(1, kEpiThreads);
-      wait_dbg(P.dbg, q_full, qph, 0x202, static_cast<uint32_t>(it), 0);
-
-      // ping-pong: this warpgroup's tiles of the item are t0, t0 + 2, ...; it may have none (an item of one tile)
-      const uint32_t t0 = kPP ? (wg ^ (g0 & 1u)) : 0, tstep = kPP ? 2 : 1;
-      if (kPP && t0 >= item.n_tiles && lane == 0) ptx::mbar_arrive(q_empty);
-      for (uint32_t t = t0; t < item.n_tiles; t += tstep) {
-        wait_dbg(P.dbg, &d_full[ds], dph, 0x204, static_cast<uint32_t>(it), t);
-        float d[MN / 2];
-        ptx::wgmma_fence();
-        const uint32_t a0 = d_lo0 + ds * (L::dec_stage >> 4);
-#pragma unroll
-        for (int kb = 0; kb < NKB; ++kb) {
-#pragma unroll
-          for (int k = 0; k < 4; ++k) {
-            const uint64_t y  = ptx::desc(a0 + kb * (kDecTile >> 4) + k * 2, ptx::kDescHiSw128);  // decoded rows
-            const uint32_t qd = q_lo0 + kb * (L::q_tile >> 4) + k * 2;                          // residual rows
-            const uint64_t r  = ptx::desc(qd, ptx::kDescHiSw128);
-            if (kQM) ptx::wgmma_bf16<MN>(d, r, y, (kb | k) != 0 ? 1u : 0u);
-            else ptx::wgmma_bf16<MN>(d, y, r, (kb | k) != 0 ? 1u : 0u);
-            if (PASSES == 2) {
-              const uint64_t rl = ptx::desc(qd + NKB * (L::q_tile >> 4), ptx::kDescHiSw128);
-              if (kQM) ptx::wgmma_bf16<MN>(d, rl, y, 1u);
-              else ptx::wgmma_bf16<MN>(d, y, rl, 1u);
+      } else {
+        // per-column state: running threshold in t = -(score) units (a row is a candidate iff t > thr), empty buffer; one set
+        // per warpgroup in ping-pong
+        for (int i = te; i < L::n_sets * NQ; i += kEpiThreads) {
+          const int col = i % NQ;
+          float thr     = INFINITY;  // columns past the item's queries never collect anything
+          if (static_cast<uint32_t>(col) < item.valid_rows) {
+            thr = -INFINITY;
+            if (P.b_keys != nullptr) {
+              const uint32_t arow = item.a_row0 + col;
+              const int kb        = *reinterpret_cast<volatile int*>(P.b_keys + (P.b_idx ? P.b_idx[arow] : arow));
+              const float bv      = __int_as_float(kb >= 0 ? kb : kb ^ 0x7fffffff);
+              thr                 = -((bv - (P.b_add ? P.b_add[arow] : 0.f)) / P.b_scale);
             }
           }
+          sThr[i] = thr;
+          sCnt[i] = 0;
         }
-        // -= |y|^2/2 : ext rows hold the three bf16 pieces of -hn/2 in both chunks, ones rows three 1s in both chunks
-        const uint64_t xd = ptx::desc(x_lo0 + ds * (L::dec_stage >> 4), ptx::kDescHiSw32), od = ptx::desc(ones_lo, ptx::kDescHiSw32);
-        if (kQM) ptx::wgmma_bf16<MN>(d, od, xd, 1u);
-        else ptx::wgmma_bf16<MN>(d, xd, od, 1u);
-        ptx::wgmma_commit();
-        ptx::wgmma_wait<0>();
-        __syncwarp();
-        if (lane == 0) {
-          ptx::mbar_arrive(&d_empty[ds]);
-          if (t + tstep >= item.n_tiles) ptx::mbar_arrive(q_empty);  // the item's residual rows may be replaced
-        }
-        if (kPP) dph ^= 1;  // (the warpgroup's own stage)
-        else if (++ds == kDecStages) { ds = 0; dph ^= 1; }
-
-        const uint32_t pos0 = item.b_row0 + t * 128 + (kQM ? rb : r0);
-        auto filter = [&](uint64_t only) -> uint64_t {
-          if constexpr (kQM) {
-            // (a warpgroup's thresholds change only in its own compaction, between its overflow barriers: read once per pass)
-            float th[2] = {thr_w[q0], thr_w[q0 + 8]};
-            if constexpr (kPP) {
-              // The other warpgroup's buffer may hold rows of LATER tiles, which lose exact ties to this tile's rows: against
-              // its threshold a row is kept iff t >= thr_x, not t > thr_x.  (Its own buffer holds only earlier rows, which
-              // win ties, so t > thr_w is exact.)  thr_x can rise while this runs: a stale value only keeps more rows.
-#pragma unroll
-              for (int h = 0; h < 2; ++h) {
-                const float tx = thr_x[q0 + 8 * h];
-                if (tx > th[h]) th[h] = nextafterf(tx, -INFINITY);
-              }
-            }
-            return pq_filter_rows<MN>(d, only, q0, pos0, th, cnt_w, cand_w, cap);
-          } else {
-            return pq_filter_frag<NQ>(d, only, lane, pos0, pos0 + 8, sThr, sCnt, sCand, cap);
-          }
-        };
-        uint64_t left = filter(~0ull);
-        // ONE barrier per tile (of the warpgroup in ping-pong, else of both) decides whether any buffer overflowed
-        while (bar_red_or(bar_id, bar_n, left != 0)) {
-          for (int col = cw0; col < NQ; col += cwn)
-            if (cnt_w[col] > cap) compact(col);  // (warp-uniform: every lane reads the same counter)
-          ptx::named_bar_sync(bar_id, bar_n);
-          if (left != 0) left = filter(left);
-        }
-      }
-      qph ^= 1;
-      if constexpr (kPP) {
-        g0 += item.n_tiles;
-        // both warpgroups' buffers are final; the read-out ranks their union (<= 2 cap <= 128 entries, see launch())
         ptx::named_bar_sync(1, kEpiThreads);
-      }
+        wait_dbg(P.dbg, q_full, qph, 0x202, static_cast<uint32_t>(it), 0);
 
-      // item done: every column's KC best -> global; publish the query's k-th best for the other items of the same query
-      for (int col = ew; col < static_cast<int>(min(item.valid_rows, static_cast<uint32_t>(NQ))); col += kEpiWarps) {
-        unsigned long long k[4];
-        int r[4];
-        const int n0 = min(sCnt[col], cap), n1 = kPP ? min(sCnt[NQ + col], cap) : 0;  // (ping-pong: the union of both sets)
-        pq_rank_select(sCand + col * cap, n0, sCand + (NQ + col) * cap, n1, lane, k, r);
-        const int n  = n0 + n1;
-        const int nk = min(n, KC);
-        const uint32_t arow = item.a_row0 + col;
-        const int64_t o     = static_cast<int64_t>(item.out_off) + static_cast<int64_t>(col) * P.out_row_stride;
-        auto emit = [&](unsigned long long key, int r) {
-          if (key == 0ull || r >= KC) return;
-          const float t = __uint_as_float(okey_inv(static_cast<uint32_t>(key >> 32)));
-          if (P.out_score != nullptr) { P.out_score[o + r] = -t; P.out_pos[o + r] = ~static_cast<uint32_t>(key); }
-          if (r == kth - 1 && P.b_keys != nullptr) {  // (n >= kth holds when such a rank exists)
-            const float pub = __fmaf_rn(P.b_scale, -t, P.b_add ? P.b_add[arow] : 0.f);
-            const int kp    = __float_as_int(pub);
-            atomicMin(P.b_keys + (P.b_idx ? P.b_idx[arow] : arow), kp >= 0 ? kp : kp ^ 0x7fffffff);
+        // ping-pong: this warpgroup's tiles of the item are t0, t0 + 2, ...; it may have none (an item of one tile)
+        const uint32_t t0 = kPP ? (wg ^ (g0 & 1u)) : 0, tstep = kPP ? 2 : 1;
+        if (kPP && t0 >= item.n_tiles && lane == 0) ptx::mbar_arrive(q_empty);
+        for (uint32_t t = t0; t < item.n_tiles; t += tstep) {
+          wait_dbg(P.dbg, &d_full[ds], dph, 0x204, static_cast<uint32_t>(it), t);
+          float d[MN / 2];
+          pq_tile_mma<MN, kQM, NKB, PASSES>(d, ds, L::dec_stage >> 4, d_lo0, x_lo0, q_lo0, L::q_tile >> 4, ones_lo);
+          __syncwarp();
+          if (lane == 0) {
+            ptx::mbar_arrive(&d_empty[ds]);
+            if (t + tstep >= item.n_tiles) ptx::mbar_arrive(q_empty);  // the item's residual rows may be replaced
           }
-        };
+          if (kPP) dph ^= 1;  // (the warpgroup's own stage)
+          else if (++ds == kDecStages) { ds = 0; dph ^= 1; }
+
+          const uint32_t pos0 = item.b_row0 + t * 128 + (kQM ? rb : r0);
+          auto filter = [&](uint64_t only) -> uint64_t {
+            if constexpr (kQM) {
+              // (a warpgroup's thresholds change only in its own compaction, between its overflow barriers: read once per pass)
+              float th[2] = {thr_w[q0], thr_w[q0 + 8]};
+              if constexpr (kPP) {
+                // The other warpgroup's buffer may hold rows of LATER tiles, which lose exact ties to this tile's rows: against
+                // its threshold a row is kept iff t >= thr_x, not t > thr_x.  (Its own buffer holds only earlier rows, which
+                // win ties, so t > thr_w is exact.)  thr_x can rise while this runs: a stale value only keeps more rows.
 #pragma unroll
-        for (int e = 0; e < 4; ++e) emit(k[e], r[e]);
-        if (P.out_score != nullptr)
-          for (int slot = nk + lane; slot < KC; slot += 32) { P.out_score[o + slot] = INFINITY; P.out_pos[o + slot] = 0xffffffffu; }
+                for (int h = 0; h < 2; ++h) {
+                  const float tx = thr_x[q0 + 8 * h];
+                  if (tx > th[h]) th[h] = nextafterf(tx, -INFINITY);
+                }
+              }
+              return pq_filter_rows<MN>(d, only, q0, pos0, th, cnt_w, cand_w, cap);
+            } else {
+              return pq_filter_frag<NQ>(d, only, lane, pos0, pos0 + 8, sThr, sCnt, sCand, cap);
+            }
+          };
+          uint64_t left = filter(~0ull);
+          // ONE barrier per tile (of the warpgroup in ping-pong, else of both) decides whether any buffer overflowed
+          while (bar_red_or(bar_id, bar_n, left != 0)) {
+            for (int col = cw0; col < NQ; col += cwn)
+              if (cnt_w[col] > cap) compact(col);  // (warp-uniform: every lane reads the same counter)
+            ptx::named_bar_sync(bar_id, bar_n);
+            if (left != 0) left = filter(left);
+          }
+        }
+        qph ^= 1;
+        if constexpr (kPP) {
+          g0 += item.n_tiles;
+          // both warpgroups' buffers are final; the read-out ranks their union (<= 2 cap <= 128 entries, see launch())
+          ptx::named_bar_sync(1, kEpiThreads);
+        }
+
+        // item done: every column's KC best -> global; publish the query's k-th best for the other items of the same query
+        for (int col = ew; col < static_cast<int>(min(item.valid_rows, static_cast<uint32_t>(NQ))); col += kEpiWarps) {
+          unsigned long long k[4];
+          int r[4];
+          const int n0 = min(sCnt[col], cap), n1 = kPP ? min(sCnt[NQ + col], cap) : 0;  // (ping-pong: the union of both sets)
+          pq_rank_select(sCand + col * cap, n0, sCand + (NQ + col) * cap, n1, lane, k, r);
+          const int n  = n0 + n1;
+          const int nk = min(n, KC);
+          const uint32_t arow = item.a_row0 + col;
+          const int64_t o     = static_cast<int64_t>(item.out_off) + static_cast<int64_t>(col) * P.out_row_stride;
+          auto emit = [&](unsigned long long key, int r) {
+            if (key == 0ull || r >= KC) return;
+            const float t = __uint_as_float(okey_inv(static_cast<uint32_t>(key >> 32)));
+            if (P.out_score != nullptr) { P.out_score[o + r] = -t; P.out_pos[o + r] = ~static_cast<uint32_t>(key); }
+            if (r == kth - 1 && P.b_keys != nullptr) {  // (n >= kth holds when such a rank exists)
+              const float pub = __fmaf_rn(P.b_scale, -t, P.b_add ? P.b_add[arow] : 0.f);
+              const int kp    = __float_as_int(pub);
+              atomicMin(P.b_keys + (P.b_idx ? P.b_idx[arow] : arow), kp >= 0 ? kp : kp ^ 0x7fffffff);
+            }
+          };
+#pragma unroll
+          for (int e = 0; e < 4; ++e) emit(k[e], r[e]);
+          if (P.out_score != nullptr)
+            for (int slot = nk + lane; slot < KC; slot += 32) { P.out_score[o + slot] = INFINITY; P.out_pos[o + slot] = 0xffffffffu; }
+        }
+        ptx::named_bar_sync(1, kEpiThreads);  // the next item's column init must not overtake another warp's read-out
       }
-      ptx::named_bar_sync(1, kEpiThreads);  // the next item's column init must not overtake another warp's read-out
     }
   }
 }
-
-#pragma nv_diag_default 128
 
 // ------------------------------------------------------------------------------------ build-side kernels
 // one CTA per 128-row tile: codes [128, pq_dim] -> lane-transposed 16-byte chunks + half norms
@@ -836,20 +820,22 @@ int env_int(const char* name, int dflt)
   return v ? atoi(v) : dflt;
 }
 
-template <int NQ, int NKB, int PASSES, bool STORE = false>
+// KC = 0: the store epilogue; otherwise the filtering one, which has no NQ = 128 two-pass kernel (pq_stream_scan rejects it)
+template <int NQ, int NKB, int PASSES>
 void launch(cudaStream_t stream, int sms, const CUtensorMap& mq_hi, const CUtensorMap& mq_lo, pq_args a, int n_items)
 {
-  using L   = layout<NQ, NKB, PASSES>;
-  auto kern = pq_stream_scan_kernel<NQ, NKB, PASSES, STORE>;
+  using L          = layout<NQ, NKB, PASSES>;
+  const bool store = a.KC == 0;
+  auto kern        = pq_stream_scan_kernel<NQ, NKB, PASSES, true>;
+  if constexpr (NQ < 128 || PASSES == 1)
+    if (!store) kern = pq_stream_scan_kernel<NQ, NKB, PASSES>;
   // free slots between compactions: cap - KC.  Ping-pong keeps one buffer set per warpgroup (L::n_sets), each with KC + 16.
   a.cap = pq_pingpong(NQ, PASSES) ? a.KC + 16 : (a.KC <= 16 ? (NQ == 128 ? 32 : 64) : (a.KC <= 32 ? 64 : 128));
   if (const int cap_env = env_int("CUVS_B200_PQ_CAP", 0)) a.cap = std::max(a.KC + 8, std::min(128, cap_env));  // bisection knob
-  if (STORE) a.cap = 0;  // no candidate buffers
+  if (store) a.cap = 0;  // no candidate buffers
   B2_EXPECTS(L::n_sets * a.cap <= 128, "pq_stream_scan: %d candidate buffer entries per query exceed the read-out's 128", L::n_sets * a.cap);
   const int fixed = L::off_cand + L::n_sets * NQ * a.cap * 8 + 1024 /*alignment slack of the dynamic segment*/;
   a.cstages = std::min(kMaxCStages, (kSmemLimit - fixed) / a.blk);
-  const int forced = env_int("CUVS_B200_PQ_CSTAGES", 0);  // limiter experiments only
-  if (forced > 0) a.cstages = std::min(a.cstages, forced);
   B2_EXPECTS(a.cstages >= 2, "pq_stream_scan: shared memory budget exceeded (NQ=%d KC=%d passes=%d)", NQ, a.KC, PASSES);
   const size_t smem = static_cast<size_t>(fixed) + static_cast<size_t>(a.cstages) * a.blk;
   static uint32_t* dbg_host = nullptr;  // CUVS_B200_PQ_DEBUG=1: deadlock report (see wait_dbg)
@@ -974,15 +960,10 @@ void pq_stream_scan(cudaStream_t stream, int device, const __nv_bfloat16* q_hi, 
   const int sms = sm_count_of(device);
   const int nkb = Kp / 64;
 #define B2_PQ_CASE(NQ_, NKB_, P_) \
-  if (KC > 0 && group == NQ_ && nkb == NKB_ && passes == P_) return launch<NQ_, NKB_, P_>(stream, sms, mq, mql, a, n_items);
+  if (group == NQ_ && nkb == NKB_ && passes == P_) return launch<NQ_, NKB_, P_>(stream, sms, mq, mql, a, n_items);
   B2_PQ_CASE(32, 1, 1) B2_PQ_CASE(64, 1, 1) B2_PQ_CASE(128, 1, 1) B2_PQ_CASE(32, 2, 1) B2_PQ_CASE(64, 2, 1) B2_PQ_CASE(128, 2, 1)
-  B2_PQ_CASE(32, 1, 2) B2_PQ_CASE(64, 1, 2) B2_PQ_CASE(32, 2, 2) B2_PQ_CASE(64, 2, 2)
+  B2_PQ_CASE(32, 1, 2) B2_PQ_CASE(64, 1, 2) B2_PQ_CASE(128, 1, 2) B2_PQ_CASE(32, 2, 2) B2_PQ_CASE(64, 2, 2) B2_PQ_CASE(128, 2, 2)
 #undef B2_PQ_CASE
-#define B2_PQ_STORE(NQ_, NKB_, P_) \
-  if (KC == 0 && group == NQ_ && nkb == NKB_ && passes == P_) return launch<NQ_, NKB_, P_, true>(stream, sms, mq, mql, a, n_items);
-  B2_PQ_STORE(32, 1, 1) B2_PQ_STORE(64, 1, 1) B2_PQ_STORE(128, 1, 1) B2_PQ_STORE(32, 2, 1) B2_PQ_STORE(64, 2, 1) B2_PQ_STORE(128, 2, 1)
-  B2_PQ_STORE(32, 1, 2) B2_PQ_STORE(64, 1, 2) B2_PQ_STORE(128, 1, 2) B2_PQ_STORE(32, 2, 2) B2_PQ_STORE(64, 2, 2) B2_PQ_STORE(128, 2, 2)
-#undef B2_PQ_STORE
   B2_FAIL("pq_stream_scan: no kernel for group=%d Kp=%d passes=%d", group, Kp, passes);
 }
 
