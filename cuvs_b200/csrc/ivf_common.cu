@@ -7,6 +7,8 @@
 
 #include <algorithm>
 #include <cfloat>
+#include <cstdlib>
+#include <functional>
 #include <vector>
 
 namespace b200 {
@@ -266,6 +268,50 @@ __global__ void gather_cands_kernel(const float* __restrict__ cs, const uint32_t
   }
   out_score[t] = s;
   out_pos[t]   = p;
+}
+
+// ---- k > 64: dense per-pair score segments (see pair_segments in ivf_common.cuh)
+// Slots are few (nq * n_probes): one CTA scans them, each thread a contiguous chunk.
+__global__ void __launch_bounds__(1024) pair_segments_kernel(const uint32_t* __restrict__ pair_list, const int* __restrict__ n_live,
+                                                             int64_t n_pairs, const int64_t* __restrict__ list_offsets,
+                                                             const uint32_t* __restrict__ list_sizes, int64_t* __restrict__ seg_off,
+                                                             uint32_t* __restrict__ seg_len, uint32_t* __restrict__ seg_base)
+{
+  __shared__ int64_t part[1024];
+  const int tid      = threadIdx.x;
+  const int64_t live = *n_live;
+  const int64_t per  = (n_pairs + 1023) / 1024;
+  const int64_t b = min(n_pairs, tid * per), e = min(n_pairs, b + per);
+  int64_t sum = 0;
+  for (int64_t i = b; i < min(e, live); ++i) sum += list_offsets[pair_list[i] + 1] - list_offsets[pair_list[i]];
+  part[tid] = sum;
+  __syncthreads();
+  for (int o = 1; o < 1024; o <<= 1) {
+    const int64_t v = tid >= o ? part[tid - o] : 0;
+    __syncthreads();
+    part[tid] += v;
+    __syncthreads();
+  }
+  int64_t run = part[tid] - sum;
+  for (int64_t i = b; i < e; ++i) {
+    seg_off[i] = run;
+    if (i < live) {
+      const uint32_t l = pair_list[i];
+      seg_len[i]       = list_sizes[l];
+      seg_base[i]      = static_cast<uint32_t>(list_offsets[l]);
+      run += list_offsets[l + 1] - list_offsets[l];
+    } else {
+      seg_len[i]  = 0;
+      seg_base[i] = 0;
+    }
+  }
+}
+
+// a store scan writes an item's pairs from the segment of its first slot on
+__global__ void item_segments_kernel(tc_item* __restrict__ items, const int* __restrict__ n_items, const int64_t* __restrict__ seg_off)
+{
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < *n_items) items[i].out_off = static_cast<uint64_t>(seg_off[items[i].a_row0]);
 }
 
 // ---- per-query merge of the probes' candidate lists ------------------------------------------
@@ -713,6 +759,42 @@ void gather_probe_candidates(cudaStream_t s, const float* cs, const uint32_t* cp
   count_launch();
   gather_cands_kernel<<<blocks_for(total, 256), 256, 0, s>>>(cs, cp, slot_of, total, KC, out_score, out_pos);
   B2_CUDA(cudaGetLastError());
+}
+
+void pair_segments(cudaStream_t s, const probe_buckets& pb, const list_layout& lists, int64_t* seg_off, uint32_t* seg_len,
+                   uint32_t* seg_base)
+{
+  count_launch();
+  pair_segments_kernel<<<1, 1024, 0, s>>>(pb.pair_list.data(), pb.n_items.data() + 1, pb.n_pairs, lists.d_offsets.data(),
+                                          lists.d_sizes.data(), seg_off, seg_len, seg_base);
+  B2_CUDA(cudaGetLastError());
+}
+
+void item_segments(cudaStream_t s, probe_buckets& pb, const int64_t* seg_off)
+{
+  count_launch();
+  item_segments_kernel<<<blocks_for(pb.max_items, 256), 256, 0, s>>>(pb.items.data(), pb.n_items.data(), seg_off);
+  B2_CUDA(cudaGetLastError());
+}
+
+int64_t large_k_rows_per_query(const list_layout& lists, uint32_t n_probes)
+{
+  const int64_t n_lists = lists.n_lists;
+  std::vector<int64_t> pad(static_cast<size_t>(n_lists));
+  for (int64_t l = 0; l < n_lists; ++l) pad[l] = lists.h_offsets[l + 1] - lists.h_offsets[l];
+  const int64_t m = std::min<int64_t>(n_probes, n_lists);
+  std::partial_sort(pad.begin(), pad.begin() + m, pad.end(), std::greater<int64_t>());
+  int64_t rows = 0;
+  for (int64_t i = 0; i < m; ++i) rows += pad[i];
+  return rows;
+}
+
+int64_t large_k_budget(const char* env_name)
+{
+  if (const char* e = getenv(env_name)) return std::max<int64_t>(1, atoll(e)) << 20;
+  size_t free_b = 0, total_b = 0;
+  B2_CUDA(cudaMemGetInfo(&free_b, &total_b));
+  return std::min<int64_t>(int64_t(8) << 30, static_cast<int64_t>(free_b / 2));
 }
 
 bool merge_probe_candidates(cudaStream_t s, const float* cs, const uint32_t* cp, const uint32_t* slot_of, const float* add,

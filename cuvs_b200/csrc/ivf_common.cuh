@@ -13,6 +13,7 @@
 // 128 probing queries instead of once per query.
 #pragma once
 #include "common.hpp"
+#include "ivf_lists.cuh"
 #include "scan_tc.cuh"
 
 #include <cuda_bf16.h>
@@ -85,6 +86,23 @@ void gather_probe_candidates(cudaStream_t s, const float* cs, const uint32_t* cp
 bool merge_probe_candidates(cudaStream_t s, const float* cs, const uint32_t* cp, const uint32_t* slot_of, const float* add,
                             float scale, const int* bound_keys, int64_t nq, int n_probes, int KCW, int k, float* out_val,
                             uint32_t* out_pos);
+
+/**
+ * k > 64 (IVF-Flat and IVF-PQ, DESIGN.md §4 and §5): dense per-pair score segments.  Live slot i, a pair of list l, owns
+ * scores[seg_off[i] .. + padded size of l): its list's rows in list order.  seg_len[i] is the list's real size (the padding
+ * rows at its end are never selected) and seg_base[i] its first index row, so column c of the segment is index row
+ * seg_base[i] + c.  Slots past the live count get seg_len 0.  All three arrays hold pb.n_pairs entries.
+ */
+void pair_segments(cudaStream_t s, const probe_buckets& pb, const list_layout& lists, int64_t* seg_off, uint32_t* seg_len,
+                   uint32_t* seg_base);
+/** Points every work item's out_off at the segment of its first slot; a store scan with a per-item row stride (n_tiles x 128)
+ *  then writes each pair's scores into its own segment. */
+void item_segments(cudaStream_t s, probe_buckets& pb, const int64_t* seg_off);
+/** Upper bound on the dense score rows of one query: the sum of the n_probes largest padded lists. */
+int64_t large_k_rows_per_query(const list_layout& lists, uint32_t n_probes);
+/** Bytes of workspace one k > 64 query batch may take: min(8 GiB, half of the free device memory), or `env_name` (MiB),
+ *  read on every call, when it is set. */
+int64_t large_k_budget(const char* env_name);
 
 /**
  * Balanced-ish Lloyd k-means on the device (fp32 data, wgmma assignment).  `centers` [k, d] is

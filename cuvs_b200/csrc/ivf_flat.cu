@@ -11,7 +11,10 @@
 //   1. coarse: dense wgmma score block queries x centres (split-bf16, fp32-grade) + select_k(n_probes)
 //   2. (query, probe) pairs are bucketed by list on the device (ivf_common.cu)
 //   3. fine:   per (list, <=128 probing queries) work item, wgmma scan of the list's bf16 rows with the
-//              fused top-k' epilogue — each list tile is read once per 128 probing queries, not once per query
+//              fused top-k' epilogue — each list tile is read once per 128 probing queries, not once per query.
+//              k > 64: the same scan with the store epilogue writes every (pair, list row) score to the pair's dense
+//              segment, and a segmented select keeps each pair's kc2 = min(2k, 2048) best (the reference's non-fused
+//              formulation, ivf_flat_search.cuh:238-295)
 //   4. per query: gather the candidates of its probes, keep the best few by approximate score, re-score
 //      them exactly in fp32 (sum (q-x)^2 / q.x — the reference's fine-scan arithmetic) and emit ids.
 #include "common.hpp"
@@ -97,6 +100,13 @@ __global__ void half_norms_filtered_kernel(const float* __restrict__ xn, const i
   const int64_t id = ids[i];
   const bool keep  = id >= 0 && id < n_bits && ((bits[id >> 5] >> (id & 31)) & 1u);
   hn[i]            = keep ? (zero ? 0.f : 0.5f * xn[i]) : INFINITY;
+}
+
+// k > 64: candidates whose scan score is not finite (rows hidden by the filter) become empty slots of the re-score
+__global__ void drop_nonfinite_kernel(const float* __restrict__ score, uint32_t* __restrict__ pos, int64_t n)
+{
+  int64_t i = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x;
+  if (i < n && !isfinite(score[i])) pos[i] = 0xffffffffu;
 }
 
 // positions of old rows in the new layout (same order inside each list)
@@ -282,16 +292,26 @@ void ivf_flat_search(resources* res, const ivf_flat_index& idx, uint32_t n_probe
   const int k      = static_cast<int>(nt.shape[1]);
   B2_EXPECTS(qt.shape[1] == idx.dim, "queries dim (%lld) != index dim (%d)", (long long)qt.shape[1], idx.dim);
   B2_EXPECTS(nt.shape[0] == nq && dt.shape[0] == nq && dt.shape[1] == k, "neighbors/distances shape mismatch");
-  B2_EXPECTS(k >= 1 && k <= 64, "ivf_flat search: k must be in [1, 64] in this build (got %d)", k);
+  B2_EXPECTS(k >= 1 && k <= kSelectMaxK, "ivf_flat search: k must be in [1, %d] (got %d)", kSelectMaxK, k);
   B2_EXPECTS(n_probes >= 1, "n_probes must be >= 1");
   if (nq == 0) return;
   n_probes         = std::min<uint32_t>(n_probes, idx.n_lists);
+  // k > 64 (DESIGN.md §4 "k > 64"): the scan stores every (pair, list row) score and a segmented select keeps kc2 per pair
+  const bool large_k = k > 64;
+  const int large_kc = std::min(2 * k, kSelectMaxK);
   {
     // Query batching: the per-(query, probe) workspaces (gathered bf16 query rows, 2 x KC candidate slots, their per-query
     // concatenation) are bounded to ~3 GiB; slots are uint32, so nq * n_probes also stays below 2^31 per batch.
     const int64_t per_query = static_cast<int64_t>(n_probes) * (idx.Kp * 2 + 2 * 64 * 8 + 16);
     int64_t batch = std::max<int64_t>(1, (int64_t(3) << 30) / per_query);
     batch         = std::min<int64_t>(batch, (int64_t(1) << 31) / std::max<uint32_t>(n_probes, 1));
+    if (large_k) {
+      // per query: dense scores (bounded by its n_probes largest lists), each pair's kc2 best and their per-query gather
+      // (8 + 8 bytes each), the gathered bf16 query rows, slot bookkeeping (32 bytes per pair) and the merged kc2
+      const int64_t per_q = large_k_rows_per_query(idx.lists, n_probes) * 4 +
+                            static_cast<int64_t>(n_probes) * (16 * large_kc + 2 * idx.Kp + 32) + static_cast<int64_t>(large_kc) * 8;
+      batch = std::min<int64_t>(batch, std::max<int64_t>(1, large_k_budget("CUVS_B200_FLAT_LARGE_K_BUDGET_MB") / per_q));
+    }
     if (nq > batch) {
       for (int64_t q0 = 0; q0 < nq; q0 += batch) {
         const int64_t rows = std::min(batch, nq - q0);
@@ -339,11 +359,12 @@ void ivf_flat_search(resources* res, const ivf_flat_index& idx, uint32_t n_probe
   // between k and the per-list capacity (and the shared pruning bound, which tracks the KC-th best): a true top-k row whose
   // bf16 score ranks a few places late must still be a candidate.  k <= 10 -> 16 slots, k <= 32 -> 32 slots; the bound is
   // only used when KC >= 1.5 k.
-  const int KC    = (k + k / 2 <= 16) ? 16 : 32;
-  const bool use_bound = KC >= k + k / 2;
+  // k > 64: no fused top-k (KC = 0, the store epilogue); each pair keeps its kc2 best from its dense score segment.
+  const int KC    = large_k ? 0 : ((k + k / 2 <= 16) ? 16 : 32);
+  const bool use_bound = !large_k && KC >= k + k / 2;
   const int lists = tc_lists_per_item();
-  const int KCW   = KC * lists;
-  B2_EXPECTS(KCW >= k, "ivf_flat search: k = %d needs the two-list tensor-core epilogue (CUVS_B200_TC_EPIW=8)", k);
+  int KCW         = KC * lists;
+  B2_EXPECTS(large_k || KCW >= k, "ivf_flat search: k = %d needs the two-list tensor-core epilogue (CUVS_B200_TC_EPIW=8)", k);
   probe_buckets pb;
   bucket_probes(res, probes.data(), nq, static_cast<int>(n_probes), idx.n_lists, idx.lists.d_offsets.data(), KCW, pb);
 
@@ -351,9 +372,31 @@ void ivf_flat_search(resources* res, const ivf_flat_index& idx, uint32_t n_probe
   const int64_t a_rows = pb.n_pairs + 128;
   dbuf<__nv_bfloat16> a_hi(static_cast<size_t>(a_rows) * idx.Kp, s);
   gather_rows_bf16(s, qp.hi.data(), pb.pair_query.data(), pb.n_items.data() + 1, a_rows, idx.Kp, a_hi.data());
-  dbuf<float> cs(static_cast<size_t>(pb.n_pairs) * KCW, s);
-  dbuf<uint32_t> cp(static_cast<size_t>(pb.n_pairs) * KCW, s);
-  {
+  dbuf<float> cs;
+  dbuf<uint32_t> cp;
+  if (large_k) {
+    // every (pair, list row) score goes to the pair's dense segment; per pair, its kc2 best rows (positions are index rows,
+    // ties go to the smaller row).  seg_len is the list's real size, so padding rows are never selected.
+    const int64_t n_pairs = pb.n_pairs;
+    dbuf<int64_t> seg_off(static_cast<size_t>(n_pairs), s);
+    dbuf<uint32_t> seg_len(static_cast<size_t>(n_pairs), s), seg_base(static_cast<size_t>(n_pairs), s);
+    pair_segments(s, pb, idx.lists, seg_off.data(), seg_len.data(), seg_base.data());
+    dbuf<float> scores(static_cast<size_t>(std::max<int64_t>(1, nq * large_k_rows_per_query(idx.lists, n_probes))), s);
+    item_segments(s, pb, seg_off.data());
+    {
+      timed_section ts("ivf_flat_scan", s);
+      tc_scan_topk(s, res->device, a_hi.data(), nullptr, a_rows, idx.hi.data(), nullptr, std::max<int64_t>(idx.lists.rows_total, 128),
+                   idx.Kp, hx, pb.items.data(), pb.max_items, pb.n_items.data(), 0, 1, scores.data(), nullptr, 0 /*per item*/);
+    }
+    int64_t max_len = 0;
+    for (int64_t v : idx.lists.h_sizes) max_len = std::max(max_len, v);
+    KCW = large_kc;
+    cs.alloc(static_cast<size_t>(n_pairs) * KCW, s);
+    cp.alloc(static_cast<size_t>(n_pairs) * KCW, s);
+    select_k_segments(s, scores.data(), seg_off.data(), seg_len.data(), seg_base.data(), n_pairs, max_len, KCW, cs.data(), cp.data(), true);
+  } else {
+    cs.alloc(static_cast<size_t>(pb.n_pairs) * KCW, s);
+    cp.alloc(static_cast<size_t>(pb.n_pairs) * KCW, s);
     // probes of one query share a running k'-th-best bound (same query => comparable scores)
     dbuf<int> bkeys(static_cast<size_t>(nq), s);
     B2_CUDA(cudaMemsetAsync(bkeys.data(), tc_bound_init_byte, sizeof(int) * nq, s));
@@ -370,10 +413,17 @@ void ivf_flat_search(resources* res, const ivf_flat_index& idx, uint32_t n_probe
   dbuf<float> gs(static_cast<size_t>(nq) * cand_w, s);
   dbuf<uint32_t> gp(static_cast<size_t>(nq) * cand_w, s);
   gather_probe_candidates(s, cs.data(), cp.data(), pb.slot_of.data(), nq, static_cast<int>(n_probes), KCW, gs.data(), gp.data());
-  const int kc2 = static_cast<int>(std::min<int64_t>(cand_w, std::max(32, 2 * k)));
+  const int kc2 = static_cast<int>(std::min<int64_t>(cand_w, large_k ? large_kc : std::max(32, 2 * k)));
   dbuf<float> ms(static_cast<size_t>(nq) * kc2, s);
   dbuf<uint32_t> mp(static_cast<size_t>(nq) * kc2, s);
   select_k(s, gs.data(), gp.data(), IDX_U32, nq, cand_w, cand_w, kc2, ms.data(), mp.data(), IDX_U32, true);
+  if (large_k) {
+    // a row hidden by the bitset filter scores +inf in the store scan but keeps its position, and the segmented select returns
+    // it whenever a pair holds fewer than kc2 kept rows: empty such slots before the exact re-score computes its true distance
+    count_launch();
+    drop_nonfinite_kernel<<<blocks_for(nq * kc2, 256), 256, 0, s>>>(ms.data(), mp.data(), nq * kc2);
+    B2_CUDA(cudaGetLastError());
+  }
   cuvsDistanceType fine = idx.metric == InnerProduct ? InnerProduct : (idx.metric == CosineExpanded ? CosineExpanded : L2Unexpanded);
   rescore_topk(s, q, nq, idx.dim, idx.data.data(), idx.dim, idx.dim, qn.data(), idx.xn.data(), fine, mp.data(), nullptr, kc2,
                idx.ids.data(), k, out_idx, out_dist, INT64_MAX, approx_map{}, nullptr, nullptr);

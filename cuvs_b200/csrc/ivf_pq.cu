@@ -398,52 +398,6 @@ __global__ void finish_ids_kernel(const uint32_t* __restrict__ pos, const int64_
   dist[i] = d;
 }
 
-// ---- k > 64: dense per-pair score segments (DESIGN.md §5 "k > 64")
-// Slot i (a live pair of list l) owns scores[seg_off[i] .. + padded size of l): its list's rows in list order.  seg_len is the
-// list's real size (the padding rows at its end are never selected) and seg_base its first index row, so that a column c of
-// the segment is index row seg_base + c.  Slots are few (nq * n_probes): one CTA scans them, each thread a contiguous chunk.
-__global__ void __launch_bounds__(1024) pair_segments_kernel(const uint32_t* __restrict__ pair_list, const int* __restrict__ n_live,
-                                                             int64_t n_pairs, const int64_t* __restrict__ list_offsets,
-                                                             const uint32_t* __restrict__ list_sizes, int64_t* __restrict__ seg_off,
-                                                             uint32_t* __restrict__ seg_len, uint32_t* __restrict__ seg_base)
-{
-  __shared__ int64_t part[1024];
-  const int tid      = threadIdx.x;
-  const int64_t live = *n_live;
-  const int64_t per  = (n_pairs + 1023) / 1024;
-  const int64_t b = min(n_pairs, tid * per), e = min(n_pairs, b + per);
-  int64_t sum = 0;
-  for (int64_t i = b; i < min(e, live); ++i) sum += list_offsets[pair_list[i] + 1] - list_offsets[pair_list[i]];
-  part[tid] = sum;
-  __syncthreads();
-  for (int o = 1; o < 1024; o <<= 1) {
-    const int64_t v = tid >= o ? part[tid - o] : 0;
-    __syncthreads();
-    part[tid] += v;
-    __syncthreads();
-  }
-  int64_t run = part[tid] - sum;
-  for (int64_t i = b; i < e; ++i) {
-    seg_off[i] = run;
-    if (i < live) {
-      const uint32_t l = pair_list[i];
-      seg_len[i]       = list_sizes[l];
-      seg_base[i]      = static_cast<uint32_t>(list_offsets[l]);
-      run += list_offsets[l + 1] - list_offsets[l];
-    } else {
-      seg_len[i]  = 0;
-      seg_base[i] = 0;
-    }
-  }
-}
-
-// the stream kernel's store epilogue writes an item's pairs from the segment of its first slot on
-__global__ void item_segments_kernel(tc_item* __restrict__ items, const int* __restrict__ n_items, const int64_t* __restrict__ seg_off)
-{
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < *n_items) items[i].out_off = static_cast<uint64_t>(seg_off[items[i].a_row0]);
-}
-
 // ---- LUT scan: one CTA per (query, probe) slot ------------------------------------------------
 constexpr int kLutThreads = 128;
 constexpr int kLutBuf     = 256;  // candidate buffer (entries) per CTA
@@ -927,28 +881,6 @@ ivf_pq_index* ivf_pq_build(resources* res, const cuvsIvfPqIndexParams& p, const 
   return idx.release();
 }
 
-// k > 64: upper bound on the dense score rows of one query, the sum of the n_probes largest padded lists
-int64_t large_k_rows_per_query(const ivf_pq_index& idx, uint32_t n_probes)
-{
-  std::vector<int64_t> pad(idx.n_lists);
-  for (uint32_t l = 0; l < idx.n_lists; ++l) pad[l] = idx.lists.h_offsets[l + 1] - idx.lists.h_offsets[l];
-  const uint32_t m = std::min<uint32_t>(n_probes, idx.n_lists);
-  std::partial_sort(pad.begin(), pad.begin() + m, pad.end(), std::greater<int64_t>());
-  int64_t rows = 0;
-  for (uint32_t i = 0; i < m; ++i) rows += pad[i];
-  return rows;
-}
-
-// k > 64: bytes of workspace one query batch may take (dense scores + per-pair top-k + merge buffers).  Default min(8 GiB, half
-// of the free device memory); CUVS_B200_PQ_LARGE_K_BUDGET_MB overrides it (read per call).
-int64_t large_k_budget()
-{
-  if (const char* e = getenv("CUVS_B200_PQ_LARGE_K_BUDGET_MB")) return std::max<int64_t>(1, atoll(e)) << 20;
-  size_t free_b = 0, total_b = 0;
-  B2_CUDA(cudaMemGetInfo(&free_b, &total_b));
-  return std::min<int64_t>(int64_t(8) << 30, static_cast<int64_t>(free_b / 2));
-}
-
 // The fine scan of one search (DESIGN.md §5), decided in one place before any work is queued.  env is CUVS_B200_PQ_PATH: lut,
 // tc (the default choice) or stream, read on every search because tests switch paths inside one process.  reduced: lut_dtype or
 // internal_distance_dtype is not fp32.  dense: the index also caches decoded rows, k <= 32, env != stream and the batch sends
@@ -1082,8 +1014,8 @@ void ivf_pq_search(resources* res, const ivf_pq_index& idx, const cuvsIvfPqSearc
     if (k > 64) {
       // k > 64: dense scores (bounded per query by its n_probes largest lists), per-pair top-k and the merge's gathered
       // candidates (8 bytes each), residual rows and slot bookkeeping, under the workspace budget
-      const int64_t per_q = large_k_rows_per_query(idx, n_probes) * 4 + static_cast<int64_t>(n_probes) * (16 * k + 4 * idx.Kp + 48);
-      batch = std::min<int64_t>(batch, std::max<int64_t>(1, large_k_budget() / per_q));
+      const int64_t per_q = large_k_rows_per_query(idx.lists, n_probes) * 4 + static_cast<int64_t>(n_probes) * (16 * k + 4 * idx.Kp + 48);
+      batch = std::min<int64_t>(batch, std::max<int64_t>(1, large_k_budget("CUVS_B200_PQ_LARGE_K_BUDGET_MB") / per_q));
     }
     if (nq > batch) {
       for (int64_t q0 = 0; q0 < nq; q0 += batch) {
@@ -1122,11 +1054,8 @@ void ivf_pq_search(resources* res, const ivf_pq_index& idx, const cuvsIvfPqSearc
     seg_off.alloc(static_cast<size_t>(n_pairs), s);
     seg_len.alloc(static_cast<size_t>(n_pairs), s);
     seg_base.alloc(static_cast<size_t>(n_pairs), s);
-    count_launch();
-    pair_segments_kernel<<<1, 1024, 0, s>>>(pb.pair_list.data(), pb.n_items.data() + 1, n_pairs, idx.lists.d_offsets.data(),
-                                            idx.lists.d_sizes.data(), seg_off.data(), seg_len.data(), seg_base.data());
-    B2_CUDA(cudaGetLastError());
-    scores.alloc(static_cast<size_t>(std::max<int64_t>(1, nq * large_k_rows_per_query(idx, n_probes))), s);
+    pair_segments(s, pb, idx.lists, seg_off.data(), seg_len.data(), seg_base.data());
+    scores.alloc(static_cast<size_t>(std::max<int64_t>(1, nq * large_k_rows_per_query(idx.lists, n_probes))), s);
   }
   // per pair: its KCW candidates (store: its k best, from the segmented select below)
   dbuf<float> cs;
@@ -1146,11 +1075,7 @@ void ivf_pq_search(resources* res, const ivf_pq_index& idx, const cuvsIvfPqSearc
   } else {
     residual_rows a;
     scale = pair_residual_rows(s, idx, q_rot.data(), pb, plan, a, add);
-    if (plan.store) {
-      count_launch();
-      item_segments_kernel<<<blocks_for(pb.max_items, 256), 256, 0, s>>>(pb.items.data(), pb.n_items.data(), seg_off.data());
-      B2_CUDA(cudaGetLastError());
-    }
+    if (plan.store) item_segments(s, pb, seg_off.data());
     // probes of one query share a running bound on its k'-th best DISTANCE: d = add[slot] + scale * s
     if (k <= plan.KC) {  // the bound tracks a k-th best out of KC kept entries
       bkeys.alloc(static_cast<size_t>(nq), s);

@@ -72,7 +72,8 @@ struct cfg {
 
 // KC > 0: fused top-KC epilogue, two candidate lists per (item, query row) — one per 64-column half of the tiles.
 // KC == 0: "store" epilogue — every score of the tile is written to
-// out_score[out_off + row * out_row_stride + (column within the item's range)] (dense distance block).
+// out_score[out_off + row * out_row_stride + (column within the item's range)] (dense distance block); out_row_stride == 0
+// stands for the item's own width, n_tiles * 128.
 template <int KB, int PASSES, int KC>
 __global__ void __launch_bounds__(128 + kEpiThreads, 1)
 tc_scan_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant__ CUtensorMap tmA_lo,
@@ -301,7 +302,9 @@ tc_scan_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
       for (int it = next_item(); it >= 0; it = next_item()) {
         const tc_item item = items[it];
         begin_item();
-        float* orow        = out_score + item.out_off + static_cast<int64_t>(row) * out_row_stride + col0;
+        // out_row_stride == 0: the item's rows are back to back, one n_tiles x 128 run each (per-pair score segments)
+        const int64_t stride = out_row_stride != 0 ? out_row_stride : static_cast<int64_t>(item.n_tiles) * 128;
+        float* orow        = out_score + item.out_off + static_cast<int64_t>(row) * stride + col0;
         const bool live    = static_cast<uint32_t>(row) < item.valid_rows;
         for (uint32_t t = 0; t < item.n_tiles; ++t) {
           uint32_t v0[32], v1[32];

@@ -76,6 +76,8 @@ void tc_pack_half_norms(cudaStream_t stream, const float* hn, int64_t rows_pad, 
  * bf16 numbers, e.g. decoded PQ rows), 1 uses hi*hi.
  * KC must be 16 or 32 — or 0 for the dense "store" epilogue: all scores of the item are written to
  * out_score[out_off + r * out_row_stride + j], j = column offset inside the item's row range (out_pos unused).
+ * out_row_stride == 0 (store only) makes the stride each item's own width, n_tiles * 128: the item's rows are written back
+ * to back, as the per-pair score segments of an IVF search need (item_segments).
  * With KC > 0 and out_score == null nothing is written (a bound warm-up pass: only `bound` is updated).
  * `dynamic_schedule`: items are handed to CTAs through a global counter (adjacent items — e.g. the query groups of one
  * IVF list — run at the same time on different SMs and share the list's tiles through L2); false = static round-robin.
