@@ -14,7 +14,8 @@
 //              fused top-k' epilogue — each list tile is read once per 128 probing queries, not once per query.
 //              k > 64: the same scan with the store epilogue writes every (pair, list row) score to the pair's dense
 //              segment, and a segmented select keeps each pair's kc2 = min(2k, 2048) best (the reference's non-fused
-//              formulation, ivf_flat_search.cuh:238-295)
+//              formulation, ivf_flat_search.cuh:238-295).  32 < k <= 64: a certificate sends the queries whose column-half
+//              lists of 32 may have dropped a candidate through that path as well (step 5)
 //   4. per query: gather the candidates of its probes, keep the best few by approximate score, re-score
 //      them exactly in fp32 (sum (q-x)^2 / q.x — the reference's fine-scan arithmetic) and emit ids.
 #include "common.hpp"
@@ -84,6 +85,49 @@ __global__ void drop_nonfinite_kernel(const float* __restrict__ score, uint32_t*
 {
   int64_t i = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x;
   if (i < n && !isfinite(score[i])) pos[i] = 0xffffffffu;
+}
+
+// 32 < k <= 64 certificate: each pair kept only the KC best rows of each column half of its list.  A half that came back full
+// may have dropped rows, all scoring no better than its last kept entry; when that entry is strictly better than the query's
+// kc2-th merged candidate, a dropped row could have made the cut, and the query is flagged (flags[nq] counts them).
+__global__ void flag_truncated_halves_kernel(const float* __restrict__ cs, const uint32_t* __restrict__ cp,
+                                             const uint32_t* __restrict__ slot_of, const float* __restrict__ ms, int64_t nq,
+                                             int n_probes, int KC, int KCW, int kc2, int* __restrict__ flags)
+{
+  int64_t q = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x;
+  if (q >= nq) return;
+  const float cut = ms[q * kc2 + kc2 - 1];
+  int flag        = 0;
+  for (int p = 0; p < n_probes && !flag; ++p) {
+    const uint32_t slot = slot_of[q * n_probes + p];
+    if (slot == 0xffffffffu) continue;
+    for (int h = KC - 1; h < KCW; h += KC) {
+      const int64_t e = static_cast<int64_t>(slot) * KCW + h;
+      if (cp[e] != 0xffffffffu && cs[e] < cut) flag = 1;
+    }
+  }
+  flags[q] = flag;
+  if (flag) atomicAdd(flags + nq, 1);
+}
+
+// dst[dst_row(i)] = src[src_row(i)] for rows of `width` elements; a null row map is the identity
+template <typename T>
+__global__ void copy_rows_kernel(const T* __restrict__ src, const int64_t* __restrict__ src_rows, T* __restrict__ dst,
+                                 const int64_t* __restrict__ dst_rows, int64_t n, int64_t width)
+{
+  int64_t t = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x;
+  if (t >= n * width) return;
+  const int64_t i = t / width, j = t % width;
+  dst[(dst_rows ? dst_rows[i] : i) * width + j] = src[(src_rows ? src_rows[i] : i) * width + j];
+}
+
+template <typename T>
+void copy_rows(cudaStream_t s, const T* src, const int64_t* src_rows, T* dst, const int64_t* dst_rows, int64_t n, int64_t width)
+{
+  if (n == 0) return;
+  count_launch();
+  copy_rows_kernel<T><<<blocks_for(n * width, 256), 256, 0, s>>>(src, src_rows, dst, dst_rows, n, width);
+  B2_CUDA(cudaGetLastError());
 }
 
 void refresh_tc_side(resources* res, ivf_flat_index& idx)
@@ -181,8 +225,9 @@ ivf_flat_index* ivf_flat_build(resources* res, const cuvsIvfFlatIndexParams& p, 
   return idx.release();
 }
 
+// store: take the k > 64 path at any k (the queries the 32 < k <= 64 certificate flags)
 void ivf_flat_search(resources* res, const ivf_flat_index& idx, uint32_t n_probes, const DLTensor& qt, const DLTensor& nt,
-                     const DLTensor& dt, const uint32_t* keep_bits = nullptr, int64_t n_bits = 0)
+                     const DLTensor& dt, const uint32_t* keep_bits = nullptr, int64_t n_bits = 0, bool store = false)
 {
   auto s           = res->stream;
   const int64_t nq = qt.shape[0];
@@ -194,7 +239,7 @@ void ivf_flat_search(resources* res, const ivf_flat_index& idx, uint32_t n_probe
   if (nq == 0) return;
   n_probes         = std::min<uint32_t>(n_probes, idx.n_lists);
   // k > 64 (DESIGN.md §4 "k > 64"): the scan stores every (pair, list row) score and a segmented select keeps kc2 per pair
-  const bool large_k = k > 64;
+  const bool large_k = k > 64 || store;
   const int large_kc = std::min(2 * k, kSelectMaxK);
   {
     // Query batching: the per-(query, probe) workspaces (gathered bf16 query rows, 2 x KC candidate slots, their per-query
@@ -213,7 +258,7 @@ void ivf_flat_search(resources* res, const ivf_flat_index& idx, uint32_t n_probe
       for (int64_t q0 = 0; q0 < nq; q0 += batch) {
         const int64_t rows = std::min(batch, nq - q0);
         dl_row_slice qs(qt, q0, rows), ns(nt, q0, rows), ds(dt, q0, rows);
-        ivf_flat_search(res, idx, n_probes, qs.t, ns.t, ds.t, keep_bits, n_bits);
+        ivf_flat_search(res, idx, n_probes, qs.t, ns.t, ds.t, keep_bits, n_bits, store);
       }
       return;
     }
@@ -326,6 +371,39 @@ void ivf_flat_search(resources* res, const ivf_flat_index& idx, uint32_t n_probe
                idx.ids.data(), k, out_idx, out_dist, INT64_MAX, approx_map{}, nullptr, nullptr);
   (void)select_min;
   postprocess_distances(s, out_dist, nq * k, idx.metric);
+
+  // ---- 5. 32 < k <= 64: queries whose pairs may have dropped a candidate (a full column half, flag_truncated_halves_kernel)
+  // are searched again on the store path, whose per-pair selection has no per-half limit.  k <= 32 keeps KC >= k per half.
+  if (large_k || k <= 32) return;
+  dbuf<int> flags(static_cast<size_t>(nq) + 1, s);
+  B2_CUDA(cudaMemsetAsync(flags.data() + nq, 0, sizeof(int), s));
+  count_launch();
+  flag_truncated_halves_kernel<<<blocks_for(nq, 256), 256, 0, s>>>(cs.data(), cp.data(), pb.slot_of.data(), ms.data(), nq,
+                                                                   static_cast<int>(n_probes), KC, KCW, kc2, flags.data());
+  B2_CUDA(cudaGetLastError());
+  std::vector<int> hflags(static_cast<size_t>(nq) + 1);
+  B2_CUDA(cudaMemcpyAsync(hflags.data(), flags.data(), sizeof(int) * (nq + 1), cudaMemcpyDeviceToHost, s));
+  B2_CUDA(cudaStreamSynchronize(s));
+  const int64_t n_flagged = hflags[nq];
+  set_last_flagged(static_cast<int>(n_flagged));
+  if (n_flagged == 0) return;
+  std::vector<int64_t> hrows;
+  hrows.reserve(static_cast<size_t>(n_flagged));
+  for (int64_t i = 0; i < nq; ++i)
+    if (hflags[i]) hrows.push_back(i);
+  dbuf<int64_t> rows(static_cast<size_t>(n_flagged), s);
+  B2_CUDA(cudaMemcpyAsync(rows.data(), hrows.data(), sizeof(int64_t) * n_flagged, cudaMemcpyHostToDevice, s));
+  dbuf<float> fq(static_cast<size_t>(n_flagged) * idx.dim, s), fd(static_cast<size_t>(n_flagged) * k, s);
+  dbuf<int64_t> fi(static_cast<size_t>(n_flagged) * k, s);
+  copy_rows(s, q, rows.data(), fq.data(), nullptr, n_flagged, idx.dim);
+  dl_row_slice sq(qt, 0, n_flagged), si(nt, 0, n_flagged), sd(dt, 0, n_flagged);
+  sq.t.data = fq.data();
+  si.t.data = fi.data();
+  sd.t.data = fd.data();
+  ivf_flat_search(res, idx, n_probes, sq.t, si.t, sd.t, keep_bits, n_bits, true);
+  copy_rows(s, fi.data(), nullptr, out_idx, rows.data(), n_flagged, k);
+  copy_rows(s, fd.data(), nullptr, out_dist, rows.data(), n_flagged, k);
+  B2_CUDA(cudaStreamSynchronize(s));  // hrows is host memory read by the copy above
 }
 
 }  // namespace

@@ -21,7 +21,7 @@
 //   lut      pq_lut_scan_kernel — the reference's formulation restated for H100: one CTA per (query, probe),
 //            LUT[pq_dim x 2^bits] in shared memory (fp32 / fp16 / fp_8bit<5>), codes read with 128-bit loads, scores
 //            accumulated in subspace order (bit-identical to oracle/oracle.c for fp32).  It serves the searches the other
-//            two do not (an index with neither, k > 64 without a code stream) and CUVS_B200_PQ_PATH=lut.
+//            two do not (an index with neither, k > 32 without a code stream) and CUVS_B200_PQ_PATH=lut.
 // Each keeps the k' best per (query, probe) in its epilogue for k <= 64.  For k > 64 the stream and LUT kernels store every
 // score to a dense per-pair segment instead, and a segmented select takes each pair's k best.  Either way the probes of a
 // query are then merged into its k best.
@@ -787,10 +787,10 @@ ivf_pq_index* ivf_pq_build(resources* res, const cuvsIvfPqIndexParams& p, const 
 //
 //                  k <= 64                                         k > 64 (store)
 //   stream         env != lut && code stream && !dense             env != lut && code stream
-//   decoded        not stream, env != lut && decoded rows          never
+//   decoded        not stream, env != lut && decoded rows, k <= 32 never
 //   lut            otherwise                                       otherwise
 //   passes         reduced ? 1 : 2                                 same
-//   KC             k <= 16 ? 16 : (k <= 32 or decoded ? 32 : 64)   0
+//   KC             k <= 16 ? 16 : (k <= 32 ? 32 : 64)              0
 //   KCW            KC x (decoded ? tc_lists_per_item() : 1)        0 to bucket_probes, k after the segment select
 //   group          stream ? pq_stream_group(pairs per list, KC, passes) : 128   same, with KC = 0
 //   pruning bound  tensor-core paths with k <= KC                  none
@@ -799,8 +799,9 @@ ivf_pq_index* ivf_pq_build(resources* res, const cuvsIvfPqIndexParams& p, const 
 // rows ARE bf16, so the scores equal the LUT sums to fp32 rounding.  A reduced-precision request takes one pass over the residual
 // rounded to bf16, the same class of approximation at tensor-core speed; lut forces the faithful LUT kernel (bit-level
 // emulation of the fp16 / fp_8bit<5> entries).  KCW: the decoded-row epilogue keeps one sorted list of KC per column half of
-// the tile; for k > KC the union of the two stands in for the pair's top-k (exact whenever no more than KC of them fall into
-// one half).  group: queries per work item, 128 for the query-major kernels; the stream kernel takes 32 / 64 / 128 from the
+// the tile, so it serves k <= KC = 32 only: for larger k the union of the two halves would lose the pair's true top-k
+// whenever more than 32 of them fall into one half, and an index without a code stream takes the LUT kernel (KC = 64).
+// group: queries per work item, 128 for the query-major kernels; the stream kernel takes 32 / 64 / 128 from the
 // average pairs per list.  store (k > 64, DESIGN.md §5 "k > 64"): the scan writes every (pair, list row) score to the pair's
 // dense segment and a segmented select takes each pair's k best; scores of one pair differ from its distances only by the
 // pair's `add` and a positive `scale`, so the per-pair order is the final one.
@@ -822,11 +823,11 @@ scan_plan plan_scan(const ivf_pq_index& idx, const cuvsIvfPqSearchParams& sp, in
   scan_plan p{};
   p.store = k > 64;
   if (!env_lut && idx.cstream.data() != nullptr && (p.store || !dense)) p.path = scan_path::stream;
-  else if (!env_lut && !p.store && idx.yhat.data() != nullptr) p.path = scan_path::decoded;
+  else if (!env_lut && k <= 32 && idx.yhat.data() != nullptr) p.path = scan_path::decoded;
   else p.path = scan_path::lut;
   const bool decoded = p.path == scan_path::decoded;
   p.passes = reduced ? 1 : 2;
-  p.KC     = p.store ? 0 : (k <= 16 ? 16 : (k <= 32 || decoded ? 32 : 64));
+  p.KC     = p.store ? 0 : (k <= 16 ? 16 : (k <= 32 ? 32 : 64));
   p.KCW    = p.KC * (decoded ? tc_lists_per_item() : 1);
   p.group  = p.path == scan_path::stream
                ? pq_stream_group(static_cast<double>(nq) * n_probes / std::max<uint32_t>(idx.n_lists, 1), p.KC, p.passes)

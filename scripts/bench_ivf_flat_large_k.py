@@ -6,8 +6,8 @@
 bench.py's ivf_flat workload: manifold data, 10M x 128, n_lists 4096, n_probes 64, batch 10k.  Searches at k in
 {10, 64, 100, 256, 1024}; every shape is run once before any timing.  Per case and round: ms per batch (CUDA events), the mean
 per-batch time of the `ivf_flat_scan` and `select_k_segments` sections (cuvsB200Timing*), the number of workspace batches the
-search split the 10k queries into (scan sections per search), and recall@k against exact ground truth on the first
-`--gt-queries` queries.  The whole set of cases is repeated `--rounds` times.  The card's name and power limit are read in the
+search split the 10k queries into (scan sections per search), recall@k against exact ground truth on the first
+`--gt-queries` queries, and for 32 < k <= 64 the share of queries the certificate sent to the store path (`flagged`).  The whole set of cases is repeated `--rounds` times.  The card's name and power limit are read in the
 same run.  Output: stdout and DIR/bench_ivf_flat_large_k.json.
 """
 from __future__ import annotations
@@ -124,6 +124,8 @@ def main():
         row = {"round": rnd, "k": k, "ms_per_batch": round(total / args.steps, 2), "ivf_flat_scan_ms": round(scan_ms / args.steps, 2),
                "select_k_segments_ms": round(sel_ms / args.steps, 2), "workspace_batches": scans // args.steps,
                f"recall@{k}": round(rec, 4)}
+        if 32 < k <= 64:
+            row["flagged"] = round(lib.cuvsB200LastFlagged() / args.nq, 4)
         print(json.dumps(row), flush=True)
         return row
 

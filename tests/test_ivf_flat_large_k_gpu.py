@@ -118,9 +118,9 @@ def test_large_k_matches_oracle(metric, d, k):
 @pytest.mark.parametrize("metric", ["sqeuclidean", "inner_product"])
 def test_first_64_of_k100_are_at_least_as_good_as_k64(metric):
     """The k = 100 search re-scores at least the k = 64 search's true top 64 in the same arithmetic: its j-th distance is never
-    worse, and almost always equal.  Uniform data over many small lists: a query's 64 nearest rows are spread over several
-    lists, so the k = 64 search's per-pair capacity (32 per column half of a list) is not the limit (on the clustered indexes
-    above most of them sit in one list, and the k = 100 search finds better rows in 4-7 % of the slots)."""
+    worse, and almost always equal.  Uniform data over many small lists, where a query's 64 nearest rows are spread over
+    several lists; tests/test_ivf_mid_k_gpu.py checks the same on clustered data, where most of them sit in one list and the
+    k = 64 search depends on its certificate sending such queries to the store path."""
     m = _mod()
     ds = uniform(30000, 32, 17)
     qs = uniform(200, 32, 18)
