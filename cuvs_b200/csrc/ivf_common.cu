@@ -252,27 +252,34 @@ __global__ void gather_rows_kernel(const uint4* __restrict__ src, const uint32_t
   dst[t] = val;
 }
 
+// out[q, p*KCW + c] = add[slot] + scale * s   (per-query concatenation of its probes' candidates; `empty` where there is none)
 __global__ void gather_cands_kernel(const float* __restrict__ cs, const uint32_t* __restrict__ cp,
-                                    const uint32_t* __restrict__ slot_of, int64_t total /*nq*n_probes*KC*/, int KC,
-                                    float* __restrict__ out_score, uint32_t* __restrict__ out_pos)
+                                    const uint32_t* __restrict__ slot_of, const float* __restrict__ add, float scale, float empty,
+                                    int64_t total, int KCW, float* __restrict__ out_score, uint32_t* __restrict__ out_pos)
 {
   int64_t t = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x;
   if (t >= total) return;
-  int64_t pair = t / KC;
-  int c        = static_cast<int>(t % KC);
+  int64_t pair  = t / KCW;
+  int c         = static_cast<int>(t % KCW);
   uint32_t slot = slot_of[pair];
-  float s      = INFINITY;
-  uint32_t p   = 0xffffffffu;
+  float s       = empty;
+  uint32_t p    = 0xffffffffu;
   if (slot != 0xffffffffu) {
-    s = cs[static_cast<int64_t>(slot) * KC + c];
-    p = cp[static_cast<int64_t>(slot) * KC + c];
+    // independent loads: the score is read before the position is known to be live
+    const int64_t e = static_cast<int64_t>(slot) * KCW + c;
+    p               = cp[e];
+    const float v   = cs[e];
+    const float a   = add ? add[slot] : 0.f;
+    if (p != 0xffffffffu) s = a + scale * v;
   }
   out_score[t] = s;
   out_pos[t]   = p;
 }
 
-// ---- k > 64: dense per-pair score segments (see pair_segments in ivf_common.cuh)
-// Slots are few (nq * n_probes): one CTA scans them, each thread a contiguous chunk.
+// ---- k > 64: dense per-pair score segments.  Live slot i, a pair of list l, owns scores[seg_off[i] .. + padded size of l):
+// its list's rows in list order.  seg_len[i] is the list's real size (the padding rows at its end are never selected) and
+// seg_base[i] its first index row, so column c of the segment is index row seg_base[i] + c.  Slots past the live count get
+// seg_len 0.  Slots are few (nq * n_probes): one CTA scans them, each thread a contiguous chunk.
 __global__ void __launch_bounds__(1024) pair_segments_kernel(const uint32_t* __restrict__ pair_list, const int* __restrict__ n_live,
                                                              int64_t n_pairs, const int64_t* __restrict__ list_offsets,
                                                              const uint32_t* __restrict__ list_sizes, int64_t* __restrict__ seg_off,
@@ -750,23 +757,34 @@ void gather_rows_bf16(cudaStream_t s, const __nv_bfloat16* src, const uint32_t* 
   B2_CUDA(cudaGetLastError());
 }
 
-void gather_probe_candidates(cudaStream_t s, const float* cs, const uint32_t* cp, const uint32_t* slot_of, int64_t nq,
-                             int n_probes, int KC, float* out_score, uint32_t* out_pos)
+void gather_probe_candidates(cudaStream_t s, const float* cs, const uint32_t* cp, const uint32_t* slot_of, const float* add,
+                             float scale, float empty, int64_t nq, int n_probes, int KCW, float* out_score, uint32_t* out_pos)
 {
-  const int64_t total = nq * n_probes * KC;
+  const int64_t total = nq * n_probes * KCW;
   if (total == 0) return;
   count_launch();
-  gather_cands_kernel<<<blocks_for(total, 256), 256, 0, s>>>(cs, cp, slot_of, total, KC, out_score, out_pos);
+  gather_cands_kernel<<<blocks_for(total, 256), 256, 0, s>>>(cs, cp, slot_of, add, scale, empty, total, KCW, out_score, out_pos);
   B2_CUDA(cudaGetLastError());
 }
 
-void pair_segments(cudaStream_t s, const probe_buckets& pb, const list_layout& lists, int64_t* seg_off, uint32_t* seg_len,
-                   uint32_t* seg_base)
+void large_k_select(cudaStream_t s, const probe_buckets& pb, const list_layout& lists, int64_t nq, uint32_t n_probes, int kp,
+                    const std::function<void(float* scores, const int64_t* seg_off)>& scan, dbuf<float>& cs,
+                    dbuf<uint32_t>& cp)
 {
+  const int64_t n_pairs = pb.n_pairs;
+  dbuf<int64_t> seg_off(static_cast<size_t>(n_pairs), s);
+  dbuf<uint32_t> seg_len(static_cast<size_t>(n_pairs), s), seg_base(static_cast<size_t>(n_pairs), s);
   count_launch();
-  pair_segments_kernel<<<1, 1024, 0, s>>>(pb.pair_list.data(), pb.n_items.data() + 1, pb.n_pairs, lists.d_offsets.data(),
-                                          lists.d_sizes.data(), seg_off, seg_len, seg_base);
+  pair_segments_kernel<<<1, 1024, 0, s>>>(pb.pair_list.data(), pb.n_items.data() + 1, n_pairs, lists.d_offsets.data(),
+                                          lists.d_sizes.data(), seg_off.data(), seg_len.data(), seg_base.data());
   B2_CUDA(cudaGetLastError());
+  dbuf<float> scores(static_cast<size_t>(std::max<int64_t>(1, nq * large_k_rows_per_query(lists, n_probes))), s);
+  scan(scores.data(), seg_off.data());
+  int64_t max_len = 0;
+  for (int64_t v : lists.h_sizes) max_len = std::max(max_len, v);
+  cs.alloc(static_cast<size_t>(n_pairs) * kp, s);
+  cp.alloc(static_cast<size_t>(n_pairs) * kp, s);
+  select_k_segments(s, scores.data(), seg_off.data(), seg_len.data(), seg_base.data(), n_pairs, max_len, kp, cs.data(), cp.data(), true);
 }
 
 void item_segments(cudaStream_t s, probe_buckets& pb, const int64_t* seg_off)
@@ -788,12 +806,35 @@ int64_t large_k_rows_per_query(const list_layout& lists, uint32_t n_probes)
   return rows;
 }
 
-int64_t large_k_budget(const char* env_name)
+int64_t query_batch_size(int64_t pair_bytes, uint32_t n_probes, int64_t large_k_query_bytes, const char* budget_env)
 {
-  if (const char* e = getenv(env_name)) return std::max<int64_t>(1, atoll(e)) << 20;
-  size_t free_b = 0, total_b = 0;
-  B2_CUDA(cudaMemGetInfo(&free_b, &total_b));
-  return std::min<int64_t>(int64_t(8) << 30, static_cast<int64_t>(free_b / 2));
+  int64_t batch = std::max<int64_t>(1, (int64_t(3) << 30) / (static_cast<int64_t>(n_probes) * pair_bytes));
+  batch         = std::min<int64_t>(batch, (int64_t(1) << 31) / std::max<uint32_t>(n_probes, 1));
+  if (large_k_query_bytes > 0) {
+    int64_t budget = 0;
+    if (const char* e = getenv(budget_env)) {
+      budget = std::max<int64_t>(1, atoll(e)) << 20;
+    } else {
+      size_t free_b = 0, total_b = 0;
+      B2_CUDA(cudaMemGetInfo(&free_b, &total_b));
+      budget = std::min<int64_t>(int64_t(8) << 30, static_cast<int64_t>(free_b / 2));
+    }
+    batch = std::min<int64_t>(batch, std::max<int64_t>(1, budget / large_k_query_bytes));
+  }
+  return batch;
+}
+
+bool search_in_batches(int64_t batch, const DLTensor& qt, const DLTensor& nt, const DLTensor& dt,
+                       const std::function<void(const DLTensor&, const DLTensor&, const DLTensor&)>& search)
+{
+  const int64_t nq = qt.shape[0];
+  if (nq <= batch) return false;
+  for (int64_t q0 = 0; q0 < nq; q0 += batch) {
+    const int64_t rows = std::min(batch, nq - q0);
+    dl_row_slice qs(qt, q0, rows), ns(nt, q0, rows), ds(dt, q0, rows);
+    search(qs.t, ns.t, ds.t);
+  }
+  return true;
 }
 
 dbuf<float> train_subsample(cudaStream_t s, const DLTensor& ds, uint32_t n_lists, double fraction, int64_t& n_train)

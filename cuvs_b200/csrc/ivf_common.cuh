@@ -18,6 +18,8 @@
 
 #include <cuda_bf16.h>
 
+#include <functional>
+
 namespace b200 {
 
 /** bf16 split planes + half-norms of a set of row vectors, padded to 128-row tiles (the "B side"). */
@@ -73,9 +75,12 @@ void bucket_probes(resources* res, const uint32_t* probes, int64_t nq, int n_pro
 void gather_rows_bf16(cudaStream_t s, const __nv_bfloat16* src, const uint32_t* pair_query, const int* n_live, int64_t rows_total,
                       int Kp, __nv_bfloat16* dst);
 
-/** Per query, concatenate the KC candidates of each of its probes: out [nq, n_probes*KC]. */
-void gather_probe_candidates(cudaStream_t s, const float* cs, const uint32_t* cp, const uint32_t* slot_of, int64_t nq,
-                             int n_probes, int KC, float* out_score, uint32_t* out_pos);
+/**
+ * Per query, concatenate the KCW candidates of each of its probes: out [nq, n_probes * KCW], value add[slot] + scale * score
+ * (add null: 0).  Empty entries, of a dropped pair or with position 0xffffffff, become (`empty`, 0xffffffff).
+ */
+void gather_probe_candidates(cudaStream_t s, const float* cs, const uint32_t* cp, const uint32_t* slot_of, const float* add,
+                             float scale, float empty, int64_t nq, int n_probes, int KCW, float* out_score, uint32_t* out_pos);
 
 /**
  * Per query: the k best (value, position) among its probes' candidates, value = add[slot] + scale * score, sorted
@@ -88,21 +93,31 @@ bool merge_probe_candidates(cudaStream_t s, const float* cs, const uint32_t* cp,
                             uint32_t* out_pos);
 
 /**
- * k > 64 (IVF-Flat and IVF-PQ, DESIGN.md §4 and §5): dense per-pair score segments.  Live slot i, a pair of list l, owns
- * scores[seg_off[i] .. + padded size of l): its list's rows in list order.  seg_len[i] is the list's real size (the padding
- * rows at its end are never selected) and seg_base[i] its first index row, so column c of the segment is index row
- * seg_base[i] + c.  Slots past the live count get seg_len 0.  All three arrays hold pb.n_pairs entries.
+ * Queries per batch of an IVF search (DESIGN.md §4a).  A (query, probe) pair's workspace takes `pair_bytes`; a batch's pairs
+ * stay within ~3 GiB and, slots being uint32, below 2^31.  k > 64 (`large_k_query_bytes` > 0, a query's workspace): a batch
+ * also stays within min(8 GiB, half of the free device memory), or within the env variable `budget_env` (MiB), read on every
+ * call, when it is set.
  */
-void pair_segments(cudaStream_t s, const probe_buckets& pb, const list_layout& lists, int64_t* seg_off, uint32_t* seg_len,
-                   uint32_t* seg_base);
+int64_t query_batch_size(int64_t pair_bytes, uint32_t n_probes, int64_t large_k_query_bytes = 0, const char* budget_env = nullptr);
+/** When nq > batch: runs `search` on the (queries, neighbors, distances) rows of each batch in turn and returns true. */
+bool search_in_batches(int64_t batch, const DLTensor& qt, const DLTensor& nt, const DLTensor& dt,
+                       const std::function<void(const DLTensor&, const DLTensor&, const DLTensor&)>& search);
+
+/**
+ * k > 64 (DESIGN.md §4a): the `kp` best rows of every pair.  Gives each live pair a dense segment of scores, one per row of
+ * its list in list order, and calls scan(scores, seg_off) to fill them (seg_off[slot]: the slot's segment; a tensor-core
+ * scan points its items there with item_segments).  Then a segmented select keeps each pair's kp best rows into cs / cp
+ * [n_pairs, kp] (positions are index rows, ties go to the smaller row, missing entries (FLT_MAX, 0xffffffff)), and the
+ * scores are released.
+ */
+void large_k_select(cudaStream_t s, const probe_buckets& pb, const list_layout& lists, int64_t nq, uint32_t n_probes, int kp,
+                    const std::function<void(float* scores, const int64_t* seg_off)>& scan, dbuf<float>& cs,
+                    dbuf<uint32_t>& cp);
 /** Points every work item's out_off at the segment of its first slot; a store scan with a per-item row stride (n_tiles x 128)
  *  then writes each pair's scores into its own segment. */
 void item_segments(cudaStream_t s, probe_buckets& pb, const int64_t* seg_off);
 /** Upper bound on the dense score rows of one query: the sum of the n_probes largest padded lists. */
 int64_t large_k_rows_per_query(const list_layout& lists, uint32_t n_probes);
-/** Bytes of workspace one k > 64 query batch may take: min(8 GiB, half of the free device memory), or `env_name` (MiB),
- *  read on every call, when it is set. */
-int64_t large_k_budget(const char* env_name);
 
 /**
  * Training rows of an IVF build: an evenly strided subsample of the rows of `ds` (fp32 [n, d], device or host), every

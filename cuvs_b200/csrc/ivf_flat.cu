@@ -241,32 +241,21 @@ void ivf_flat_search(resources* res, const ivf_flat_index& idx, uint32_t n_probe
   // k > 64 (DESIGN.md §4 "k > 64"): the scan stores every (pair, list row) score and a segmented select keeps kc2 per pair
   const bool large_k = k > 64 || store;
   const int large_kc = std::min(2 * k, kSelectMaxK);
-  {
-    // Query batching: the per-(query, probe) workspaces (gathered bf16 query rows, 2 x KC candidate slots, their per-query
-    // concatenation) are bounded to ~3 GiB; slots are uint32, so nq * n_probes also stays below 2^31 per batch.
-    const int64_t per_query = static_cast<int64_t>(n_probes) * (idx.Kp * 2 + 2 * 64 * 8 + 16);
-    int64_t batch = std::max<int64_t>(1, (int64_t(3) << 30) / per_query);
-    batch         = std::min<int64_t>(batch, (int64_t(1) << 31) / std::max<uint32_t>(n_probes, 1));
-    if (large_k) {
-      // per query: dense scores (bounded by its n_probes largest lists), each pair's kc2 best and their per-query gather
-      // (8 + 8 bytes each), the gathered bf16 query rows, slot bookkeeping (32 bytes per pair) and the merged kc2
-      const int64_t per_q = large_k_rows_per_query(idx.lists, n_probes) * 4 +
-                            static_cast<int64_t>(n_probes) * (16 * large_kc + 2 * idx.Kp + 32) + static_cast<int64_t>(large_kc) * 8;
-      batch = std::min<int64_t>(batch, std::max<int64_t>(1, large_k_budget("CUVS_B200_FLAT_LARGE_K_BUDGET_MB") / per_q));
-    }
-    if (nq > batch) {
-      for (int64_t q0 = 0; q0 < nq; q0 += batch) {
-        const int64_t rows = std::min(batch, nq - q0);
-        dl_row_slice qs(qt, q0, rows), ns(nt, q0, rows), ds(dt, q0, rows);
-        ivf_flat_search(res, idx, n_probes, qs.t, ns.t, ds.t, keep_bits, n_bits, store);
-      }
-      return;
-    }
-  }
+  // Query batching.  Per (query, probe) pair: the gathered bf16 query row, 2 x KC candidate slots and their per-query
+  // concatenation.  k > 64, per query: dense scores (bounded by its n_probes largest lists), each pair's kc2 best and their
+  // per-query gather (8 + 8 bytes each), the gathered bf16 query rows, slot bookkeeping (32 bytes per pair) and the merged kc2.
+  const int64_t large_k_bytes = !large_k ? 0
+                                         : large_k_rows_per_query(idx.lists, n_probes) * 4 +
+                                             static_cast<int64_t>(n_probes) * (16 * large_kc + 2 * idx.Kp + 32) +
+                                             static_cast<int64_t>(large_kc) * 8;
+  const int64_t batch = query_batch_size(idx.Kp * 2 + 2 * 64 * 8 + 16, n_probes, large_k_bytes, "CUVS_B200_FLAT_LARGE_K_BUDGET_MB");
+  if (search_in_batches(batch, qt, nt, dt, [&](const DLTensor& qs, const DLTensor& ns, const DLTensor& ds) {
+        ivf_flat_search(res, idx, n_probes, qs, ns, ds, keep_bits, n_bits, store);
+      }))
+    return;
   const float* q   = dl_ptr<float>(qt);
   int64_t* out_idx = dl_ptr<int64_t>(nt);
   float* out_dist  = dl_ptr<float>(dt);
-  const bool select_min = idx.metric != InnerProduct;
 
   // ---- 1. coarse
   dbuf<float> qn(static_cast<size_t>(nq), s);
@@ -317,25 +306,14 @@ void ivf_flat_search(resources* res, const ivf_flat_index& idx, uint32_t n_probe
   dbuf<float> cs;
   dbuf<uint32_t> cp;
   if (large_k) {
-    // every (pair, list row) score goes to the pair's dense segment; per pair, its kc2 best rows (positions are index rows,
-    // ties go to the smaller row).  seg_len is the list's real size, so padding rows are never selected.
-    const int64_t n_pairs = pb.n_pairs;
-    dbuf<int64_t> seg_off(static_cast<size_t>(n_pairs), s);
-    dbuf<uint32_t> seg_len(static_cast<size_t>(n_pairs), s), seg_base(static_cast<size_t>(n_pairs), s);
-    pair_segments(s, pb, idx.lists, seg_off.data(), seg_len.data(), seg_base.data());
-    dbuf<float> scores(static_cast<size_t>(std::max<int64_t>(1, nq * large_k_rows_per_query(idx.lists, n_probes))), s);
-    item_segments(s, pb, seg_off.data());
-    {
+    // every (pair, list row) score goes to the pair's dense segment; each pair keeps its kc2 best rows
+    large_k_select(s, pb, idx.lists, nq, n_probes, large_kc, [&](float* scores, const int64_t* seg_off) {
+      item_segments(s, pb, seg_off);
       timed_section ts("ivf_flat_scan", s);
       tc_scan_topk(s, res->device, a_hi.data(), nullptr, a_rows, idx.hi.data(), nullptr, std::max<int64_t>(idx.lists.rows_total, 128),
-                   idx.Kp, hx, pb.items.data(), pb.max_items, pb.n_items.data(), 0, 1, scores.data(), nullptr, 0 /*per item*/);
-    }
-    int64_t max_len = 0;
-    for (int64_t v : idx.lists.h_sizes) max_len = std::max(max_len, v);
+                   idx.Kp, hx, pb.items.data(), pb.max_items, pb.n_items.data(), 0, 1, scores, nullptr, 0 /*per item*/);
+    }, cs, cp);
     KCW = large_kc;
-    cs.alloc(static_cast<size_t>(n_pairs) * KCW, s);
-    cp.alloc(static_cast<size_t>(n_pairs) * KCW, s);
-    select_k_segments(s, scores.data(), seg_off.data(), seg_len.data(), seg_base.data(), n_pairs, max_len, KCW, cs.data(), cp.data(), true);
   } else {
     cs.alloc(static_cast<size_t>(pb.n_pairs) * KCW, s);
     cp.alloc(static_cast<size_t>(pb.n_pairs) * KCW, s);
@@ -354,7 +332,9 @@ void ivf_flat_search(resources* res, const ivf_flat_index& idx, uint32_t n_probe
   const int64_t cand_w = static_cast<int64_t>(n_probes) * KCW;
   dbuf<float> gs(static_cast<size_t>(nq) * cand_w, s);
   dbuf<uint32_t> gp(static_cast<size_t>(nq) * cand_w, s);
-  gather_probe_candidates(s, cs.data(), cp.data(), pb.slot_of.data(), nq, static_cast<int>(n_probes), KCW, gs.data(), gp.data());
+  // empty entries +inf: FLT_MAX made the ivf_flat bench search ~3 % slower (DESIGN.md §4a)
+  gather_probe_candidates(s, cs.data(), cp.data(), pb.slot_of.data(), nullptr, 1.0f, INFINITY, nq, static_cast<int>(n_probes), KCW, gs.data(),
+                          gp.data());
   const int kc2 = static_cast<int>(std::min<int64_t>(cand_w, large_k ? large_kc : std::max(32, 2 * k)));
   dbuf<float> ms(static_cast<size_t>(nq) * kc2, s);
   dbuf<uint32_t> mp(static_cast<size_t>(nq) * kc2, s);
@@ -369,7 +349,6 @@ void ivf_flat_search(resources* res, const ivf_flat_index& idx, uint32_t n_probe
   cuvsDistanceType fine = idx.metric == InnerProduct ? InnerProduct : (idx.metric == CosineExpanded ? CosineExpanded : L2Unexpanded);
   rescore_topk(s, q, nq, idx.dim, idx.data.data(), idx.dim, idx.dim, qn.data(), idx.xn.data(), fine, mp.data(), nullptr, kc2,
                idx.ids.data(), k, out_idx, out_dist, INT64_MAX, approx_map{}, nullptr, nullptr);
-  (void)select_min;
   postprocess_distances(s, out_dist, nq * k, idx.metric);
 
   // ---- 5. 32 < k <= 64: queries whose pairs may have dropped a candidate (a full column half, flag_truncated_halves_kernel)

@@ -321,26 +321,6 @@ __global__ void pair_rows_kernel(const float* __restrict__ q_rot, const float* _
   }
 }
 
-// out[q, p*KCW + c] = add[slot] + scale * s   (per-query concatenation of its probes' candidates)
-__global__ void gather_pq_cands_kernel(const float* __restrict__ cs, const uint32_t* __restrict__ cp,
-                                       const uint32_t* __restrict__ slot_of, const float* __restrict__ add, float scale,
-                                       int64_t total, int KCW, float* __restrict__ out_score, uint32_t* __restrict__ out_pos)
-{
-  int64_t t = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x;
-  if (t >= total) return;
-  int64_t pair  = t / KCW;
-  int c         = static_cast<int>(t % KCW);
-  uint32_t slot = slot_of[pair];
-  float s       = FLT_MAX;
-  uint32_t p    = 0xffffffffu;
-  if (slot != 0xffffffffu) {
-    p = cp[static_cast<int64_t>(slot) * KCW + c];
-    if (p != 0xffffffffu) s = (add ? add[slot] : 0.f) + scale * cs[static_cast<int64_t>(slot) * KCW + c];
-  }
-  out_score[t] = s;
-  out_pos[t]   = p;
-}
-
 __global__ void finish_ids_kernel(const uint32_t* __restrict__ pos, const int64_t* __restrict__ ids, float* __restrict__ dist,
                                   int64_t count, int metric, int64_t* __restrict__ out_idx)
 {
@@ -903,29 +883,18 @@ void ivf_pq_search(resources* res, const ivf_pq_index& idx, const cuvsIvfPqSearc
   B2_EXPECTS(sp.internal_distance_dtype == CUDA_R_32F || sp.internal_distance_dtype == CUDA_R_16F, "unsupported internal_distance_dtype");
   if (nq == 0) return;
   const uint32_t n_probes = std::min<uint32_t>(sp.n_probes, idx.n_lists);
-  {
-    // Query batching (ivf_pq_search.cuh:960-1010 loops over max_internal_batch_size): the per-(query, probe) workspaces
-    // below — residual rows (Kp bf16 per pass) and 2 x KC candidate slots — are bounded to ~3 GiB; a 10k x 48-probe batch
-    // needs 0.3 GiB and runs in one piece.  Slots are uint32: nq * n_probes must stay below 2^32 as well.
-    const int64_t per_query = static_cast<int64_t>(n_probes) * (2 * idx.Kp * 2 + 64 * 8 + 16);
-    int64_t batch = std::max<int64_t>(1, (int64_t(3) << 30) / per_query);
-    batch         = std::min<int64_t>(batch, (int64_t(1) << 31) / std::max<uint32_t>(n_probes, 1));
-    if (sp.max_internal_batch_size > 0 && n_probes > 256) batch = std::min<int64_t>(batch, std::max<uint32_t>(sp.max_internal_batch_size, 128));
-    if (k > 64) {
-      // k > 64: dense scores (bounded per query by its n_probes largest lists), per-pair top-k and the merge's gathered
-      // candidates (8 bytes each), residual rows and slot bookkeeping, under the workspace budget
-      const int64_t per_q = large_k_rows_per_query(idx.lists, n_probes) * 4 + static_cast<int64_t>(n_probes) * (16 * k + 4 * idx.Kp + 48);
-      batch = std::min<int64_t>(batch, std::max<int64_t>(1, large_k_budget("CUVS_B200_PQ_LARGE_K_BUDGET_MB") / per_q));
-    }
-    if (nq > batch) {
-      for (int64_t q0 = 0; q0 < nq; q0 += batch) {
-        const int64_t rows = std::min(batch, nq - q0);
-        dl_row_slice qs(qt, q0, rows), ns(nt, q0, rows), ds(dt, q0, rows);
-        ivf_pq_search(res, idx, sp, qs.t, ns.t, ds.t);
-      }
-      return;
-    }
-  }
+  // Query batching (ivf_pq_search.cuh:960-1010 loops over max_internal_batch_size).  Per (query, probe) pair: residual rows
+  // (Kp bf16 per pass) and 2 x KC candidate slots; a 10k x 48-probe batch needs 0.3 GiB and runs in one piece.  k > 64, per
+  // query: dense scores (bounded by its n_probes largest lists), per-pair top-k and the merge's gathered candidates (8 bytes
+  // each), residual rows and slot bookkeeping.
+  const int64_t large_k_bytes =
+    k <= 64 ? 0 : large_k_rows_per_query(idx.lists, n_probes) * 4 + static_cast<int64_t>(n_probes) * (16 * k + 4 * idx.Kp + 48);
+  int64_t batch = query_batch_size(2 * idx.Kp * 2 + 64 * 8 + 16, n_probes, large_k_bytes, "CUVS_B200_PQ_LARGE_K_BUDGET_MB");
+  if (sp.max_internal_batch_size > 0 && n_probes > 256) batch = std::min<int64_t>(batch, std::max<uint32_t>(sp.max_internal_batch_size, 128));
+  if (search_in_batches(batch, qt, nt, dt, [&](const DLTensor& qs, const DLTensor& ns, const DLTensor& ds) {
+        ivf_pq_search(res, idx, sp, qs, ns, ds);
+      }))
+    return;
   const float* q   = dl_ptr<float>(qt);
   int64_t* out_idx = dl_ptr<int64_t>(nt);
   float* out_dist  = dl_ptr<float>(dt);
@@ -946,36 +915,19 @@ void ivf_pq_search(resources* res, const ivf_pq_index& idx, const cuvsIvfPqSearc
   probe_buckets pb;
   bucket_probes(res, probes.data(), nq, static_cast<int>(n_probes), idx.n_lists, idx.lists.d_offsets.data(), plan.KCW, pb, 0, 0xffffffffu,
                 plan.group);
-  const int64_t n_pairs = pb.n_pairs;
-  dbuf<int64_t> seg_off;
-  dbuf<uint32_t> seg_len, seg_base;
-  dbuf<float> scores;  // store: the dense segments
-  if (plan.store) {
-    seg_off.alloc(static_cast<size_t>(n_pairs), s);
-    seg_len.alloc(static_cast<size_t>(n_pairs), s);
-    seg_base.alloc(static_cast<size_t>(n_pairs), s);
-    pair_segments(s, pb, idx.lists, seg_off.data(), seg_len.data(), seg_base.data());
-    scores.alloc(static_cast<size_t>(std::max<int64_t>(1, nq * large_k_rows_per_query(idx.lists, n_probes))), s);
-  }
-  // per pair: its KCW candidates (store: its k best, from the segmented select below)
-  dbuf<float> cs;
-  dbuf<uint32_t> cp;
-  if (!plan.store) {
-    cs.alloc(static_cast<size_t>(n_pairs) * plan.KCW, s);
-    cp.alloc(static_cast<size_t>(n_pairs) * plan.KCW, s);
-  }
-  float* const scan_out = plan.store ? scores.data() : cs.data();
   dbuf<float> add;
   dbuf<int> bkeys;  // per-query pruning bound of the tensor-core scan (tc_bound), reused by the merge
   float scale = 1.0f;
-  if (plan.path == scan_path::lut) {
-    ensure_flat_codes(res, idx);
-    (plan.store ? launch_lut_scan<true> : launch_lut_scan<false>)(s, idx, sp, q_rot.data(), pb, plan.KC, scan_out, cp.data(), plan.KCW,
-                                                                  seg_off.data());
-  } else {
+  // out / out_pos: each pair's KCW candidates; store: the dense segments at seg_off (out_pos unused)
+  auto scan = [&](float* out, uint32_t* out_pos, const int64_t* seg_off) {
+    if (plan.path == scan_path::lut) {
+      ensure_flat_codes(res, idx);
+      (plan.store ? launch_lut_scan<true> : launch_lut_scan<false>)(s, idx, sp, q_rot.data(), pb, plan.KC, out, out_pos, plan.KCW, seg_off);
+      return;
+    }
     residual_rows a;
     scale = pair_residual_rows(s, idx, q_rot.data(), pb, plan, a, add);
-    if (plan.store) item_segments(s, pb, seg_off.data());
+    if (plan.store) item_segments(s, pb, seg_off);
     // probes of one query share a running bound on its k'-th best DISTANCE: d = add[slot] + scale * s
     if (k <= plan.KC) {  // the bound tracks a k-th best out of KC kept entries
       bkeys.alloc(static_cast<size_t>(nq), s);
@@ -990,23 +942,24 @@ void ivf_pq_search(resources* res, const ivf_pq_index& idx, const cuvsIvfPqSearc
     timed_section ts("pq_scan", s);
     if (plan.path == scan_path::stream)
       pq_stream_scan(s, res->device, a.hi.data(), a.lo.data(), a.rows, idx.Kp, idx.cstream.data(), idx.cb_words.data(), idx.pq_dim,
-                     pb.items.data(), pb.max_items, pb.n_items.data(), plan.group, plan.KC, plan.passes, scan_out, cp.data(), plan.KCW,
+                     pb.items.data(), pb.max_items, pb.n_items.data(), plan.group, plan.KC, plan.passes, out, out_pos, plan.KCW,
                      bkeys.data() ? &bnd : nullptr);
     else
       tc_scan_topk(s, res->device, a.hi.data(), a.lo.data(), a.rows, idx.yhat.data(), nullptr, std::max<int64_t>(idx.lists.rows_total, 128),
-                   idx.Kp, idx.hx.data(), pb.items.data(), pb.max_items, pb.n_items.data(), plan.KC, plan.passes, cs.data(), cp.data(),
+                   idx.Kp, idx.hx.data(), pb.items.data(), pb.max_items, pb.n_items.data(), plan.KC, plan.passes, out, out_pos,
                    plan.KCW, bkeys.data() ? &bnd : nullptr);
-  }
+  };
+  // per pair: its KCW candidates (store: its k best)
+  dbuf<float> cs;
+  dbuf<uint32_t> cp;
   int KCW = plan.KCW;
   if (plan.store) {
-    // per pair: its k best rows (positions are index rows); ties go to the smaller row
-    int64_t max_len = 0;
-    for (int64_t v : idx.lists.h_sizes) max_len = std::max(max_len, v);
-    cs.alloc(static_cast<size_t>(n_pairs) * k, s);
-    cp.alloc(static_cast<size_t>(n_pairs) * k, s);
-    select_k_segments(s, scores.data(), seg_off.data(), seg_len.data(), seg_base.data(), n_pairs, max_len, k, cs.data(), cp.data(), true);
-    scores.release();
+    large_k_select(s, pb, idx.lists, nq, n_probes, k, [&](float* scores, const int64_t* seg_off) { scan(scores, nullptr, seg_off); }, cs, cp);
     KCW = k;
+  } else {
+    cs.alloc(static_cast<size_t>(pb.n_pairs) * KCW, s);
+    cp.alloc(static_cast<size_t>(pb.n_pairs) * KCW, s);
+    scan(cs.data(), cp.data(), nullptr);
   }
 
   // ---- per query: concatenate its probes' candidates (in final distance units), top-k, ids
@@ -1017,9 +970,8 @@ void ivf_pq_search(resources* res, const ivf_pq_index& idx, const cuvsIvfPqSearc
                                KCW, k, out_dist, mp.data()))) {
     dbuf<float> gs(static_cast<size_t>(nq) * cand_w, s);
     dbuf<uint32_t> gp(static_cast<size_t>(nq) * cand_w, s);
-    count_launch();
-    gather_pq_cands_kernel<<<blocks_for(nq * cand_w, 256), 256, 0, s>>>(cs.data(), cp.data(), pb.slot_of.data(), add.data(), scale,
-                                                                         nq * cand_w, KCW, gs.data(), gp.data());
+    gather_probe_candidates(s, cs.data(), cp.data(), pb.slot_of.data(), add.data(), scale, FLT_MAX, nq, static_cast<int>(n_probes), KCW, gs.data(),
+                            gp.data());
     select_k(s, gs.data(), gp.data(), IDX_U32, nq, cand_w, cand_w, k, out_dist, mp.data(), IDX_U32, true);
   }
   count_launch();

@@ -11,13 +11,15 @@
     python scripts/ab_ivf_outputs.py {flat|pq} compare-builds DIR_A DIR_B [--by-id]
 
 Searches.  `build` writes seeded indexes to DIR, and both `run`s search the same files, so the comparison covers the search
-alone.  `run` writes one SHA-256 of the neighbours and distances per search, or "nondeterministic" when two runs of the search
-in the same process differ.  `compare` lists the searches whose results differ and counts those that are nondeterministic in
-either run.
+alone.  `run` writes, per search, one SHA-256 of the neighbours and distances and the number of kernels the library launched
+for it (cuvsB200KernelLaunches), or "nondeterministic" when two runs of the search in the same process differ in either.
+`compare` lists the searches whose results or launch counts differ and counts those that are nondeterministic in either run.
 * flat: dim 128 with 256 lists and dim 96 with 64 lists (the dense coarse select), dim 256 with 128 lists (the streamed-A scan
   kernel) and dim 64 with 4096 lists (the fused coarse select), each in L2, L2 with sqrt, inner product and cosine.  `run`
-  searches each at k in {10, 32, 64} (the fused top-k path; the optional KS, e.g. 100,1024, replaces that list), two batch
-  sizes, without and with a bitset filter that keeps 40 % of the rows.
+  searches each at k in {10, 32, 33, 48, 64, 65, 100, 1024, 2048} (the fused top-k path, the 32 < k <= 64 certificate and the
+  k > 64 store path; the optional KS, e.g. 100,1024, replaces that list), two batch sizes (only the smaller at k = 2048),
+  without and with a bitset filter that keeps 40 % of the rows, and k > 64 once more at the smaller batch under a 1 MB
+  workspace budget (CUVS_B200_FLAT_LARGE_K_BUDGET_MB) that splits it.
 * pq: indexes that reach every fine-scan path: code stream only; code stream + decoded-row cache (probed densely by the larger
   batch); per-cluster codebooks; pq_bits 5; conservative_memory_allocation, which keeps no decoded rows.  Each comes in L2,
   inner product and cosine.  `run` searches each with CUVS_B200_PQ_PATH unset / lut / stream, the LUT / distance dtypes
@@ -59,7 +61,7 @@ INDEXES = {
     },
 }
 METRICS = {"flat": ("sqeuclidean", "euclidean", "inner_product", "cosine"), "pq": ("sqeuclidean", "inner_product", "cosine")}
-KS = {"flat": (10, 32, 64), "pq": (10, 32, 33, 64, 65, 100, 2048)}
+KS = {"flat": (10, 32, 33, 48, 64, 65, 100, 1024, 2048), "pq": (10, 32, 33, 64, 65, 100, 2048)}
 PQ_DTYPES = {"f32": ("float32", "float32"), "f16": ("float16", "float32"), "u8": ("uint8", "float32"), "f16_f16": ("float16", "float16")}
 N_ROWS = 60_000
 WAYS = ("device", "host", "extend")
@@ -123,10 +125,26 @@ def build_files(kind, d):
                     _mod(kind).save(os.path.join(d, f"{metric}_{name}_{way}_{rep}.bin"), _build(kind, metric, name, way))
 
 
-def _digest(dist, i):
+def _launches():
+    import ctypes
+    from cuvs_b200._capi import lib
+    lib.cuvsB200KernelLaunches.restype = ctypes.c_longlong
+    return int(lib.cuvsB200KernelLaunches())
+
+
+def _record(search):
+    """-> "<SHA-256 of the distances and neighbours> launches=<kernel launches>" of search(), or "nondeterministic" when two
+    calls return different results.  The launches are the second call's: the first may also do one-time work, such as the
+    flat code layout the first LUT-kernel search of an IVF-PQ index builds."""
     import torch
-    torch.cuda.synchronize()
-    return hashlib.sha256(dist.cpu().numpy().tobytes() + i.cpu().numpy().tobytes()).hexdigest()
+    seen, n = set(), 0
+    for _ in range(2):
+        n0 = _launches()
+        dist, i = search()
+        torch.cuda.synchronize()
+        n = _launches() - n0
+        seen.add(hashlib.sha256(dist.cpu().numpy().tobytes() + i.cpu().numpy().tobytes()).hexdigest())
+    return f"{seen.pop()} launches={n}" if len(seen) == 1 else "nondeterministic"
 
 
 def _run_flat(d, ks):
@@ -144,10 +162,14 @@ def _run_flat(d, ks):
             sp = ivf_flat.SearchParams(n_probes=16)
             print(f"{metric} {name}", flush=True)
             for k in ks:
-                for nq in (300, 3000):
-                    for filtered in (False, True):
-                        h = {_digest(*ivf_flat.search(sp, idx, q[:nq], k, filter=bits if filtered else None)) for _ in range(2)}
-                        res[f"{metric}/{name}/k={k}/nq={nq}/filtered={filtered}"] = h.pop() if len(h) == 1 else "nondeterministic"
+                for nq in ((300,) if k == 2048 else (300, 3000)):
+                    for split in ((False, True) if k > 64 and nq == 300 else (False,)):
+                        _set_env("CUVS_B200_FLAT_LARGE_K_BUDGET_MB", "1" if split else None)
+                        for filtered in (False, True):
+                            f = bits if filtered else None
+                            key = f"{metric}/{name}/k={k}/nq={nq}/filtered={filtered}" + ("/split=True" if split else "")
+                            res[key] = _record(lambda: ivf_flat.search(sp, idx, q[:nq], k, filter=f))
+            _set_env("CUVS_B200_FLAT_LARGE_K_BUDGET_MB", None)
     return res
 
 
@@ -170,9 +192,8 @@ def _run_pq(d, ks):
                         for nq in ((300,) if k == 2048 else (300, 3000)):
                             for split in ((False, True) if k > 64 else (False,)):
                                 _set_env("CUVS_B200_PQ_LARGE_K_BUDGET_MB", "1" if split else None)
-                                h = {_digest(*ivf_pq.search(sp, idx, q[:nq], k)) for _ in range(2)}
                                 res[f"{metric}/{name}/path={env}/{dt}/k={k}/nq={nq}/split={split}"] = \
-                                    h.pop() if len(h) == 1 else "nondeterministic"
+                                    _record(lambda: ivf_pq.search(sp, idx, q[:nq], k))
             _set_env("CUVS_B200_PQ_PATH", None)
             _set_env("CUVS_B200_PQ_LARGE_K_BUDGET_MB", None)
     return res

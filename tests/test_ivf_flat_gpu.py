@@ -8,6 +8,7 @@ import pytest
 import torch
 
 import oracle
+from tests.ivf_oracle import flat_lists, flat_search
 from tests.util import clustered, launches, uniform
 
 pytestmark = pytest.mark.gpu
@@ -16,19 +17,6 @@ pytestmark = pytest.mark.gpu
 def _mod():
     from cuvs_b200.neighbors import ivf_flat
     return ivf_flat
-
-
-def _lists_of(index):
-    sizes = index.list_sizes.cpu().numpy().astype(np.int64)
-    ids = [index.list_indices(l).cpu().numpy() for l in range(index.n_lists)]
-    return sizes, ids
-
-
-def _oracle_search(index, ds, qs, n_probes, k, metric):
-    sizes, ids = _lists_of(index)
-    offsets = np.concatenate([[0], np.cumsum(sizes)])
-    all_ids = np.concatenate(ids) if len(ids) else np.zeros(0, np.int64)
-    return oracle.ivf_flat_search(index.centers.cpu().numpy(), offsets, ds[all_ids], all_ids, qs, n_probes, k, metric)
 
 
 @pytest.mark.parametrize("n,d,n_lists,n_probes,k,metric", [
@@ -45,9 +33,9 @@ def test_search_matches_oracle(n, d, n_lists, n_probes, k, metric):
     dist, idx = m.search(m.SearchParams(n_probes=n_probes), index, torch.from_numpy(qs).cuda(), k)
     assert launches() > l0
     dist, idx = dist.cpu().numpy(), idx.cpu().numpy()
-    sizes, ids = _lists_of(index)
-    assert sizes.sum() == n and sorted(np.concatenate(ids).tolist()) == list(range(n))
-    rd, ri = _oracle_search(index, ds, qs, n_probes, k, metric)
+    _, ids = flat_lists(index)
+    assert index.list_sizes.cpu().numpy().sum() == n and sorted(ids.tolist()) == list(range(n))
+    rd, ri = flat_search(index, ds, qs, n_probes, k, metric)
     # element-wise: same id, or an equal-distance tie (ann_utils.cuh:257-289)
     assert oracle.recall_with_ties(idx, dist, ri, rd, eps=1e-3) >= 0.999
     same = (idx == ri).mean()
@@ -116,11 +104,7 @@ def test_bitset_prefilter_equals_search_over_the_kept_rows():
     dist, idx = dist.cpu().numpy(), idx.cpu().numpy()
     valid = idx != np.iinfo(np.int64).max
     assert keep[idx[valid]].all(), "a filtered-out row was returned"
-    sizes, ids = _lists_of(index)
-    ids_f = [i[keep[i]] for i in ids]
-    offsets = np.concatenate([[0], np.cumsum([len(i) for i in ids_f])])
-    all_ids = np.concatenate(ids_f)
-    rd, ri = oracle.ivf_flat_search(index.centers.cpu().numpy(), offsets, ds[all_ids], all_ids, qs, 8, 10, "sqeuclidean")
+    rd, ri = flat_search(index, ds, qs, 8, 10, "sqeuclidean", keep)
     assert oracle.recall_with_ties(idx, dist, ri, rd, eps=1e-3) >= 0.999
 
 
@@ -151,5 +135,5 @@ def test_fused_coarse_search_equals_the_dense_one(n_probes, nq, monkeypatch):
     d0, i0, d1, i1 = d0.cpu().numpy(), i0.cpu().numpy(), d1.cpu().numpy(), i1.cpu().numpy()
     np.testing.assert_array_equal(i1, i0)
     np.testing.assert_array_equal(d1, d0)
-    rd, ri = _oracle_search(index, ds, qs[:64], n_probes, k, "sqeuclidean")
+    rd, ri = flat_search(index, ds, qs[:64], n_probes, k, "sqeuclidean")
     assert oracle.recall_with_ties(i1[:64], d1[:64], ri, rd, eps=1e-3) >= 0.999

@@ -18,11 +18,11 @@ import pytest
 import torch
 
 import oracle
+from tests.ivf_oracle import I64_MAX, check_rows, flat_search
 from tests.util import clustered, uniform
 
 pytestmark = pytest.mark.gpu
 
-I64_MAX = np.iinfo(np.int64).max
 FLT_MAX = np.finfo(np.float32).max
 N_LISTS = 64
 N_PROBES = 32  # ~15k probed rows per query: more than 2k for every k below
@@ -57,20 +57,6 @@ def _search(index, qs, n_probes, k, **kw):
     return d.cpu().numpy(), i.cpu().numpy()
 
 
-def _oracle_search(index, ds, qs, n_probes, k, metric):
-    sizes = index.list_sizes.cpu().numpy().astype(np.int64)
-    ids = [index.list_indices(l).cpu().numpy() for l in range(index.n_lists)]
-    offsets = np.concatenate([[0], np.cumsum(sizes)])
-    all_ids = np.concatenate(ids)
-    return oracle.ivf_flat_search(index.centers.cpu().numpy(), offsets, ds[all_ids], all_ids, qs, n_probes, k, metric)
-
-
-def _unique_rows(i):
-    for row in i:
-        real = row[row != I64_MAX]
-        assert len(np.unique(real)) == len(real), "an id is returned twice in one row"
-
-
 def _timed_count(name, fn):
     """Runs fn with the library's section timers on; returns how many `name` sections it ran."""
     from cuvs_b200._capi import lib
@@ -103,11 +89,11 @@ def test_large_k_matches_oracle(metric, d, k):
         floor = 1.0
     else:
         dist, idx = _search(index, qs, N_PROBES, k)
-        rd, ri = _oracle_search(index, ds, qs, N_PROBES, k, metric)
+        rd, ri = flat_search(index, ds, qs, N_PROBES, k, metric)
         floor = N_PROBES / N_LISTS
     assert idx.shape == (len(qs), k)
     assert (idx != I64_MAX).all(), "the probed lists hold more than k rows"
-    _unique_rows(idx)
+    check_rows(idx)
     rec = oracle.recall_with_ties(idx, dist, ri, rd, eps=1e-3)
     assert rec >= (0.999 if k <= 1024 else 0.99), rec
     # against exact ground truth: the reference test-suite's recall floor n_probes / n_lists
@@ -147,7 +133,7 @@ def test_bitset_filter_never_returns_a_filtered_row():
     dist, idx = _search(index, qs, N_PROBES, k, filter=filters.from_bitset(torch.from_numpy(bits.view(np.int32)).cuda()))
     valid = idx != I64_MAX
     assert keep[idx[valid]].all(), "a filtered-out row was returned"
-    _unique_rows(idx)
+    check_rows(idx)
     sizes = index.list_sizes.cpu().numpy().astype(np.int64)
     ids_f = [i[keep[i]] for i in (index.list_indices(l).cpu().numpy() for l in range(index.n_lists))]
     offsets = np.concatenate([[0], np.cumsum([len(i) for i in ids_f])])
@@ -170,7 +156,7 @@ def test_missing_slots_are_filled(metric):
     assert missing[:, int(index.list_sizes.to(torch.int64).max()):].all()
     assert (dist[missing] == (-FLT_MAX if metric == "inner_product" else FLT_MAX)).all()
     assert (~missing).sum(axis=1).min() >= 1
-    _unique_rows(idx)
+    check_rows(idx)
     if metric == "sqeuclidean":
         assert (idx[:, 0] == np.arange(4)).all()
 
@@ -228,7 +214,7 @@ def test_multi_gpu_ivf_flat_k100_matches_exact_knn(mode):
     check(lib.cuvsMultiGpuIvfFlatSearch(res, sp, index, d_q.ptr, d_nb.ptr, d_dd.ptr))
     gd, gi = oracle.knn(ds, qs, k)
     assert oracle.recall_with_ties(nb.numpy(), dd.numpy(), gi, gd, eps=1e-3) >= 0.999
-    _unique_rows(nb.numpy())
+    check_rows(nb.numpy())
     check(lib.cuvsMultiGpuIvfFlatIndexDestroy(index))
     check(lib.cuvsMultiGpuIvfFlatSearchParamsDestroy(sp))
     check(lib.cuvsMultiGpuIvfFlatIndexParamsDestroy(ip))

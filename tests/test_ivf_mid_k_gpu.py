@@ -11,11 +11,11 @@ import pytest
 import torch
 
 import oracle
+from tests.ivf_oracle import I64_MAX, check_rows, flat_search
 from tests.util import clustered, uniform
 
 pytestmark = pytest.mark.gpu
 
-I64_MAX = np.iinfo(np.int64).max
 KS = [33, 48, 64]
 _INDEX = {}
 
@@ -48,33 +48,14 @@ def _search(index, qs, n_probes, k, **kw):
     return d.cpu().numpy(), i.cpu().numpy()
 
 
-def _lists(index, keep=None):
-    ids = [index.list_indices(l).cpu().numpy() for l in range(index.n_lists)]
-    if keep is not None:
-        ids = [i[keep[i]] for i in ids]
-    offsets = np.concatenate([[0], np.cumsum([len(i) for i in ids])])
-    return offsets, np.concatenate(ids)
-
-
-def _oracle_search(index, ds, qs, n_probes, k, metric, keep=None):
-    offsets, all_ids = _lists(index, keep)
-    return oracle.ivf_flat_search(index.centers.cpu().numpy(), offsets, ds[all_ids], all_ids, qs, n_probes, k, metric)
-
-
-def _unique_rows(i):
-    for row in i:
-        real = row[row != I64_MAX]
-        assert len(np.unique(real)) == len(real), "an id is returned twice in one row"
-
-
 @pytest.mark.parametrize("k", KS)
 @pytest.mark.parametrize("metric", ["sqeuclidean", "inner_product", "euclidean"])
 @pytest.mark.parametrize("data", ["clustered", "uniform"])
 def test_search_matches_oracle(data, metric, k):
     index, ds, qs, n_probes = _index(data, metric)
     dist, idx = _search(index, qs, n_probes, k)
-    rd, ri = _oracle_search(index, ds, qs, n_probes, k, metric)
-    _unique_rows(idx)
+    rd, ri = flat_search(index, ds, qs, n_probes, k, metric)
+    check_rows(idx)
     assert (idx != I64_MAX).all()
     rec = oracle.recall_with_ties(idx, dist, ri, rd, eps=1e-3)
     assert rec >= 0.999, rec
@@ -88,7 +69,7 @@ def test_cosine_with_every_list_probed_is_exact(k):
     index, ds, qs, _ = _index("clustered", "cosine")
     dist, idx = _search(index, qs, index.n_lists, k)
     rd, ri = oracle.knn(ds, qs, k, "cosine")
-    _unique_rows(idx)
+    check_rows(idx)
     assert oracle.recall_with_ties(idx, dist, ri, rd, eps=1e-3) >= 0.999
 
 
@@ -102,8 +83,8 @@ def test_bitset_filter_at_k64():
     dist, idx = _search(index, qs, n_probes, 64, filter=filters.from_bitset(torch.from_numpy(bits.view(np.int32)).cuda()))
     valid = idx != I64_MAX
     assert keep[idx[valid]].all(), "a filtered-out row was returned"
-    _unique_rows(idx)
-    rd, ri = _oracle_search(index, ds, qs, n_probes, 64, "sqeuclidean", keep)
+    check_rows(idx)
+    rd, ri = flat_search(index, ds, qs, n_probes, 64, "sqeuclidean", keep)
     assert (valid == (ri != I64_MAX)).all(), "the number of results differs from the oracle's"
     assert oracle.recall_with_ties(idx, dist, ri, rd, eps=1e-3) >= 0.999
     assert (idx == ri).mean() >= 0.995

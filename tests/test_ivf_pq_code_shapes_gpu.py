@@ -18,8 +18,8 @@ import pytest
 import torch
 
 import oracle
+from tests.ivf_oracle import check_rows, pq_search
 from tests.ivf_pq_codes import index_codes, unpack_codes
-from tests.ivf_pq_cosine_ref import ivf_pq_cosine_search
 from tests.util import uniform
 
 pytestmark = pytest.mark.gpu
@@ -75,13 +75,7 @@ def _per_cluster(shape):
 
 
 def _oracle(index, shape, qs, n_probes, k, metric="sqeuclidean", lut="f32", dist="f32"):
-    offs, codes, ids = index_codes(index)
-    kw = dict(pq_bits=index.pq_bits, per_cluster=_per_cluster(shape), lut_dtype=lut, dist_dtype=dist)
-    if metric == "cosine":
-        return ivf_pq_cosine_search(index.centers_rot.cpu().numpy(), index.rotation_matrix.cpu().numpy(),
-                                    index.pq_centers.cpu().numpy(), offs, codes, ids, qs, n_probes, k, **kw)
-    return oracle.ivf_pq_search(index.centers.cpu().numpy(), index.centers_rot.cpu().numpy(), index.rotation_matrix.cpu().numpy(),
-                                index.pq_centers.cpu().numpy(), offs, codes, ids, qs, n_probes, k, metric, **kw)
+    return pq_search(index, qs, n_probes, k, metric, lut, dist, per_cluster=_per_cluster(shape))
 
 
 def _search(monkeypatch, index, qs, n_probes, k, path, lut="f32", dist="f32"):
@@ -91,13 +85,6 @@ def _search(monkeypatch, index, qs, n_probes, k, path, lut="f32", dist="f32"):
           "internal_distance_dtype": {"f32": np.float32, "f16": np.float16}[dist]}
     d, i = m.search(m.SearchParams(n_probes=n_probes, **kw), index, torch.from_numpy(qs).cuda(), k)
     return d.cpu().numpy(), i.cpu().numpy()
-
-
-def _check_rows(i, n):
-    for row in i:
-        real = row[row != np.iinfo(np.int64).max]
-        assert len(np.unique(real)) == len(real), "an id is returned twice in one row"
-        assert ((real >= 0) & (real < n)).all()
 
 
 def test_shapes_are_built_as_asked():
@@ -124,7 +111,7 @@ def test_lut_scan_matches_oracle(monkeypatch, shape, lut, dist, tol):
     ds, qs, index = _built(shape)
     d, i = _search(monkeypatch, index, qs, N_PROBES, 32, "lut", lut, dist)
     rd, ri = _oracle(index, shape, qs, N_PROBES, 32, lut=lut, dist=dist)
-    _check_rows(i, N)
+    check_rows(i, N)
     assert oracle.recall_with_ties(i, d, ri, rd, eps=tol) >= 0.999
     if dist == "f32":
         same = i == ri
@@ -140,7 +127,7 @@ def test_tensor_core_request_matches_oracle(monkeypatch, shape, k):
     ds, qs, index = _built(shape)
     d, i = _search(monkeypatch, index, qs, N_PROBES, k, "tc")
     rd, ri = _oracle(index, shape, qs, N_PROBES, k)
-    _check_rows(i, N)
+    check_rows(i, N)
     assert oracle.recall_with_ties(i, d, ri, rd, eps=2e-3) >= 0.995
 
 
@@ -150,7 +137,7 @@ def test_store_path_k100_matches_oracle(monkeypatch, shape, path):
     ds, qs, index = _built(shape)
     d, i = _search(monkeypatch, index, qs, N_PROBES, 100, path)
     rd, ri = _oracle(index, shape, qs, N_PROBES, 100)
-    _check_rows(i, N)
+    check_rows(i, N)
     if path == "lut" or not index.streamed:  # the LUT kernel's store mode
         assert oracle.recall_with_ties(i, d, ri, rd, eps=1e-5) >= 0.999
     else:  # the code stream's store epilogue (the bar of test_ivf_pq_large_k_gpu.py::test_stream_store_matches_oracle)
@@ -165,7 +152,7 @@ def test_other_metrics_match_oracle(monkeypatch, shape, metric, path):
     for k in (10, 64):
         d, i = _search(monkeypatch, index, qs, N_PROBES, k, path)
         rd, ri = _oracle(index, shape, qs, N_PROBES, k, metric)
-        _check_rows(i, N)
+        check_rows(i, N)
         if path == "lut":
             assert oracle.recall_with_ties(i, d, ri, rd, eps=1e-5) >= 0.999
         else:  # (the decoded rows of an inner-product index hold c + y rounded to bf16: the bar of test_other_metrics)

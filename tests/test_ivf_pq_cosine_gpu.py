@@ -13,7 +13,8 @@ import pytest
 import torch
 
 import oracle
-from tests.ivf_pq_cosine_ref import ivf_pq_cosine_search
+from tests.ivf_oracle import pq_search
+from tests.ivf_pq_codes import index_codes
 from tests.util import clustered, uniform
 
 pytestmark = pytest.mark.gpu
@@ -31,30 +32,16 @@ def mixed_norm(n, d, seed, n_centers=64, centers=None):
     return (x * f[:, None]).astype(np.float32), centers
 
 
-def _unpack(index):
-    """-> (offsets, codes [n, pq_dim] one code per byte, ids) from the C getters (8-bit codes here)."""
-    sizes = index.list_sizes.cpu().numpy().astype(np.int64)
-    offs = np.concatenate([[0], np.cumsum(sizes)])
-    codes, ids = [], []
-    for l in range(index.n_lists):
-        if sizes[l]:
-            codes.append(index.list_data(l).cpu().numpy())
-            ids.append(index.list_indices(l).cpu().numpy())
-    return offs, np.concatenate(codes), np.concatenate(ids)
-
-
 def _by_id(index):
     """-> (ids, list label, codes) of every stored row, ordered by id: with the default ids, the order of the dataset."""
-    offs, codes, ids = _unpack(index)
+    offs, codes, ids = index_codes(index)
     labels = np.searchsorted(offs, np.arange(len(ids)), side="right") - 1
     order = np.argsort(ids, kind="stable")
     return ids[order], labels[order], codes[order]
 
 
 def _oracle(index, qs, n_probes, k, lut="f32", dist="f32"):
-    offs, codes, ids = _unpack(index)
-    return ivf_pq_cosine_search(index.centers_rot.cpu().numpy(), index.rotation_matrix.cpu().numpy(), index.pq_centers.cpu().numpy(),
-                                offs, codes, ids, qs, n_probes, k, pq_bits=8, lut_dtype=lut, dist_dtype=dist)
+    return pq_search(index, qs, n_probes, k, "cosine", lut, dist)
 
 
 def _search(index, qs, n_probes, k, path, **kw):
@@ -205,7 +192,7 @@ def test_extend_in_chunks_equals_build_with_data():
     m.extend(empty, torch.from_numpy(ds[5000:]).cuda(), torch.from_numpy(ids[5000:]).cuda())
     assert len(empty) == len(ds)
     assert np.array_equal(full.list_sizes.cpu().numpy(), empty.list_sizes.cpu().numpy())
-    for a, b in zip(_unpack(full), _unpack(empty)):
+    for a, b in zip(index_codes(full), index_codes(empty)):
         assert np.array_equal(a, b)
 
 
@@ -233,7 +220,7 @@ def test_build_is_deterministic():
     out = []
     for _ in range(2):
         index = m.build(m.IndexParams(n_lists=64, pq_dim=64, metric="cosine", kmeans_n_iters=10), ds)
-        out.append((index.centers.cpu().numpy().copy(), index.pq_centers.cpu().numpy().copy()) + _unpack(index))
+        out.append((index.centers.cpu().numpy().copy(), index.pq_centers.cpu().numpy().copy()) + index_codes(index))
     for a, b in zip(*out):
         assert np.array_equal(a, b)
 
@@ -255,7 +242,7 @@ def test_narrow_dtypes_match_the_widened_fp32_index(dtype):
     wide = m.build(params, torch.from_numpy(x.astype(np.float32)).cuda())
     assert np.array_equal(narrow.centers.cpu().numpy(), wide.centers.cpu().numpy())
     assert np.array_equal(narrow.pq_centers.cpu().numpy(), wide.pq_centers.cpu().numpy())
-    for a, b in zip(_unpack(narrow), _unpack(wide)):
+    for a, b in zip(index_codes(narrow), index_codes(wide)):
         assert np.array_equal(a, b)
     d1, i1 = _search(narrow, q, 8, 10, "auto")
     d2, i2 = _search(wide, q.astype(np.float32), 8, 10, "auto")

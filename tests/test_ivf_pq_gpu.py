@@ -13,6 +13,8 @@ import pytest
 import torch
 
 import oracle
+from tests.ivf_oracle import pq_search
+from tests.ivf_pq_codes import index_codes
 from tests.util import clustered, uniform
 
 pytestmark = pytest.mark.gpu
@@ -21,25 +23,6 @@ pytestmark = pytest.mark.gpu
 def _mod():
     from cuvs_b200.neighbors import ivf_pq
     return ivf_pq
-
-
-def _unpack(index):
-    """-> (offsets, codes [n, pq_dim] one code per byte, ids) from the C getters (8-bit codes here)."""
-    sizes = index.list_sizes.cpu().numpy().astype(np.int64)
-    offs = np.concatenate([[0], np.cumsum(sizes)])
-    codes, ids = [], []
-    for l in range(index.n_lists):
-        if sizes[l]:
-            codes.append(index.list_data(l).cpu().numpy())
-            ids.append(index.list_indices(l).cpu().numpy())
-    return offs, np.concatenate(codes), np.concatenate(ids)
-
-
-def _oracle(index, qs, n_probes, k, metric, lut="f32", dist="f32"):
-    offs, codes, ids = _unpack(index)
-    return oracle.ivf_pq_search(index.centers.cpu().numpy(), index.centers_rot.cpu().numpy(), index.rotation_matrix.cpu().numpy(),
-                                index.pq_centers.cpu().numpy(), offs, codes, ids, qs, n_probes, k, metric, pq_bits=8,
-                                lut_dtype=lut, dist_dtype=dist)
 
 
 def _search(index, qs, n_probes, k, path, **kw):
@@ -64,7 +47,7 @@ def test_index_shapes_and_packing(small_index):
     assert tuple(index.pq_centers.shape) == (32, 2, 256) and tuple(index.centers_padded.shape) == (32, 72)
     cp = index.centers_padded.cpu().numpy()
     np.testing.assert_allclose(cp[:, 64], (cp[:, :64] ** 2).sum(1), rtol=1e-5)  # |c|^2 column (ivf_pq_index.cu:78-80)
-    offs, codes, ids = _unpack(index)
+    offs, codes, ids = index_codes(index)
     assert sorted(ids.tolist()) == list(range(4096)) and codes.shape == (4096, 32)
     # codes really are the nearest codebook entries of the rotated residuals (transform == what is stored)
     m = _mod()
@@ -80,7 +63,7 @@ def test_lut_scan_matches_oracle(small_index, lut, dist, tol):
     kw = {"lut_dtype": {"f32": np.float32, "f16": np.float16, "fp8": np.uint8}[lut],
           "internal_distance_dtype": {"f32": np.float32, "f16": np.float16}[dist]}
     d, i = _search(index, qs, 8, 32, "lut", **kw)
-    rd, ri = _oracle(index, qs, 8, 32, "sqeuclidean", lut, dist)
+    rd, ri = pq_search(index, qs, 8, 32, "sqeuclidean", lut, dist)
     assert oracle.recall_with_ties(i, d, ri, rd, eps=max(tol, 1e-5)) >= 0.999
     if dist == "f32":
         same = i == ri
@@ -91,7 +74,7 @@ def test_lut_scan_matches_oracle(small_index, lut, dist, tol):
 def test_tensor_core_path_matches_lut_semantics(small_index):
     ds, qs, index = small_index
     d, i = _search(index, qs, 8, 32, "tc")
-    rd, ri = _oracle(index, qs, 8, 32, "sqeuclidean")
+    rd, ri = pq_search(index, qs, 8, 32, "sqeuclidean")
     assert oracle.recall_with_ties(i, d, ri, rd, eps=2e-3) >= 0.995
     same = i == ri
     assert same.mean() >= 0.97
@@ -120,7 +103,7 @@ def test_other_metrics(metric, path):
     qs, _ = clustered(200, 96, 4, centers=centers)
     index = m.build(m.IndexParams(n_lists=64, pq_dim=48, metric=metric, kmeans_n_iters=10), torch.from_numpy(ds).cuda())
     d, i = _search(index, qs, 16, 10, path)
-    rd, ri = _oracle(index, qs, 16, 10, metric)
+    rd, ri = pq_search(index, qs, 16, 10, metric)
     assert oracle.recall_with_ties(i, d, ri, rd, eps=3e-3) >= 0.99
 
 
@@ -183,7 +166,7 @@ def test_wide_vectors_take_the_streamed_scan():
     index = m.build(m.IndexParams(n_lists=16, pq_dim=96, kmeans_n_iters=10, kmeans_trainset_fraction=1.0), torch.from_numpy(ds).cuda())
     assert index.pq_len == 2
     d, i = _search(index, qs, 8, 10, "tc")
-    rd, ri = _oracle(index, qs, 8, 10, "sqeuclidean")
+    rd, ri = pq_search(index, qs, 8, 10, "sqeuclidean")
     assert oracle.recall_with_ties(i, d, ri, rd, eps=2e-3) >= 0.99
     gd, gi = oracle.knn(ds, qs, 10)
     assert oracle.recall(i, gi) >= 0.6  # iid-uniform 192-d data, 8 of 16 lists, 2 dims per code: PQ noise, not the scan
@@ -212,13 +195,13 @@ def test_one_pass_scan_matches_reduced_lut_oracle(metric, lut, dim, pq_dim):
     # fp_8bit<5> entries carry ~2^-4 (signed variant for inner product: 2^-3) and the 64 entries of a score add up, so the
     # reference's own fp8 answer sits several percent away from the exact LUT sum; ours (bf16 residual, exact codebook) is the
     # more accurate of the two and is compared at the fp8 format's error scale.
-    rd, ri = _oracle(index, qs, 12, 10, metric, lut, "f32")
+    rd, ri = pq_search(index, qs, 12, 10, metric, lut, "f32")
     # (floor 0.975, not 0.99: the clustered test data has ~1000 near-equidistant neighbours per point, so a 0.5 % score error
     # flips ranks across the k-th position, and a flipped row only counts when its distance lands within eps of a true one;
     # the k-means build is not bit-reproducible either, so the figure moves by ~0.5 % between runs)
     assert oracle.recall_with_ties(i, d, ri, rd, eps=1e-2 if lut == "f16" else 8e-2) >= 0.975
     # ... and against the fp32-LUT answer it is at least as close as the reference's reduced LUTs are allowed to be
-    fd, fi = _oracle(index, qs, 12, 10, metric, "f32", "f32")
+    fd, fi = pq_search(index, qs, 12, 10, metric, "f32", "f32")
     assert oracle.recall_with_ties(i, d, fi, fd, eps=1e-2) >= 0.975
     same = i == fi
     assert same.mean() >= (0.9 if metric == "sqeuclidean" else 0.75)  # (inner-product scores of ~150 with near-ties: ranks swap)
@@ -261,7 +244,7 @@ def test_streamed_scan_all_shapes(small_index, stream_index_128, group, which, k
         d, i = _search(index, qs, 8, k, "stream", **kw)
     finally:
         del os.environ["CUVS_B200_PQ_GROUP"]
-    rd, ri = _oracle(index, qs, 8, k, "sqeuclidean", lut, "f32")
+    rd, ri = pq_search(index, qs, 8, k, "sqeuclidean", lut, "f32")
     eps = 2e-3 if lut == "f32" else 1e-2
     assert oracle.recall_with_ties(i, d, ri, rd, eps=eps) >= (0.99 if lut == "f32" else 0.975)
     # returned ids are unique per query and really belong to the probed lists' rows (no padding rows, no garbage)
@@ -275,7 +258,7 @@ def test_streamed_scan_k_up_to_64(stream_index_128, k):
     ds, qs, index = stream_index_128
     assert index.streamed
     d, i = _search(index, qs, 8, k, "stream", lut_dtype=np.float16)
-    rd, ri = _oracle(index, qs, 8, k, "sqeuclidean", "f16", "f32")
+    rd, ri = pq_search(index, qs, 8, k, "sqeuclidean", "f16", "f32")
     assert oracle.recall_with_ties(i, d, ri, rd, eps=1e-2) >= 0.975
     assert all(len(set(r.tolist())) == k for r in i) and (i >= 0).all() and (i < len(ds)).all()
     d2, i2 = _search(index, qs, 8, k, "lut", lut_dtype=np.float16)
@@ -283,7 +266,7 @@ def test_streamed_scan_k_up_to_64(stream_index_128, k):
     assert same >= 0.97, same
     # the 2-pass scan (fp32 LUT semantics) through the same wide buffers
     d3, i3 = _search(index, qs, 8, k, "stream")
-    rd3, ri3 = _oracle(index, qs, 8, k, "sqeuclidean", "f32", "f32")
+    rd3, ri3 = pq_search(index, qs, 8, k, "sqeuclidean", "f32", "f32")
     assert oracle.recall_with_ties(i3, d3, ri3, rd3, eps=2e-3) >= 0.99
 
 
@@ -311,7 +294,7 @@ def test_small_index_dense_batch_takes_the_decoded_row_cache(stream_index_128):
     d_str, i_str = _search(index, q, 8, 10, "stream", lut_dtype=np.float16)
     same = np.mean([len(set(a) & set(b)) / 10.0 for a, b in zip(i_dense, i_str)])
     assert same >= 0.995, same
-    rd, ri = _oracle(index, q, 8, 10, "sqeuclidean", "f16", "f32")
+    rd, ri = pq_search(index, q, 8, 10, "sqeuclidean", "f16", "f32")
     assert oracle.recall_with_ties(i_dense, d_dense, ri, rd, eps=1e-2) >= 0.975
 
 
@@ -323,7 +306,7 @@ def test_streamed_scan_empty_and_tiny_lists():
     index = m.build(m.IndexParams(n_lists=128, pq_dim=32, kmeans_n_iters=4, kmeans_trainset_fraction=1.0), torch.from_numpy(ds).cuda())
     assert index.streamed
     d, i = _search(index, qs, 128, 10, "stream", lut_dtype=np.float16)
-    rd, ri = _oracle(index, qs, 128, 10, "sqeuclidean", "f16", "f32")
+    rd, ri = pq_search(index, qs, 128, 10, "sqeuclidean", "f16", "f32")
     assert oracle.recall_with_ties(i, d, ri, rd, eps=1e-2) >= 0.99
 
 

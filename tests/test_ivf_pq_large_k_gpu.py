@@ -10,6 +10,7 @@ import pytest
 import torch
 
 import oracle
+from tests.ivf_oracle import check_rows, pq_search
 from tests.util import clustered, uniform
 
 pytestmark = pytest.mark.gpu
@@ -20,24 +21,6 @@ KS = [65, 100, 128, 129, 256, 257, 1023, 2048]
 def _mod():
     from cuvs_b200.neighbors import ivf_pq
     return ivf_pq
-
-
-def _unpack(index):
-    sizes = index.list_sizes.cpu().numpy().astype(np.int64)
-    offs = np.concatenate([[0], np.cumsum(sizes)])
-    codes, ids = [], []
-    for l in range(index.n_lists):
-        if sizes[l]:
-            codes.append(index.list_data(l).cpu().numpy())
-            ids.append(index.list_indices(l).cpu().numpy())
-    return offs, np.concatenate(codes), np.concatenate(ids)
-
-
-def _oracle(index, qs, n_probes, k, metric, lut="f32"):
-    offs, codes, ids = _unpack(index)
-    return oracle.ivf_pq_search(index.centers.cpu().numpy(), index.centers_rot.cpu().numpy(), index.rotation_matrix.cpu().numpy(),
-                                index.pq_centers.cpu().numpy(), offs, codes, ids, qs, n_probes, k, metric, pq_bits=8,
-                                lut_dtype=lut)
 
 
 def _search(monkeypatch, index, qs, n_probes, k, path, lut="f32", **env):
@@ -54,13 +37,6 @@ def _search(monkeypatch, index, qs, n_probes, k, path, lut="f32", **env):
 
 def _probes(n_lists, k, base=8):
     return max(base, min(n_lists, k))
-
-
-def _check_rows(i, n):
-    for row in i:
-        real = row[row != np.iinfo(np.int64).max]
-        assert len(np.unique(real)) == len(real)
-        assert ((real >= 0) & (real < n)).all()
 
 
 def _check_prefix(d64, i64, dk, ik):
@@ -89,8 +65,8 @@ def test_lut_store_matches_oracle(monkeypatch, stream_index, k):
     ds, qs, index = stream_index
     p = _probes(32, k)
     d, i = _search(monkeypatch, index, qs, p, k, "lut")
-    rd, ri = _oracle(index, qs, p, k, "sqeuclidean")
-    _check_rows(i, len(ds))
+    rd, ri = pq_search(index, qs, p, k, "sqeuclidean")
+    check_rows(i, len(ds))
     assert oracle.recall_with_ties(i, d, ri, rd, eps=1e-5) >= 0.999
     same = i == ri
     assert same.mean() >= 0.99
@@ -103,8 +79,8 @@ def test_stream_store_matches_oracle(monkeypatch, stream_index, k, lut):
     ds, qs, index = stream_index
     p = _probes(32, k)
     d, i = _search(monkeypatch, index, qs, p, k, "stream", lut=lut)
-    rd, ri = _oracle(index, qs, p, k, "sqeuclidean", lut=lut)
-    _check_rows(i, len(ds))
+    rd, ri = pq_search(index, qs, p, k, "sqeuclidean", lut=lut)
+    check_rows(i, len(ds))
     if lut == "f32":
         assert oracle.recall_with_ties(i, d, ri, rd, eps=2e-3) >= 0.99
     else:
@@ -133,10 +109,10 @@ def test_metrics_and_index_shapes(monkeypatch, metric, shape):
     for path in (["stream", "lut"] if shape == "stream" else ["lut"]):  # k > 64 serves these shapes with the LUT kernel
         d64, i64 = _search(monkeypatch, index, qs, 40, 64, path)
         dk, ik = _search(monkeypatch, index, qs, 40, 100, path)
-        _check_rows(ik, len(ds))
+        check_rows(ik, len(ds))
         _check_prefix(d64, i64, dk, ik)
-        if metric == "inner_product" and shape == "stream" and path == "lut":  # (the helper unpacks 8-bit per-subspace codes)
-            rd, ri = _oracle(index, qs, 40, 100, metric)
+        if metric == "inner_product" and shape == "stream" and path == "lut":
+            rd, ri = pq_search(index, qs, 40, 100, metric)
             assert oracle.recall_with_ties(ik, dk, ri, rd, eps=1e-5) >= 0.999
 
 
@@ -151,7 +127,7 @@ def test_reference_special_cases_recall_floor(monkeypatch, k, path):
     index = m.build(m.IndexParams(n_lists=100, kmeans_trainset_fraction=1.0), torch.from_numpy(ds).cuda())
     d, i = _search(monkeypatch, index, qs, 100, k, path)
     gd, gi = oracle.knn(ds, qs, k)
-    _check_rows(i, len(ds))
+    check_rows(i, len(ds))
     assert oracle.recall_with_ties(i, d, gi, gd, eps=1e-4 * 4) >= 0.86
 
 
