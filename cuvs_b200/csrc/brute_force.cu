@@ -29,7 +29,6 @@
 #include <algorithm>
 #include <cfloat>
 #include <cmath>
-#include <cstdlib>
 #include <cstring>
 #include <fstream>
 #include <memory>
@@ -269,7 +268,7 @@ static void bf_tc_candidates(resources* res, const bf_index& idx, const float* q
   tc_split_planes(stream, q, nq, idx.d, idx.d, idx.Kp, qhi.data(), qlo.data(), nq_pad, qscale.data());
 
   dbuf<tc_item> items(static_cast<size_t>(n_items), stream);
-  const int KCW = KC * tc_lists_per_item();  // candidates per (item, query row)
+  const int KCW = KC * kTcListsPerItem;  // candidates per (item, query row)
   make_items_kernel<<<(n_items + 127) / 128, 128, 0, stream>>>(items.data(), m_tiles, splits, nq, static_cast<uint32_t>(b_tiles), KCW);
   B2_CUDA(cudaGetLastError());
   count_launch();
@@ -347,12 +346,11 @@ static void bf_search(resources* res, const bf_index& idx, const DLTensor& qt, c
   }
 
   const bool select_min = metric_is_min_close(idx.metric);
-  static const bool force_exact = getenv("CUVS_B200_FORCE_EXACT") != nullptr;  // test knob
   // k <= 24: fused lists of 16 / 32, merged to the list length.  24 < k <= 64 (the reference's fused range,
   // knn_brute_force.cuh:447-451): fused lists of 32 per (column half, split), merged to 64 / 96 candidates, and the
   // certificate additionally uses the lists' own worst entries (bf_cands::floor) — a row of the true top-k can only be missing
   // when more than 32 of them fall into one list, which the certificate detects (flagged queries take the exact path).
-  const bool use_tc     = idx.tc && filt.kind == 0 && k <= 64 && idx.n > 0 && !force_exact;
+  const bool use_tc     = idx.tc && filt.kind == 0 && k <= 64 && idx.n > 0;
   set_last_flagged(0);
   if (!use_tc) {
     search_exact(res, idx, q, nq, 0, k, out_idx, out_dist, filt);

@@ -624,7 +624,7 @@ static bool coarse_select_fused(resources* res, const tc_rows_tmp& q, const tc_r
   int splits = std::max((2 * sms + m_tiles - 1) / m_tiles, (n_probes + 15) / 16);
   splits     = static_cast<int>(std::min<int64_t>(splits, std::min<int64_t>(16, b_tiles / 4)));
   splits     = std::max(splits, 1);
-  const int KCW = KC * tc_lists_per_item();
+  const int KCW = KC * kTcListsPerItem;
   const int W   = splits * KCW;
   if (W > kCoarseMaxW || W < 4 * n_probes) return false;
   const int n_items = m_tiles * splits;
@@ -693,8 +693,7 @@ void assign_nearest(resources* res, const __nv_bfloat16* x_hi, const __nv_bfloat
   if (n == 0) return;
   B2_EXPECTS(Kp == centers.Kp, "assign_nearest: dimension mismatch");
   const int KC         = 16;
-  const int lists      = tc_lists_per_item();
-  const int KCW        = KC * lists;
+  const int KCW        = KC * kTcListsPerItem;
   const int64_t chunk  = int64_t(1) << 20;  // rows per launch: bounds the (score,pos) scratch to 256 MiB
   const bool three     = x_lo != nullptr && centers.lo.data() != nullptr;
   dbuf<float> cs(static_cast<size_t>(std::min(chunk, tc_pad_rows(n))) * KCW, s);
@@ -711,7 +710,7 @@ void assign_nearest(resources* res, const __nv_bfloat16* x_hi, const __nv_bfloat
                  centers.lo.data(), centers.rows_pad, Kp, centers.hx.data(), items.data(), m_tiles, nullptr, KC,
                  three ? 3 : 1, cs.data(), cp.data(), KCW);
     count_launch();
-    first_of_rows_kernel<<<blocks_for(rows, 256), 256, 0, s>>>(cp.data(), cs.data(), rows, KC, lists, labels + r0,
+    first_of_rows_kernel<<<blocks_for(rows, 256), 256, 0, s>>>(cp.data(), cs.data(), rows, KC, kTcListsPerItem, labels + r0,
                                                                scores ? scores + r0 : nullptr);
     B2_CUDA(cudaGetLastError());
   }

@@ -293,9 +293,7 @@ void ivf_flat_search(resources* res, const ivf_flat_index& idx, uint32_t n_probe
   // k > 64: no fused top-k (KC = 0, the store epilogue); each pair keeps its kc2 best from its dense score segment.
   const int KC    = large_k ? 0 : ((k + k / 2 <= 16) ? 16 : 32);
   const bool use_bound = !large_k && KC >= k + k / 2;
-  const int lists = tc_lists_per_item();
-  int KCW         = KC * lists;
-  B2_EXPECTS(large_k || KCW >= k, "ivf_flat search: k = %d needs the two-list tensor-core epilogue (CUVS_B200_TC_EPIW=8)", k);
+  int KCW         = KC * kTcListsPerItem;
   probe_buckets pb;
   bucket_probes(res, probes.data(), nq, static_cast<int>(n_probes), idx.n_lists, idx.lists.d_offsets.data(), KCW, pb);
 

@@ -771,7 +771,7 @@ ivf_pq_index* ivf_pq_build(resources* res, const cuvsIvfPqIndexParams& p, const 
 //   lut            otherwise                                       otherwise
 //   passes         reduced ? 1 : 2                                 same
 //   KC             k <= 16 ? 16 : (k <= 32 ? 32 : 64)              0
-//   KCW            KC x (decoded ? tc_lists_per_item() : 1)        0 to bucket_probes, k after the segment select
+//   KCW            KC x (decoded ? kTcListsPerItem : 1)            0 to bucket_probes, k after the segment select
 //   group          stream ? pq_stream_group(pairs per list, KC, passes) : 128   same, with KC = 0
 //   pruning bound  tensor-core paths with k <= KC                  none
 //
@@ -808,7 +808,7 @@ scan_plan plan_scan(const ivf_pq_index& idx, const cuvsIvfPqSearchParams& sp, in
   const bool decoded = p.path == scan_path::decoded;
   p.passes = reduced ? 1 : 2;
   p.KC     = p.store ? 0 : (k <= 16 ? 16 : (k <= 32 ? 32 : 64));
-  p.KCW    = p.KC * (decoded ? tc_lists_per_item() : 1);
+  p.KCW    = p.KC * (decoded ? kTcListsPerItem : 1);
   p.group  = p.path == scan_path::stream
                ? pq_stream_group(static_cast<double>(nq) * n_probes / std::max<uint32_t>(idx.n_lists, 1), p.KC, p.passes)
                : 128;

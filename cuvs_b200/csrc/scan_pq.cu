@@ -35,12 +35,10 @@
 #include "timing.hpp"
 
 #include <cuda.h>
-#include <unistd.h>
 
 #include <cmath>
 #include <cstdio>
 #include <cstdlib>
-#include <cstring>
 #include <mutex>
 
 namespace b200 {
@@ -78,42 +76,7 @@ struct pq_args {
   int cap;      // candidate buffer entries per query (KC < cap <= 128)
   int cstages;  // code ring depth
   int blk;      // bytes of one tile block of the stream
-  int dbg_mode;   // CUVS_B200_PQ_DEBUG value: (the kernel reads only whether it is set)
-  uint32_t* dbg;  // CUVS_B200_PQ_DEBUG=1: mapped host memory, [grid][8] = {code of the wait that timed out, parity, item, tile, ...}
 };
-
-// Debug wait: identical to ptx::mbar_wait unless P.dbg is set; then a wait that does not complete within ~2 s records where
-// it is stuck (role/barrier code, parity, progress counters) in mapped host memory and traps, so a deadlock becomes a report.
-// (Inlined: a call inside a warpgroup whose register budget setmaxnreg changed cannot be register-allocated.)
-__device__ __forceinline__ void wait_dbg_slow(uint32_t* dbg, uint64_t* bar, uint32_t parity, uint32_t code, uint32_t a, uint32_t b)
-{
-  for (uint32_t spin = 0; spin < 4000000u; ++spin) {
-    uint32_t ok;
-    asm volatile(
-      "{\n\t"
-      ".reg .pred P;\n\t"
-      "mbarrier.test_wait.parity.shared::cta.b64 P, [%1], %2;\n\t"
-      "selp.b32 %0, 1, 0, P;\n\t"
-      "}\n"
-      : "=r"(ok)
-      : "r"(ptx::smem_u32(bar)), "r"(parity)
-      : "memory");
-    if (ok) return;
-    __nanosleep(500);
-  }
-  if ((threadIdx.x & 31) == 0) {
-    uint32_t* d = dbg + blockIdx.x * 16;
-    if (atomicCAS(d, 0u, code) == 0u) { d[1] = parity; d[2] = a; d[3] = b; d[4] = threadIdx.x >> 5; }
-    __threadfence_system();
-  }
-  __nanosleep(100000000);
-  __trap();
-}
-__device__ __forceinline__ void wait_dbg(uint32_t* dbg, uint64_t* bar, uint32_t parity, uint32_t code, uint32_t a, uint32_t b)
-{
-  if (dbg == nullptr) ptx::mbar_wait(bar, parity);
-  else wait_dbg_slow(dbg, bar, parity, code, a, b);
-}
 
 __device__ __forceinline__ bool bar_red_or(uint32_t id, uint32_t nthreads, bool pred)
 {
@@ -399,7 +362,7 @@ pq_stream_scan_kernel(const __grid_constant__ CUtensorMap tmQ_hi, const __grid_c
     // ------------------------------------------------------------------ producer (whole warp loops, one elected lane issues)
     uint32_t cs = 0, cph = 0, qph = 0, ss = 0, sp = 0;
     for (;;) {
-      wait_dbg(P.dbg, &s_empty[ss], sp ^ 1, 0x101, ss, 0);
+      ptx::mbar_wait(&s_empty[ss], sp ^ 1);
       int it = 0;
       if (lane == 0) {
         it = atomicAdd(P.sched, 1);
@@ -414,7 +377,7 @@ pq_stream_scan_kernel(const __grid_constant__ CUtensorMap tmQ_hi, const __grid_c
       item.a_row0  = __shfl_sync(0xffffffffu, item.a_row0, 0);
       item.b_row0  = __shfl_sync(0xffffffffu, item.b_row0, 0);
       item.n_tiles = __shfl_sync(0xffffffffu, item.n_tiles, 0);
-      wait_dbg(P.dbg, q_empty, qph ^ 1, 0x102, static_cast<uint32_t>(it), 0);
+      ptx::mbar_wait(q_empty, qph ^ 1);
       if (ptx::elect_one()) {
         ptx::mbar_arrive_expect_tx(q_full, L::q_bytes);
 #pragma unroll
@@ -426,7 +389,7 @@ pq_stream_scan_kernel(const __grid_constant__ CUtensorMap tmQ_hi, const __grid_c
       qph ^= 1;
       const uint8_t* src = P.stream + static_cast<int64_t>(item.b_row0 >> 7) * P.blk;
       for (uint32_t t = 0; t < item.n_tiles; ++t) {
-        wait_dbg(P.dbg, &c_empty[cs], cph ^ 1, 0x103, static_cast<uint32_t>(it), t);
+        ptx::mbar_wait(&c_empty[cs], cph ^ 1);
         if (ptx::elect_one()) {
           ptx::mbar_arrive_expect_tx(&c_full[cs], static_cast<uint32_t>(P.blk));
           ptx::bulk_load_1d(sCode + cs * P.blk, src + static_cast<int64_t>(t) * P.blk, static_cast<uint32_t>(P.blk), &c_full[cs]);
@@ -445,14 +408,14 @@ pq_stream_scan_kernel(const __grid_constant__ CUtensorMap tmQ_hi, const __grid_c
     const uint32_t cb_lane32 = ptx::smem_u32(sCb) + static_cast<uint32_t>(lane) * 4u;  // this lane's word of codebook row 0
     uint32_t cs = 0, cph = 0, ds = 0, dph = 0, ss = 0, sp = 0;
     for (;;) {
-      wait_dbg(P.dbg, &s_full[ss], sp, 0x301, ss, 0);
+      ptx::mbar_wait(&s_full[ss], sp);
       const int it = __shfl_sync(0xffffffffu, s_item[ss], 0);  // (consumes the load before the slot is handed back)
       if (lane == 0) ptx::mbar_arrive(&s_empty[ss]);
       if (++ss == kSched) { ss = 0; sp ^= 1; }
       if (it < 0) break;
       const uint32_t n_tiles = P.items[it].n_tiles;
       for (uint32_t t = 0; t < n_tiles; ++t) {
-        wait_dbg(P.dbg, &c_full[cs], cph, 0x302, static_cast<uint32_t>(it), t);
+        ptx::mbar_wait(&c_full[cs], cph);
         const uint8_t* cst = sCode + cs * P.blk;
         uint4 cw[NKB];
 #pragma unroll
@@ -467,7 +430,7 @@ pq_stream_scan_kernel(const __grid_constant__ CUtensorMap tmQ_hi, const __grid_c
         const uint32_t cs_read = cs;
         if (++cs == ncs) { cs = 0; cph ^= 1; }
 
-        wait_dbg(P.dbg, &d_empty[ds], dph ^ 1, 0x303, static_cast<uint32_t>(it), t);
+        ptx::mbar_wait(&d_empty[ds], dph ^ 1);
         uint8_t* dst = sDec + ds * L::dec_stage + (2 * dw) * 1024;
 #pragma unroll
         for (int h = 0; h < NKB; ++h) {
@@ -567,18 +530,18 @@ pq_stream_scan_kernel(const __grid_constant__ CUtensorMap tmQ_hi, const __grid_c
     };
 
     for (;;) {
-      wait_dbg(P.dbg, &s_full[ss], sp, 0x401, ss, 0);
+      ptx::mbar_wait(&s_full[ss], sp);
       const int it = __shfl_sync(0xffffffffu, s_item[ss], 0);  // (consumes the load before the slot is handed back)
       if (lane == 0) ptx::mbar_arrive(&s_empty[ss]);
       if (++ss == kSched) { ss = 0; sp ^= 1; }
       if (it < 0) break;
       const tc_item item = P.items[it];
       if constexpr (STORE) {
-        wait_dbg(P.dbg, q_full, qph, 0x202, static_cast<uint32_t>(it), 0);
+        ptx::mbar_wait(q_full, qph);
         const int64_t seg = static_cast<int64_t>(item.n_tiles) * 128;  // a pair's segment: its list's padded rows
         float* out        = P.out_score + item.out_off;
         for (uint32_t t = 0; t < item.n_tiles; ++t) {
-          wait_dbg(P.dbg, &d_full[ds], dph, 0x204, static_cast<uint32_t>(it), t);
+          ptx::mbar_wait(&d_full[ds], dph);
           float d[MN / 2];
           pq_tile_mma<MN, kQM, NKB, PASSES>(d, ds, L::dec_stage >> 4, d_lo0, x_lo0, q_lo0, L::q_tile >> 4, ones_lo);
           __syncwarp();
@@ -631,13 +594,13 @@ pq_stream_scan_kernel(const __grid_constant__ CUtensorMap tmQ_hi, const __grid_c
           sCnt[i] = 0;
         }
         ptx::named_bar_sync(1, kEpiThreads);
-        wait_dbg(P.dbg, q_full, qph, 0x202, static_cast<uint32_t>(it), 0);
+        ptx::mbar_wait(q_full, qph);
 
         // ping-pong: this warpgroup's tiles of the item are t0, t0 + 2, ...; it may have none (an item of one tile)
         const uint32_t t0 = kPP ? (wg ^ (g0 & 1u)) : 0, tstep = kPP ? 2 : 1;
         if (kPP && t0 >= item.n_tiles && lane == 0) ptx::mbar_arrive(q_empty);
         for (uint32_t t = t0; t < item.n_tiles; t += tstep) {
-          wait_dbg(P.dbg, &d_full[ds], dph, 0x204, static_cast<uint32_t>(it), t);
+          ptx::mbar_wait(&d_full[ds], dph);
           float d[MN / 2];
           pq_tile_mma<MN, kQM, NKB, PASSES>(d, ds, L::dec_stage >> 4, d_lo0, x_lo0, q_lo0, L::q_tile >> 4, ones_lo);
           __syncwarp();
@@ -838,43 +801,15 @@ void launch(cudaStream_t stream, int sms, const CUtensorMap& mq_hi, const CUtens
   a.cstages = std::min(kMaxCStages, (kSmemLimit - fixed) / a.blk);
   B2_EXPECTS(a.cstages >= 2, "pq_stream_scan: shared memory budget exceeded (NQ=%d KC=%d passes=%d)", NQ, a.KC, PASSES);
   const size_t smem = static_cast<size_t>(fixed) + static_cast<size_t>(a.cstages) * a.blk;
-  static uint32_t* dbg_host = nullptr;  // CUVS_B200_PQ_DEBUG=1: deadlock report (see wait_dbg)
-  if (env_int("CUVS_B200_PQ_DEBUG", 0)) {
-    if (!dbg_host) B2_CUDA(cudaHostAlloc(reinterpret_cast<void**>(&dbg_host), 16 * sizeof(uint32_t) * 1024, cudaHostAllocMapped));
-    memset(dbg_host, 0, 16 * sizeof(uint32_t) * 1024);
-    uint32_t* dptr = nullptr;
-    B2_CUDA(cudaHostGetDevicePointer(reinterpret_cast<void**>(&dptr), dbg_host, 0));
-    a.dbg = dptr;
-    a.dbg_mode = env_int("CUVS_B200_PQ_DEBUG", 0);
+  if (env_int("CUVS_B200_PQ_DEBUG", 0))  // the launch configuration, on stderr
     fprintf(stderr, "[pq_stream_scan] NQ=%d NKB=%d PASSES=%d KC=%d cap=%d cstages=%d blk=%d smem=%zu items<=%d\n", NQ, NKB, PASSES, a.KC, a.cap,
             a.cstages, a.blk, smem, n_items);
-  }
   B2_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
   const int grid = n_items < sms ? n_items : sms;
   timed_section ts("pq_stream_scan", stream);
   count_launch();
   kern<<<grid, kThreads, smem, stream>>>(mq_hi, mq_lo, a);
   B2_CUDA(cudaGetLastError());
-  if (a.dbg != nullptr) {
-    cudaError_t e = cudaErrorNotReady;
-    for (int i = 0; i < 80 && e == cudaErrorNotReady; ++i) {  // poll for ~8 s: a hang must not block the host forever
-      e = cudaStreamQuery(stream);
-      if (e == cudaErrorNotReady) usleep(100000);
-    }
-    int shown = 0;
-    for (int b = 0; b < grid && b < 1024 && shown < 6; ++b)
-      if (dbg_host[b * 16] || e != cudaSuccess) {
-        ++shown;
-        fprintf(stderr, "[pq_stream_scan] CTA %d: stuck wait 0x%x parity %u a=%u b=%u warp %u\n", b, dbg_host[b * 16],
-                dbg_host[b * 16 + 1], dbg_host[b * 16 + 2], dbg_host[b * 16 + 3], dbg_host[b * 16 + 4]);
-      }
-    if (e == cudaErrorNotReady) {
-      fprintf(stderr, "[pq_stream_scan] kernel still running after 8 s: giving up (process exits)\n");
-      fflush(stderr);
-      _exit(3);
-    }
-    B2_EXPECTS(e == cudaSuccess, "pq_stream_scan (debug): kernel failed: %s", cudaGetErrorString(e));
-  }
 }
 
 }  // namespace

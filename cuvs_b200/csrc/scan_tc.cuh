@@ -46,9 +46,9 @@ constexpr int tc_bound_init_byte = 0x7f;  // memset value: 0x7f7f7f7f decodes to
 inline int tc_pad_k(int d) { return (d + 63) / 64 * 64; }
 inline int64_t tc_pad_rows(int64_t n) { return (n + kTcTile - 1) / kTcTile * kTcTile; }
 
-/** Candidate lists the kernel emits per (item, query row): 2 (two epilogue threads per accumulator row, each owning
- *  64 of the tile's 128 columns).  Every list holds KC entries; list j sits at +j*KC. */
-int tc_lists_per_item();
+/** Candidate lists the kernel emits per (item, query row): two epilogue threads per accumulator row, each owning
+ *  64 of the tile's 128 columns.  Every list holds KC entries; list j sits at +j*KC. */
+constexpr int kTcListsPerItem = 2;
 
 /** True when the device/shape combination is served by the wgmma kernel (sm_90, padded dim <= kTcMaxK). */
 bool tc_supported(int device, int d);
@@ -70,7 +70,7 @@ void tc_half_norms(cudaStream_t stream, const float* xn, int64_t n, int64_t rows
 void tc_pack_half_norms(cudaStream_t stream, const float* hn, int64_t rows_pad, __nv_bfloat16* hx);
 
 /**
- * Run the scan.  For every item and every valid row r the kernel writes tc_lists_per_item() lists of KC
+ * Run the scan.  For every item and every valid row r the kernel writes kTcListsPerItem lists of KC
  * (score, position) pairs, each sorted best-first, at out_off + r * out_row_stride (+0..lists*KC-1); empty slots hold
  * (+inf, 0xffffffff).  `passes` = 3 uses hi*hi + lo*hi + hi*lo (fp32-grade products), 2 uses (hi + lo)*hi (exact when the B rows are
  * bf16 numbers, e.g. decoded PQ rows), 1 uses hi*hi.
