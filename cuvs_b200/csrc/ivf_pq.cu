@@ -43,6 +43,7 @@
 #include <cuda_fp16.h>
 
 #include <algorithm>
+#include <atomic>
 #include <cfloat>
 #include <cmath>
 #include <cstdlib>
@@ -760,6 +761,21 @@ ivf_pq_index* ivf_pq_build(resources* res, const cuvsIvfPqIndexParams& p, const 
   return idx.release();
 }
 
+// Test hook (cuvsB200IvfPqKeepPrimedBounds): the calling thread's last bounds as the pre-pass left them, before the scan
+std::atomic<int> g_keep_primed{0};
+thread_local std::vector<float> t_primed;
+void keep_primed_bounds(cudaStream_t s, const int* bkeys, int64_t nq)
+{
+  std::vector<int> keys(static_cast<size_t>(nq));
+  B2_CUDA(cudaMemcpyAsync(keys.data(), bkeys, sizeof(int) * nq, cudaMemcpyDeviceToHost, s));
+  B2_CUDA(cudaStreamSynchronize(s));
+  t_primed.resize(keys.size());
+  for (size_t i = 0; i < keys.size(); ++i) {
+    const int kb = keys[i] >= 0 ? keys[i] : keys[i] ^ 0x7fffffff;
+    std::memcpy(&t_primed[i], &kb, sizeof(float));
+  }
+}
+
 // The fine scan of one search (DESIGN.md §5), decided in one place before any work is queued.  env is CUVS_B200_PQ_PATH: lut,
 // tc (the default choice) or stream, read on every search because tests switch paths inside one process.  reduced: lut_dtype or
 // internal_distance_dtype is not fp32.  dense: the index also caches decoded rows, k <= 32, env != stream and the batch sends
@@ -939,6 +955,16 @@ void ivf_pq_search(resources* res, const ivf_pq_index& idx, const cuvsIvfPqSearc
     bnd.add   = add.data();
     bnd.scale = scale;
     bnd.kth   = k;  // only the query's k best survive the merge below
+    // every query starts the scan with a finite bound instead of waiting for its first finished item (DESIGN.md §5)
+    if (plan.path == scan_path::stream && bkeys.data() != nullptr && pq_stream_bound_enabled()) {
+      {
+        timed_section tp("pq_bound_prime", s);
+        pq_bound_prime(s, res->device, idx.cstream.data(), idx.cb_words.data(), idx.pq_dim, a.hi.data(), a.lo.data(), idx.Kp,
+                       plan.passes, pb.slot_of.data(), pb.pair_list.data(), idx.lists.d_offsets.data(), add.data(), scale, nq,
+                       static_cast<int>(n_probes), k, bkeys.data());
+      }
+      if (g_keep_primed.load()) keep_primed_bounds(s, bkeys.data(), nq);
+    }
     timed_section ts("pq_scan", s);
     if (plan.path == scan_path::stream)
       pq_stream_scan(s, res->device, a.hi.data(), a.lo.data(), a.rows, idx.Kp, idx.cstream.data(), idx.cb_words.data(), idx.pq_dim,
@@ -1026,6 +1052,15 @@ cuvsError_t cuvsIvfPqIndexDestroy(cuvsIvfPqIndex_t index)
     delete reinterpret_cast<ivf_pq_index*>(index->addr);
     delete index;
   });
+}
+
+void cuvsB200IvfPqKeepPrimedBounds(int on) { g_keep_primed.store(on); }
+
+int64_t cuvsB200IvfPqPrimedBounds(float* out, int64_t cap)
+{
+  const int64_t n = static_cast<int64_t>(t_primed.size());
+  if (out) std::memcpy(out, t_primed.data(), sizeof(float) * static_cast<size_t>(std::max<int64_t>(0, std::min(n, cap))));
+  return n;
 }
 
 cuvsError_t cuvsB200IvfPqIndexInfo(cuvsIvfPqIndex_t index, int* path, int64_t* device_bytes)

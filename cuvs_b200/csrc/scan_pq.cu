@@ -732,6 +732,195 @@ __global__ void __launch_bounds__(128) pq_stream_to_flat_kernel(const uint8_t* _
   for (int o = threadIdx.x; o < 128 * pq_dim / 16; o += blockDim.x) out[o] = reinterpret_cast<const uint4*>(sc)[o];
 }
 
+// ------------------------------------------------------------------------------------ pruning-bound pre-pass
+// One warp per query (grid-stride).  The query's first n_pair_probes live probes (probes are in rank order: nearest first), the
+// first n_tiles tiles of each probe's list: every row scored in fp32, s = hn - r.y, by the decode warps' gather (lane l owns
+// subspaces l + 32 h, 16 rows per 128-bit code load) and a shuffle reduce-scatter that leaves row 16 g + lane / 2 on the even
+// lanes.  Each row's score is raised by the margin below and turned into a distance as the merge does (fmaf(scale, s, add));
+// every even lane keeps its kPrimeKeep smallest, and the k-th smallest of those kept values -- if finite, at least k rows lie at or
+// below it -- is raised once more and min-ed into the query's bound.  DESIGN.md §5 ("Bound pre-pass") gives the argument.
+constexpr int kPrimeWarps = 8;
+constexpr int kPrimeKeep  = 4;  // per even lane: 16 lanes x 4 >= 64 >= k
+
+// One step of the reduce-scatter of 2N per-lane partial sums over lane bit 2N: the lane keeps the N rows its bit selects,
+// summed with its partner's.  (selp in asm: a plain select between two elements becomes a computed index into local memory.)
+template <int N>
+__device__ __forceinline__ void prime_reduce_step(float (&part)[16], int lane)
+{
+  const uint32_t up = (lane & (2 * N)) != 0 ? 1u : 0u;
+#pragma unroll
+  for (int i = 0; i < N; ++i) {
+    float give, keep;
+    asm("{\n\t.reg .pred p;\n\tsetp.ne.u32 p, %4, 0;\n\tselp.f32 %0, %2, %3, p;\n\tselp.f32 %1, %3, %2, p;\n\t}"
+        : "=f"(give), "=f"(keep) : "f"(part[i]), "f"(part[i + N]), "r"(up));
+    part[i] = keep + __shfl_xor_sync(0xffffffffu, give, 2 * N);
+  }
+}
+
+template <int NKB, int PASSES>
+__global__ void __launch_bounds__(32 * kPrimeWarps, 3)  // (3 CTAs per SM: shared memory allows 3, see pq_bound_prime)
+pq_bound_prime_kernel(const uint8_t* __restrict__ stream, const uint32_t* __restrict__ cb_words, const __nv_bfloat16* __restrict__ q_hi,
+                      const __nv_bfloat16* __restrict__ q_lo, const uint32_t* __restrict__ slot_of, const uint32_t* __restrict__ pair_list,
+                      const int64_t* __restrict__ list_offsets, const float* __restrict__ add, float scale, int64_t nq, int n_probes,
+                      int n_pair_probes, int n_tiles, int k, int* __restrict__ b_keys)
+{
+  constexpr int Kp    = 64 * NKB;     // residual columns: 2 per subspace, pq_dim = 32 NKB
+  constexpr int codes = 4096 * NKB;   // code bytes of a tile block, followed by the 128 half-norms
+  constexpr int blk   = codes + 512;
+  extern __shared__ __align__(16) uint32_t sCbw[];  // [NKB][256][32] codebook words, then ymax[Kp]
+  float* sYmax = reinterpret_cast<float*>(sCbw + NKB * 8192);
+  for (int i = threadIdx.x; i < NKB * 8192 / 4; i += blockDim.x)
+    reinterpret_cast<uint4*>(sCbw)[i] = reinterpret_cast<const uint4*>(cb_words)[i];
+  __syncthreads();
+  // ymax[c] = max over codes of |entry| of column c (column 2 j + e = component e of subspace j): with it,
+  // sum_j |r_j y_j| <= sum_j |r_j| ymax_j for every row of the query's lists
+  // (every thread: one column, one 1/nsplit of the codes; the partial maxima meet in shared memory as non-negative floats,
+  // whose bit patterns order like the floats)
+  for (int c = threadIdx.x; c < Kp; c += blockDim.x) sYmax[c] = 0.f;
+  __syncthreads();
+  {
+    constexpr int nsplit = 32 * kPrimeWarps / Kp;
+    const int c = threadIdx.x % Kp, part = threadIdx.x / Kp;
+    const int j = c >> 1, h = j >> 5, l = j & 31;
+    float m = 0.f;
+#pragma unroll 8
+    for (int code = part; code < 256; code += nsplit) {
+      const uint32_t w = sCbw[(h * 256 + code) * 32 + l];
+      m = fmaxf(m, fabsf(__uint_as_float((c & 1) ? (w & 0xffff0000u) : (w << 16))));
+    }
+    atomicMax(reinterpret_cast<int*>(sYmax) + c, __float_as_int(m));
+  }
+  __syncthreads();
+
+  const int lane = threadIdx.x & 31;
+  const uint32_t cb_lane = ptx::smem_u32(sCbw) + static_cast<uint32_t>(lane) * 4u;
+  for (int64_t q = blockIdx.x * static_cast<int64_t>(kPrimeWarps) + (threadIdx.x >> 5); q < nq; q += gridDim.x * static_cast<int64_t>(kPrimeWarps)) {
+    const uint32_t* slots = slot_of + q * n_probes;
+    // M = max |add| over the query's pairs: every pair converts the bound back to a threshold with its own add
+    float amax = 0.f;
+    for (int p = lane; p < n_probes; p += 32) {
+      const uint32_t s = slots[p];
+      if (s != 0xffffffffu) amax = fmaxf(amax, fabsf(add[s]));
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, o));
+
+    float best[kPrimeKeep];
+#pragma unroll
+    for (int j = 0; j < kPrimeKeep; ++j) best[j] = INFINITY;
+    int taken = 0;
+    for (int p = 0; p < n_probes && taken < n_pair_probes; ++p) {
+      const uint32_t slot = slots[p];
+      if (slot == 0xffffffffu) continue;
+      ++taken;
+      const float a = add[slot];
+      // this lane's residual columns 64 h + 2 lane + {0, 1} (one bf16x2 word per plane), and A = sum_j |r_j| ymax_j
+      float r[NKB][2][PASSES];
+      float A = 0.f;
+#pragma unroll
+      for (int h = 0; h < NKB; ++h)
+#pragma unroll
+        for (int pl = 0; pl < PASSES; ++pl) {
+          const __nv_bfloat16* src = pl == 0 ? q_hi : q_lo;
+          const uint32_t w = *reinterpret_cast<const uint32_t*>(src + static_cast<int64_t>(slot) * Kp + 64 * h + 2 * lane);
+          r[h][0][pl] = __uint_as_float(w << 16);
+          r[h][1][pl] = __uint_as_float(w & 0xffff0000u);
+          A = fmaf(fabsf(r[h][0][pl]), sYmax[64 * h + 2 * lane], A);
+          A = fmaf(fabsf(r[h][1][pl]), sYmax[64 * h + 2 * lane + 1], A);
+        }
+#pragma unroll
+      for (int o = 16; o > 0; o >>= 1) A += __shfl_xor_sync(0xffffffffu, A, o);
+      const uint32_t l   = pair_list[slot];
+      const int64_t row0 = list_offsets[l];
+      const int nt       = static_cast<int>(min(static_cast<int64_t>(n_tiles), (list_offsets[l + 1] - row0) / 128));
+      // 16-row groups of the scored tiles in order; the codes and half-norm of the next group load while this one is scored
+      const uint8_t* first = stream + (row0 / 128) * blk;
+      auto group_codes = [&](int tg, int h) {
+        return *reinterpret_cast<const uint4*>(first + (tg >> 3) * blk + (tg & 7) * (NKB * 512) + h * 512 + lane * 16);
+      };
+      auto group_hn = [&](int tg) { return reinterpret_cast<const float*>(first + (tg >> 3) * blk + codes)[16 * (tg & 7) + (lane >> 1)]; };
+      uint4 nxt[NKB];
+      float nxt_hn = 0.f;
+      if (nt > 0) {
+#pragma unroll
+        for (int h = 0; h < NKB; ++h) nxt[h] = group_codes(0, h);
+        nxt_hn = group_hn(0);
+      }
+      for (int tg = 0; tg < 8 * nt; ++tg) {
+        uint4 cur[NKB];
+#pragma unroll
+        for (int h = 0; h < NKB; ++h) cur[h] = nxt[h];
+        const float hn = nxt_hn;
+        if (tg + 1 < 8 * nt) {
+#pragma unroll
+          for (int h = 0; h < NKB; ++h) nxt[h] = group_codes(tg + 1, h);
+          nxt_hn = group_hn(tg + 1);
+        }
+        {
+          float part[16];
+#pragma unroll
+          for (int i = 0; i < 16; ++i) part[i] = 0.f;
+#pragma unroll
+          for (int h = 0; h < NKB; ++h) {
+            const uint4 cw = cur[h];
+            const uint32_t w4[4] = {cw.x, cw.y, cw.z, cw.w};
+#pragma unroll
+            for (int i = 0; i < 16; ++i) {
+              const uint32_t c = __byte_perm(w4[i >> 2], 0u, 0x4440u | static_cast<uint32_t>(i & 3));
+              uint32_t w;
+              asm("ld.shared.u32 %0, [%1];" : "=r"(w) : "r"(cb_lane + static_cast<uint32_t>(h) * 32768u + (c << 7)));
+              const float e0 = __uint_as_float(w << 16), e1 = __uint_as_float(w & 0xffff0000u);
+#pragma unroll
+              for (int pl = 0; pl < PASSES; ++pl) {
+                part[i] = fmaf(r[h][0][pl], e0, part[i]);
+                part[i] = fmaf(r[h][1][pl], e1, part[i]);
+              }
+            }
+          }
+          prime_reduce_step<8>(part, lane);
+          prime_reduce_step<4>(part, lane);
+          prime_reduce_step<2>(part, lane);
+          prime_reduce_step<1>(part, lane);
+          const float dot = part[0] + __shfl_xor_sync(0xffffffffu, part[0], 1);  // row 16 (tg % 8) + lane / 2 of the tile
+          if ((lane & 1) == 0 && hn < INFINITY) {  // (padding rows: hn = +inf)
+            const float sp = hn - dot;
+            const float m  = __fmul_ru(0x1p-12f, __fadd_ru(fabsf(hn), A));
+            float u        = __fmaf_rn(scale, __fadd_ru(sp, m), a);
+#pragma unroll
+            for (int j = 0; j < kPrimeKeep; ++j) {
+              const float lo = fminf(best[j], u);
+              u              = fmaxf(best[j], u);
+              best[j]        = lo;
+            }
+          }
+        }
+      }
+    }
+    // k-th smallest of the kept values (odd lanes keep +inf): bisection over the order-preserving keys, the smallest key with
+    // at least k kept keys at or below it, i.e. the k-th smallest kept value itself
+    uint32_t key[kPrimeKeep];
+#pragma unroll
+    for (int j = 0; j < kPrimeKeep; ++j) key[j] = okey(__float_as_uint(best[j]));
+    uint32_t lo = 0u, hi = 0xffffffffu;
+    while (lo < hi) {  // (warp-uniform)
+      const uint32_t mid = lo + ((hi - lo) >> 1);
+      uint32_t c = 0;
+#pragma unroll
+      for (int j = 0; j < kPrimeKeep; ++j) c += key[j] <= mid ? 1u : 0u;
+      if (__reduce_add_sync(0xffffffffu, c) >= static_cast<uint32_t>(k)) hi = mid;
+      else lo = mid + 1u;
+    }
+    const float kth = __uint_as_float(okey_inv(lo));
+    if (lane == 0 && kth < INFINITY) {
+      const float B = __fadd_ru(__fadd_ru(kth, __fmul_ru(0x1p-21f, __fadd_ru(fabsf(kth), amax))), 1e-30f);
+      if (B < INFINITY) {
+        const int kb = __float_as_int(B);
+        atomicMin(b_keys + q, kb >= 0 ? kb : kb ^ 0x7fffffff);
+      }
+    }
+  }
+}
+
 __global__ void pq_cb_words_kernel(const float* __restrict__ pq_centers, int pq_dim, uint32_t* __restrict__ words)
 {
   const int t = blockIdx.x * blockDim.x + threadIdx.x;
@@ -844,6 +1033,36 @@ void pq_stream_to_flat(cudaStream_t s, const uint8_t* stream, int64_t rows_total
   B2_CUDA(cudaGetLastError());
 }
 
+void pq_bound_prime(cudaStream_t s, int device, const uint8_t* code_stream, const uint32_t* cb_words, int pq_dim, const __nv_bfloat16* q_hi,
+                    const __nv_bfloat16* q_lo, int Kp, int passes, const uint32_t* slot_of, const uint32_t* pair_list, const int64_t* list_offsets,
+                    const float* add, float scale, int64_t nq, int n_probes, int k, int* b_keys)
+{
+  // Scored rows per query: the first 4 tiles (512 rows) of its nearest list.  Chosen by a sweep on the 50M x 128 flagship
+  // (DESIGN.md §5): scan + pre-pass was lowest at P = 1, T = 4; more tiles still shorten the scan, but past 4 each costs
+  // ~35 us per 10k queries (one more 8.7 KB tile per query, decoded by one warp), more than the scan then saves; a second
+  // list saved less than more tiles of the first.
+  constexpr int kPrimeProbes = 1, kPrimeTiles = 4;
+  if (nq == 0) return;
+  B2_EXPECTS(Kp == 2 * pq_dim && (pq_dim == 32 || pq_dim == 64), "pq_bound_prime: pq_dim must be 32 or 64 with pq_len 2 (Kp=%d)", Kp);
+  B2_EXPECTS(passes == 1 || (passes == 2 && q_lo != nullptr), "pq_bound_prime: passes must be 1, or 2 with a lo plane");
+  B2_EXPECTS(k >= 1 && k <= 16 * kPrimeKeep, "pq_bound_prime: k must be in [1, %d]", 16 * kPrimeKeep);
+  const int nkb      = pq_dim / 32;
+  const size_t smem  = static_cast<size_t>(nkb) * 32768 + static_cast<size_t>(nkb) * 64 * sizeof(float);
+  const int64_t need = (nq + kPrimeWarps - 1) / kPrimeWarps;
+  const int grid     = static_cast<int>(std::min<int64_t>(need, 3 * static_cast<int64_t>(sm_count_of(device))));  // 3 fit per SM
+  auto run = [&](auto kern) {
+    B2_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
+    count_launch();
+    kern<<<grid, 32 * kPrimeWarps, smem, s>>>(code_stream, cb_words, q_hi, q_lo, slot_of, pair_list, list_offsets, add, scale, nq, n_probes,
+                                              kPrimeProbes, kPrimeTiles, k, b_keys);
+  };
+  if (nkb == 1) passes == 1 ? run(pq_bound_prime_kernel<1, 1>) : run(pq_bound_prime_kernel<1, 2>);
+  else passes == 1 ? run(pq_bound_prime_kernel<2, 1>) : run(pq_bound_prime_kernel<2, 2>);
+  B2_CUDA(cudaGetLastError());
+}
+
+bool pq_stream_bound_enabled() { return env_int("CUVS_B200_PQ_NO_BOUND", 0) == 0; }
+
 int pq_stream_group(double pairs_per_list, int KC, int passes)
 {
   const int forced = env_int("CUVS_B200_PQ_GROUP", 0);  // tests and limiter experiments (read per call)
@@ -875,7 +1094,7 @@ void pq_stream_scan(cudaStream_t stream, int device, const __nv_bfloat16* q_hi, 
   a.out_score = out_score;
   a.out_pos = out_pos;
   a.out_row_stride = out_row_stride;
-  if (KC > 0 && bound != nullptr && bound->keys != nullptr && !env_int("CUVS_B200_PQ_NO_BOUND", 0)) {
+  if (KC > 0 && bound != nullptr && bound->keys != nullptr && pq_stream_bound_enabled()) {
     a.b_keys = bound->keys;
     a.b_idx = bound->idx;
     a.b_add = bound->add;

@@ -43,6 +43,10 @@ void pq_stream_build(cudaStream_t s, const uint8_t* codes, const int64_t* ids, i
 /** The flat form back from the stream: codes [rows_total, pq_dim], one code per byte (getters, extend, serialize, LUT path). */
 void pq_stream_to_flat(cudaStream_t s, const uint8_t* stream, int64_t rows_total, int pq_dim, uint8_t* codes);
 
+/** False when CUVS_B200_PQ_NO_BOUND is set (not "0"): the filtering scan then takes no pruning bound, and the search runs no
+ *  bound pre-pass (pq_bound_prime). */
+bool pq_stream_bound_enabled();
+
 /** Queries per work item the scan wants for an average of `pairs_per_list` probing queries per list (32, 64 or 128);
  *  KC = 0 (store epilogue) is not limited by candidate buffers. */
 int pq_stream_group(double pairs_per_list, int KC, int passes);
@@ -59,5 +63,18 @@ void pq_stream_scan(cudaStream_t stream, int device, const __nv_bfloat16* q_hi, 
                     const uint8_t* code_stream, const uint32_t* cb_words, int pq_dim, const tc_item* items_dev, int n_items,
                     const int* n_items_dev, int group, int KC, int passes, float* out_score, uint32_t* out_pos, int64_t out_row_stride,
                     const tc_bound* bound);
+
+/**
+ * Pruning-bound pre-pass of the filtering scan (KC > 0 with a bound): for each of the nq queries, scores the first rows of
+ * its nearest probed list(s) in fp32 from the code stream and the pair's residual rows (q_hi, and q_lo with two passes), and
+ * atomically lowers b_keys[q] (tc_bound key encoding, distance units: add[slot] + scale * score) to a value that is at least
+ * the k-th best distance pq_stream_scan and the merge will find among those rows, raised far enough that every row of the
+ * query's final top k still passes each item's starting threshold (DESIGN.md §5).  slot_of [nq, n_probes] (probes in rank
+ * order), pair_list [slots], list_offsets [n_lists + 1] (padded row offsets), add [slots]; residual rows [slots, Kp] with
+ * Kp = 2 * pq_dim; k <= 64.
+ */
+void pq_bound_prime(cudaStream_t s, int device, const uint8_t* code_stream, const uint32_t* cb_words, int pq_dim, const __nv_bfloat16* q_hi,
+                    const __nv_bfloat16* q_lo, int Kp, int passes, const uint32_t* slot_of, const uint32_t* pair_list, const int64_t* list_offsets,
+                    const float* add, float scale, int64_t nq, int n_probes, int k, int* b_keys);
 
 }  // namespace b200

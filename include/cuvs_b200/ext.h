@@ -49,6 +49,11 @@ CUVS_EXPORT cuvsError_t cuvsB200IvfFlatSetCenters(cuvsResources_t res, cuvsIvfFl
  * decoded bf16 rows (decoded-row wgmma scan, scan_tc.cu; on a streamed index: the small-index cache used by densely probing
  * batches), 0 = LUT kernel only. */
 CUVS_EXPORT cuvsError_t cuvsB200IvfPqIndexInfo(cuvsIvfPqIndex_t index, int* path, int64_t* device_bytes);
+/* IVF-PQ bound pre-pass (DESIGN.md §5): with on != 0, every later code-stream search that runs the pre-pass keeps, for the
+ * calling thread, each query's pruning bound (distance units; 3.39e38 = none) as the pre-pass left it, before the scan.
+ * cuvsB200IvfPqPrimedBounds copies up to cap of the last search's (last query batch's) bounds to out and returns their count. */
+CUVS_EXPORT void cuvsB200IvfPqKeepPrimedBounds(int on);
+CUVS_EXPORT int64_t cuvsB200IvfPqPrimedBounds(float* out, int64_t cap);
 
 /* ---- multi-GPU exchange step (one process per GPU; DESIGN.md §7) ------------------------------------------------
  * The index is sharded by IVF list: every rank searches the lists it owns for the whole query batch and holds a partial
