@@ -240,16 +240,33 @@ __global__ void make_list_items_kernel(const uint32_t* __restrict__ counts, cons
   }
 }
 
-__global__ void gather_rows_kernel(const uint4* __restrict__ src, const uint32_t* __restrict__ pair_query,
-                                   const int* __restrict__ n_live, int64_t rows_total, int vec_per_row, uint4* __restrict__ dst)
+// per pair: r = q[query] - c[list] (L2) or q[query] (IP) as bf16 A rows; add[slot] = |r|^2 (L2) or -(q . c) (IP: the B rows
+// hold residuals, so the centre's part of q . x is the pair's).  Cosine (q and c already unit) adds 1 to the offset, so that
+// every reader of `add` sees cosine distances 1 - q.c - q.(x - c).
+__global__ void pair_rows_kernel(const float* __restrict__ q, const float* __restrict__ centers,
+                                 const uint32_t* __restrict__ pair_query, const uint32_t* __restrict__ pair_list,
+                                 const int* __restrict__ n_live, int64_t rows_total, int dim, int Kp, bool ip,
+                                 __nv_bfloat16* __restrict__ a_hi,
+                                 __nv_bfloat16* __restrict__ a_lo, float* __restrict__ add, bool cosine)
 {
-  int64_t t = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x;
-  if (t >= rows_total * vec_per_row) return;
-  int64_t r = t / vec_per_row;
-  int v     = static_cast<int>(t % vec_per_row);
-  uint4 val = make_uint4(0, 0, 0, 0);
-  if (r < *n_live) val = src[static_cast<int64_t>(pair_query[r]) * vec_per_row + v];
-  dst[t] = val;
+  int64_t r = (blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x) >> 5;
+  int lane  = threadIdx.x & 31;
+  if (r >= rows_total) return;
+  float nrm = 0.f;
+  const bool live = r < *n_live;
+  const float* qr = live ? q + static_cast<int64_t>(pair_query[r]) * dim : nullptr;
+  const float* cr = live ? centers + static_cast<int64_t>(pair_list[r]) * dim : nullptr;
+  for (int j = lane; j < Kp; j += 32) {
+    float v = 0.f;
+    if (live && j < dim) v = ip ? qr[j] : qr[j] - cr[j];
+    __nv_bfloat16 h = __float2bfloat16_rn(v);
+    a_hi[r * Kp + j] = h;
+    if (a_lo) a_lo[r * Kp + j] = __float2bfloat16_rn(v - __bfloat162float(h));
+    nrm = ip ? ((live && j < dim) ? fmaf(-qr[j], cr[j], nrm) : nrm) : fmaf(v, v, nrm);
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) nrm += __shfl_xor_sync(0xffffffffu, nrm, o);
+  if (lane == 0 && live) add[r] = cosine ? nrm + 1.0f : nrm;
 }
 
 // out[q, p*KCW + c] = add[slot] + scale * s   (per-query concatenation of its probes' candidates; `empty` where there is none)
@@ -746,14 +763,19 @@ void bucket_probes(resources* res, const uint32_t* probes, int64_t nq, int n_pro
   B2_CUDA(cudaGetLastError());
 }
 
-void gather_rows_bf16(cudaStream_t s, const __nv_bfloat16* src, const uint32_t* pair_query, const int* n_live, int64_t rows_total,
-                      int Kp, __nv_bfloat16* dst)
+float pair_residual_rows(cudaStream_t s, const float* q, const float* centers, int dim, int Kp, cuvsDistanceType metric,
+                         const probe_buckets& pb, bool with_lo, residual_rows& a, dbuf<float>& add)
 {
-  const int vec = Kp * 2 / 16;
+  const bool ip = is_ip(metric);
+  a.rows        = pb.n_pairs + 128;
+  a.hi.alloc(static_cast<size_t>(a.rows) * Kp, s);
+  if (with_lo) a.lo.alloc(static_cast<size_t>(a.rows) * Kp, s);
+  add.alloc(static_cast<size_t>(pb.n_pairs), s);
   count_launch();
-  gather_rows_kernel<<<blocks_for(rows_total * vec, 256), 256, 0, s>>>(reinterpret_cast<const uint4*>(src), pair_query, n_live,
-                                                                        rows_total, vec, reinterpret_cast<uint4*>(dst));
+  pair_rows_kernel<<<blocks_for(a.rows * 32, 256), 256, 0, s>>>(q, centers, pb.pair_query.data(), pb.pair_list.data(), pb.n_items.data() + 1,
+                                                                 a.rows, dim, Kp, ip, a.hi.data(), a.lo.data(), add.data(), metric == CosineExpanded);
   B2_CUDA(cudaGetLastError());
+  return ip ? 1.0f : 2.0f;
 }
 
 void gather_probe_candidates(cudaStream_t s, const float* cs, const uint32_t* cp, const uint32_t* slot_of, const float* add,

@@ -71,9 +71,21 @@ void bucket_probes(resources* res, const uint32_t* probes, int64_t nq, int n_pro
                    uint32_t max_tiles = 0xffffffffu /*scan at most this many tiles of each list (bound warm-up)*/,
                    int group = 128 /*pairs (A rows) per work item*/);
 
-/** Gather bf16 rows: dst[slot] = src[pair_query[slot]] (Kp elements each); rows >= *n_live are zeroed up to rows_total. */
-void gather_rows_bf16(cudaStream_t s, const __nv_bfloat16* src, const uint32_t* pair_query, const int* n_live, int64_t rows_total,
-                      int Kp, __nv_bfloat16* dst);
+/** The A rows of an IVF fine scan, one per pair slot (slots of dropped pairs are never read; the 128 rows past the pairs are
+ *  zero). */
+struct residual_rows {
+  int64_t rows = 0;
+  dbuf<__nv_bfloat16> hi, lo;
+};
+/**
+ * Per pair slot, for a scan of list rows that hold residuals x - c (with half norms |x - c|^2/2 for L2, 0 otherwise), from the
+ * fp32 query rows q [nq, dim] and list centres [n_lists, dim] (cosine: both unit): bf16 planes of q - c (L2) or q (inner
+ * product, cosine), hi and, `with_lo`, lo, and add[slot], the pair's offset: |q - c|^2 (L2), -q.c (inner product), 1 - q.c
+ * (cosine).  Returns `scale`: a pair's distance is add[slot] + scale * score, 2 for L2 (|q - x|^2 = |q - c|^2 +
+ * 2 (|x - c|^2/2 - (q - c).(x - c))) and 1 otherwise.  Scores of different pairs are only comparable in these units.
+ */
+float pair_residual_rows(cudaStream_t s, const float* q, const float* centers, int dim, int Kp, cuvsDistanceType metric,
+                         const probe_buckets& pb, bool with_lo, residual_rows& a, dbuf<float>& add);
 
 /**
  * Per query, concatenate the KCW candidates of each of its probes: out [nq, n_probes * KCW], value add[slot] + scale * score

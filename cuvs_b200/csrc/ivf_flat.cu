@@ -10,7 +10,7 @@
 // Search (DESIGN.md §4):
 //   1. coarse: dense wgmma score block queries x centres (split-bf16, fp32-grade) + select_k(n_probes)
 //   2. (query, probe) pairs are bucketed by list on the device (ivf_common.cu)
-//   3. fine:   per (list, <=128 probing queries) work item, wgmma scan of the list's bf16 rows with the
+//   3. fine:   per (list, <=128 probing queries) work item, wgmma scan of the list's bf16 residual rows x - c with the
 //              fused top-k' epilogue — each list tile is read once per 128 probing queries, not once per query.
 //              k > 64: the same scan with the store epilogue writes every (pair, list row) score to the pair's dense
 //              segment, and a segmented select keeps each pair's kc2 = min(2k, 2048) best (the reference's non-fused
@@ -48,17 +48,59 @@ struct ivf_flat_index {
   uint32_t kmeans_n_iters = 20;
   double kmeans_trainset_fraction = 0.5;
   owned<float> centers;  // [n_lists, dim]
+  owned<float> centers_unit;  // cosine: [n_lists, dim] the unit centres the scan's residuals are taken from
   tc_rows centers_tc;    // split planes + |c|^2/2 (0 for inner product)
   list_layout lists;
   owned<float> data;         // [rows_total, dim], list-major, zero padding rows
   owned<int64_t> ids;        // [rows_total], kPadId on padding rows
-  owned<float> xn;           // [rows_total] |x|^2 (cosine / certificate use)
-  owned<__nv_bfloat16> hi;   // [rows_total, Kp] bf16 rows (normalised for cosine)
-  owned<__nv_bfloat16> hx;   // [rows_total, 16] half-norm plane: |x|^2/2, +inf on padding rows (scan_tc.cuh)
+  owned<float> xn;           // [rows_total] |x|^2 (the exact re-score)
+  owned<float> rn;           // [rows_total] |x - c|^2 of the residual rows below
+  owned<__nv_bfloat16> hi;   // [rows_total, Kp] bf16 residuals x - c of each row's list centre (cosine: x/|x| - c/|c|)
+  owned<__nv_bfloat16> hx;   // [rows_total, 16] half-norm plane: |x - c|^2/2 (0 for inner product), +inf on padding rows (scan_tc.cuh)
+  // (cosine is scanned as L2 over the unit vectors, 2 - 2 q.x = |q - x|^2: the error then follows |q - c|, not |q| = 1)
   int Kp = 0;
 };
 
 namespace {
+
+// The centres the scan's residuals are taken from: the unit centres for cosine (the rows and queries are unit there too).
+const float* residual_centers(const ivf_flat_index& idx)
+{
+  return idx.metric == CosineExpanded ? idx.centers_unit.data() : idx.centers.data();
+}
+// The metric the scan ranks by: cosine ranks as L2 over unit vectors.
+cuvsDistanceType scan_metric(const ivf_flat_index& idx) { return idx.metric == CosineExpanded ? L2Expanded : idx.metric; }
+
+// One warp per list row: hi = bf16(x * scale - c_l) and rn = |x * scale - c_l|^2 (fp32), with l the row's list (the last with
+// offsets[l] <= row) and scale = row_scale[row] (null: 1).  Padding rows get a zero residual.
+__global__ void residual_rows_kernel(const float* __restrict__ x, const int64_t* __restrict__ ids, const float* __restrict__ row_scale,
+                                     int64_t rows, int dim, int Kp, const float* __restrict__ centers,
+                                     const int64_t* __restrict__ offsets, int64_t n_lists, __nv_bfloat16* __restrict__ hi,
+                                     float* __restrict__ rn)
+{
+  const int64_t r = (blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x) >> 5;
+  const int lane  = threadIdx.x & 31;
+  if (r >= rows) return;
+  const bool pad = ids[r] == kPadId;
+  int64_t lo = 0, up = n_lists;
+  while (up - lo > 1) {
+    const int64_t mid = (lo + up) >> 1;
+    if (offsets[mid] <= r) lo = mid;
+    else up = mid;
+  }
+  const float sc  = row_scale ? row_scale[r] : 1.f;
+  const float* xr = x + r * dim;
+  const float* cr = centers + lo * dim;
+  float nrm       = 0.f;
+  for (int j = lane; j < Kp; j += 32) {
+    const float v = (!pad && j < dim) ? xr[j] * sc - cr[j] : 0.f;
+    hi[r * Kp + j] = __float2bfloat16_rn(v);
+    nrm            = fmaf(v, v, nrm);
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) nrm += __shfl_xor_sync(0xffffffffu, nrm, o);
+  if (lane == 0) rn[r] = nrm;
+}
 
 __global__ void half_norms_masked_kernel(const float* __restrict__ xn, const int64_t* __restrict__ ids, int64_t n, bool zero,
                                          float* __restrict__ hn)
@@ -89,10 +131,12 @@ __global__ void drop_nonfinite_kernel(const float* __restrict__ score, uint32_t*
 
 // 32 < k <= 64 certificate: each pair kept only the KC best rows of each column half of its list.  A half that came back full
 // may have dropped rows, all scoring no better than its last kept entry; when that entry is strictly better than the query's
-// kc2-th merged candidate, a dropped row could have made the cut, and the query is flagged (flags[nq] counts them).
+// kc2-th merged candidate, a dropped row could have made the cut, and the query is flagged (flags[nq] counts them).  Entries are
+// compared in the merged candidates' units, add[slot] + scale * score.
 __global__ void flag_truncated_halves_kernel(const float* __restrict__ cs, const uint32_t* __restrict__ cp,
-                                             const uint32_t* __restrict__ slot_of, const float* __restrict__ ms, int64_t nq,
-                                             int n_probes, int KC, int KCW, int kc2, int* __restrict__ flags)
+                                             const uint32_t* __restrict__ slot_of, const float* __restrict__ add, float scale,
+                                             const float* __restrict__ ms, int64_t nq, int n_probes, int KC, int KCW, int kc2,
+                                             int* __restrict__ flags)
 {
   int64_t q = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x;
   if (q >= nq) return;
@@ -103,7 +147,7 @@ __global__ void flag_truncated_halves_kernel(const float* __restrict__ cs, const
     if (slot == 0xffffffffu) continue;
     for (int h = KC - 1; h < KCW; h += KC) {
       const int64_t e = static_cast<int64_t>(slot) * KCW + h;
-      if (cp[e] != 0xffffffffu && cs[e] < cut) flag = 1;
+      if (cp[e] != 0xffffffffu && add[slot] + scale * cs[e] < cut) flag = 1;
     }
   }
   flags[q] = flag;
@@ -130,6 +174,8 @@ void copy_rows(cudaStream_t s, const T* src, const int64_t* src_rows, T* dst, co
   B2_CUDA(cudaGetLastError());
 }
 
+// The scan's side of the list rows (DESIGN.md §4): bf16 residuals against the row's list centre and their half norms.  Rebuilt
+// whenever the rows change (extend, load); the centres change only while the index is empty.
 void refresh_tc_side(resources* res, ivf_flat_index& idx)
 {
   auto s          = res->stream;
@@ -138,6 +184,7 @@ void refresh_tc_side(resources* res, ivf_flat_index& idx)
   idx.hi.alloc(static_cast<size_t>(std::max<int64_t>(R, 128)) * idx.Kp);
   idx.hx.alloc(static_cast<size_t>(std::max<int64_t>(R, 128)) * 16);
   idx.xn.alloc(static_cast<size_t>(std::max<int64_t>(R, 128)));
+  idx.rn.alloc(static_cast<size_t>(std::max<int64_t>(R, 128)));
   if (R == 0) return;
   row_norms(s, idx.data.data(), R, idx.dim, idx.dim, idx.xn.data());
   dbuf<float> scale;
@@ -145,10 +192,12 @@ void refresh_tc_side(resources* res, ivf_flat_index& idx)
     scale.alloc(static_cast<size_t>(R), s);
     rsqrt_rows(s, idx.xn.data(), R, scale.data());
   }
-  tc_split_planes(s, idx.data.data(), R, idx.dim, idx.dim, idx.Kp, idx.hi.data(), nullptr, R, scale.data());
-  count_launch();
+  count_launch(2);
+  residual_rows_kernel<<<blocks_for(R * 32, 256), 256, 0, s>>>(idx.data.data(), idx.ids.data(), scale.data(), R, idx.dim, idx.Kp,
+                                                                residual_centers(idx), idx.lists.d_offsets.data(), idx.n_lists,
+                                                                idx.hi.data(), idx.rn.data());
   dbuf<float> hn(static_cast<size_t>(R), s);
-  half_norms_masked_kernel<<<blocks_for(R, 256), 256, 0, s>>>(idx.xn.data(), idx.ids.data(), R, !is_l2(idx.metric), hn.data());
+  half_norms_masked_kernel<<<blocks_for(R, 256), 256, 0, s>>>(idx.rn.data(), idx.ids.data(), R, !is_l2(scan_metric(idx)), hn.data());
   B2_CUDA(cudaGetLastError());
   tc_pack_half_norms(s, hn.data(), R, idx.hx.data());
 }
@@ -162,6 +211,9 @@ void refresh_centers_tc(resources* res, ivf_flat_index& idx)
   if (idx.metric == CosineExpanded) {
     scale.alloc(static_cast<size_t>(idx.n_lists), s);
     rsqrt_rows(s, cn.data(), idx.n_lists, scale.data());
+    idx.centers_unit.alloc(static_cast<size_t>(idx.n_lists) * idx.dim);
+    B2_CUDA(cudaMemcpyAsync(idx.centers_unit.data(), idx.centers.data(), sizeof(float) * idx.n_lists * idx.dim, cudaMemcpyDeviceToDevice, s));
+    normalize_rows(s, idx.centers_unit.data(), idx.n_lists, idx.dim, idx.dim);
   }
   idx.centers_tc.build(s, idx.centers.data(), idx.n_lists, idx.dim, is_l2(idx.metric) ? cn.data() : nullptr, true, scale.data());
 }
@@ -241,14 +293,14 @@ void ivf_flat_search(resources* res, const ivf_flat_index& idx, uint32_t n_probe
   // k > 64 (DESIGN.md §4 "k > 64"): the scan stores every (pair, list row) score and a segmented select keeps kc2 per pair
   const bool large_k = k > 64 || store;
   const int large_kc = std::min(2 * k, kSelectMaxK);
-  // Query batching.  Per (query, probe) pair: the gathered bf16 query row, 2 x KC candidate slots and their per-query
-  // concatenation.  k > 64, per query: dense scores (bounded by its n_probes largest lists), each pair's kc2 best and their
+  // Query batching.  Per (query, probe) pair: the bf16 query residual row and its offset, 2 x KC candidate slots and their
+  // per-query concatenation.  k > 64, per query: dense scores (bounded by its n_probes largest lists), each pair's kc2 best and their
   // per-query gather (8 + 8 bytes each), the gathered bf16 query rows, slot bookkeeping (32 bytes per pair) and the merged kc2.
   const int64_t large_k_bytes = !large_k ? 0
                                          : large_k_rows_per_query(idx.lists, n_probes) * 4 +
                                              static_cast<int64_t>(n_probes) * (16 * large_kc + 2 * idx.Kp + 32) +
                                              static_cast<int64_t>(large_kc) * 8;
-  const int64_t batch = query_batch_size(idx.Kp * 2 + 2 * 64 * 8 + 16, n_probes, large_k_bytes, "CUVS_B200_FLAT_LARGE_K_BUDGET_MB");
+  const int64_t batch = query_batch_size(idx.Kp * 2 + 4 + 2 * 64 * 8 + 16, n_probes, large_k_bytes, "CUVS_B200_FLAT_LARGE_K_BUDGET_MB");
   if (search_in_batches(batch, qt, nt, dt, [&](const DLTensor& qs, const DLTensor& ns, const DLTensor& ds) {
         ivf_flat_search(res, idx, n_probes, qs, ns, ds, keep_bits, n_bits, store);
       }))
@@ -278,7 +330,7 @@ void ivf_flat_search(resources* res, const ivf_flat_index& idx, uint32_t n_probe
     dbuf<float> hn(static_cast<size_t>(R), s);
     hx_f.alloc(static_cast<size_t>(std::max<int64_t>(R, 128)) * 16, s);
     count_launch();
-    half_norms_filtered_kernel<<<blocks_for(R, 256), 256, 0, s>>>(idx.xn.data(), idx.ids.data(), R, !is_l2(idx.metric), keep_bits, n_bits,
+    half_norms_filtered_kernel<<<blocks_for(R, 256), 256, 0, s>>>(idx.rn.data(), idx.ids.data(), R, !is_l2(scan_metric(idx)), keep_bits, n_bits,
                                                                    hn.data());
     B2_CUDA(cudaGetLastError());
     tc_pack_half_norms(s, hn.data(), R, hx_f.data());
@@ -297,10 +349,19 @@ void ivf_flat_search(resources* res, const ivf_flat_index& idx, uint32_t n_probe
   probe_buckets pb;
   bucket_probes(res, probes.data(), nq, static_cast<int>(n_probes), idx.n_lists, idx.lists.d_offsets.data(), KCW, pb);
 
-  // ---- 3. fine scan: gathered query rows (A) x list rows (B)
-  const int64_t a_rows = pb.n_pairs + 128;
-  dbuf<__nv_bfloat16> a_hi(static_cast<size_t>(a_rows) * idx.Kp, s);
-  gather_rows_bf16(s, qp.hi.data(), pb.pair_query.data(), pb.n_items.data() + 1, a_rows, idx.Kp, a_hi.data());
+  // ---- 3. fine scan: per-pair query residuals (A) x list residuals (B).  Scores of different pairs compare as distances,
+  // add[slot] + scale * score (pair_residual_rows); cosine scores the unit query as L2 (scan_metric).
+  const float* qf = q;
+  dbuf<float> q_unit;
+  if (idx.metric == CosineExpanded) {
+    q_unit.alloc(static_cast<size_t>(nq) * idx.dim, s);
+    B2_CUDA(cudaMemcpyAsync(q_unit.data(), q, sizeof(float) * nq * idx.dim, cudaMemcpyDeviceToDevice, s));
+    normalize_rows(s, q_unit.data(), nq, idx.dim, idx.dim);
+    qf = q_unit.data();
+  }
+  residual_rows a;
+  dbuf<float> add;
+  const float scale = pair_residual_rows(s, qf, residual_centers(idx), idx.dim, idx.Kp, scan_metric(idx), pb, false, a, add);
   dbuf<float> cs;
   dbuf<uint32_t> cp;
   if (large_k) {
@@ -308,21 +369,23 @@ void ivf_flat_search(resources* res, const ivf_flat_index& idx, uint32_t n_probe
     large_k_select(s, pb, idx.lists, nq, n_probes, large_kc, [&](float* scores, const int64_t* seg_off) {
       item_segments(s, pb, seg_off);
       timed_section ts("ivf_flat_scan", s);
-      tc_scan_topk(s, res->device, a_hi.data(), nullptr, a_rows, idx.hi.data(), nullptr, std::max<int64_t>(idx.lists.rows_total, 128),
+      tc_scan_topk(s, res->device, a.hi.data(), nullptr, a.rows, idx.hi.data(), nullptr, std::max<int64_t>(idx.lists.rows_total, 128),
                    idx.Kp, hx, pb.items.data(), pb.max_items, pb.n_items.data(), 0, 1, scores, nullptr, 0 /*per item*/);
     }, cs, cp);
     KCW = large_kc;
   } else {
     cs.alloc(static_cast<size_t>(pb.n_pairs) * KCW, s);
     cp.alloc(static_cast<size_t>(pb.n_pairs) * KCW, s);
-    // probes of one query share a running k'-th-best bound (same query => comparable scores)
+    // probes of one query share a running bound on its k'-th best distance, add[slot] + scale * score
     dbuf<int> bkeys(static_cast<size_t>(nq), s);
     B2_CUDA(cudaMemsetAsync(bkeys.data(), tc_bound_init_byte, sizeof(int) * nq, s));
     tc_bound bnd;
-    bnd.keys = bkeys.data();
-    bnd.idx  = pb.pair_query.data();
+    bnd.keys  = bkeys.data();
+    bnd.idx   = pb.pair_query.data();
+    bnd.add   = add.data();
+    bnd.scale = scale;
     timed_section ts("ivf_flat_scan", s);
-    tc_scan_topk(s, res->device, a_hi.data(), nullptr, a_rows, idx.hi.data(), nullptr, std::max<int64_t>(idx.lists.rows_total, 128),
+    tc_scan_topk(s, res->device, a.hi.data(), nullptr, a.rows, idx.hi.data(), nullptr, std::max<int64_t>(idx.lists.rows_total, 128),
                  idx.Kp, hx, pb.items.data(), pb.max_items, pb.n_items.data(), KC, 1, cs.data(), cp.data(), KCW, use_bound ? &bnd : nullptr);
   }
 
@@ -331,7 +394,7 @@ void ivf_flat_search(resources* res, const ivf_flat_index& idx, uint32_t n_probe
   dbuf<float> gs(static_cast<size_t>(nq) * cand_w, s);
   dbuf<uint32_t> gp(static_cast<size_t>(nq) * cand_w, s);
   // empty entries +inf: FLT_MAX made the ivf_flat bench search ~3 % slower (DESIGN.md §4a)
-  gather_probe_candidates(s, cs.data(), cp.data(), pb.slot_of.data(), nullptr, 1.0f, INFINITY, nq, static_cast<int>(n_probes), KCW, gs.data(),
+  gather_probe_candidates(s, cs.data(), cp.data(), pb.slot_of.data(), add.data(), scale, INFINITY, nq, static_cast<int>(n_probes), KCW, gs.data(),
                           gp.data());
   const int kc2 = static_cast<int>(std::min<int64_t>(cand_w, large_k ? large_kc : std::max(32, 2 * k)));
   dbuf<float> ms(static_cast<size_t>(nq) * kc2, s);
@@ -355,8 +418,8 @@ void ivf_flat_search(resources* res, const ivf_flat_index& idx, uint32_t n_probe
   dbuf<int> flags(static_cast<size_t>(nq) + 1, s);
   B2_CUDA(cudaMemsetAsync(flags.data() + nq, 0, sizeof(int), s));
   count_launch();
-  flag_truncated_halves_kernel<<<blocks_for(nq, 256), 256, 0, s>>>(cs.data(), cp.data(), pb.slot_of.data(), ms.data(), nq,
-                                                                   static_cast<int>(n_probes), KC, KCW, kc2, flags.data());
+  flag_truncated_halves_kernel<<<blocks_for(nq, 256), 256, 0, s>>>(cs.data(), cp.data(), pb.slot_of.data(), add.data(), scale, ms.data(),
+                                                                   nq, static_cast<int>(n_probes), KC, KCW, kc2, flags.data());
   B2_CUDA(cudaGetLastError());
   std::vector<int> hflags(static_cast<size_t>(nq) + 1);
   B2_CUDA(cudaMemcpyAsync(hflags.data(), flags.data(), sizeof(int) * (nq + 1), cudaMemcpyDeviceToHost, s));

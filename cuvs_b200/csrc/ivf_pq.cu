@@ -243,8 +243,7 @@ __global__ void pq_init_kernel(float* __restrict__ pq_centers, int64_t n_books, 
 // decoded bf16 rows + half norms from codes (the decoded scan).  one warp per row.
 __global__ void pq_decode_kernel(const uint8_t* __restrict__ codes, const int64_t* __restrict__ ids, int64_t rows, int pq_dim,
                                  int pq_len, int book, int Kp, const float* __restrict__ pq_centers, int per_cluster,
-                                 const int64_t* __restrict__ list_offsets, int64_t n_lists, bool ip,
-                                 const float* __restrict__ centers_rot, int rot_dim, __nv_bfloat16* __restrict__ yhat,
+                                 const int64_t* __restrict__ list_offsets, int64_t n_lists, bool ip, __nv_bfloat16* __restrict__ yhat,
                                  float* __restrict__ hn)
 {
   int64_t r = (blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x) >> 5;
@@ -252,7 +251,7 @@ __global__ void pq_decode_kernel(const uint8_t* __restrict__ codes, const int64_
   if (r >= rows) return;
   const bool pad = ids[r] == kPadId;
   int64_t list   = 0;
-  if (per_cluster || ip) {  // binary search of the owning list
+  if (per_cluster) {  // binary search of the owning list
     int64_t lo = 0, hi = n_lists;
     while (hi - lo > 1) { int64_t mid = (lo + hi) >> 1; if (list_offsets[mid] <= r) lo = mid; else hi = mid; }
     list = lo;
@@ -265,7 +264,6 @@ __global__ void pq_decode_kernel(const uint8_t* __restrict__ codes, const int64_
       int code = codes[r * pq_dim + sub];
       int64_t b = per_cluster ? list : sub;
       v = pq_centers[(b * pq_len + t) * book + code];
-      if (ip) v += centers_rot[list * rot_dim + j];  // inner product scans the full reconstruction
     }
     __nv_bfloat16 hv = __float2bfloat16_rn(v);
     yhat[r * Kp + j] = hv;
@@ -288,40 +286,6 @@ __global__ void make_centers_ext_kernel(const float* __restrict__ centers, int64
 }
 
 // ------------------------------------------------------------------ search-side kernels
-// per pair: r = q_rot[query] - c_rot[list] (L2) or q_rot[query] (IP) as bf16 A rows; add[slot] = |r|^2 (L2) or 0 (IP).
-// Cosine (q_rot already unit) adds the reference's +1 to the offset, so that every reader of `add` sees final distances:
-// 1 - q.c on code-only rows, 1 on decoded rows (c is inside y there).
-__global__ void pair_rows_kernel(const float* __restrict__ q_rot, const float* __restrict__ centers_rot,
-                                 const uint32_t* __restrict__ pair_query, const uint32_t* __restrict__ pair_list,
-                                 const int* __restrict__ n_live, int64_t rows_total, int rot_dim, int Kp, bool ip,
-                                 __nv_bfloat16* __restrict__ a_hi,
-                                 __nv_bfloat16* __restrict__ a_lo, float* __restrict__ add, bool ip_center_in_add, bool cosine)
-{
-  int64_t r = (blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x) >> 5;
-  int lane  = threadIdx.x & 31;
-  if (r >= rows_total) return;
-  float nrm = 0.f;
-  const bool live = r < *n_live;
-  const float* qr = live ? q_rot + static_cast<int64_t>(pair_query[r]) * rot_dim : nullptr;
-  const float* cr = live ? centers_rot + static_cast<int64_t>(pair_list[r]) * rot_dim : nullptr;
-  for (int j = lane; j < Kp; j += 32) {
-    float v = 0.f;
-    if (live && j < rot_dim) v = ip ? qr[j] : qr[j] - cr[j];
-    __nv_bfloat16 h = __float2bfloat16_rn(v);
-    a_hi[r * Kp + j] = h;
-    if (a_lo) a_lo[r * Kp + j] = __float2bfloat16_rn(v - __bfloat162float(h));
-    // L2: |r|^2.  Inner product over code-only rows (the streamed scan decodes y, not c + y): -(q . c) of the pair
-    nrm = (ip && ip_center_in_add) ? ((live && j < rot_dim) ? fmaf(-qr[j], cr[j], nrm) : nrm) : fmaf(v, v, nrm);
-  }
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) nrm += __shfl_xor_sync(0xffffffffu, nrm, o);
-  if (lane == 0 && live) {
-    float a = (ip && !ip_center_in_add) ? 0.f : nrm;
-    if (cosine) a += 1.0f;
-    add[r] = a;
-  }
-}
-
 __global__ void finish_ids_kernel(const uint32_t* __restrict__ pos, const int64_t* __restrict__ ids, float* __restrict__ dist,
                                   int64_t count, int metric, int64_t* __restrict__ out_idx)
 {
@@ -609,8 +573,7 @@ void refresh_decoded(resources* res, ivf_pq_index& idx)
       count_launch();
       pq_decode_kernel<<<blocks_for(R * 32, 256), 256, 0, s>>>(idx.codes.data(), idx.ids.data(), R, idx.pq_dim, idx.pq_len, idx.book(),
                                                                idx.Kp, idx.pq_centers.data(), false, idx.lists.d_offsets.data(), idx.n_lists,
-                                                               is_ip(idx.metric), idx.centers_rot.data(), idx.rot_dim, idx.yhat.data(),
-                                                               hn.data());
+                                                               is_ip(idx.metric), idx.yhat.data(), hn.data());
       B2_CUDA(cudaGetLastError());
       tc_pack_half_norms(s, hn.data(), R, idx.hx.data());
     } else {
@@ -631,8 +594,8 @@ void refresh_decoded(resources* res, ivf_pq_index& idx)
   pq_decode_kernel<<<blocks_for(R * 32, 256), 256, 0, s>>>(idx.codes.data(), idx.ids.data(), R, idx.pq_dim, idx.pq_len, idx.book(),
                                                            idx.Kp, idx.pq_centers.data(),
                                                            idx.codebook_kind == CUVS_IVF_PQ_CODEBOOK_GEN_PER_CLUSTER,
-                                                           idx.lists.d_offsets.data(), idx.n_lists, is_ip(idx.metric),
-                                                           idx.centers_rot.data(), idx.rot_dim, idx.yhat.data(), hn.data());
+                                                           idx.lists.d_offsets.data(), idx.n_lists, is_ip(idx.metric), idx.yhat.data(),
+                                                           hn.data());
   B2_CUDA(cudaGetLastError());
   tc_pack_half_norms(s, hn.data(), R, idx.hx.data());
 }
@@ -831,31 +794,6 @@ scan_plan plan_scan(const ivf_pq_index& idx, const cuvsIvfPqSearchParams& sp, in
   return p;
 }
 
-// Residual rows of the tensor-core scans, one per pair slot (slots of dropped pairs are never read; the 128 rows past the pairs
-// are zero): bf16 planes of q_rot - c_rot (L2) or q_rot (IP), hi and, with two passes, lo; add[slot] is the pair's offset (see
-// pair_rows_kernel).  Returns `scale`: a distance is add[slot] + scale * score (L2: |r|^2 + 2 (|y|^2/2 - r.y); IP: -(q.(c+y));
-// cosine: 1 - q.(c+y)).
-struct residual_rows {
-  int64_t rows = 0;
-  dbuf<__nv_bfloat16> hi, lo;
-};
-float pair_residual_rows(cudaStream_t s, const ivf_pq_index& idx, const float* q_rot, const probe_buckets& pb, const scan_plan& plan,
-                         residual_rows& a, dbuf<float>& add)
-{
-  const bool ip = is_ip(idx.metric);
-  a.rows        = pb.n_pairs + 128;
-  a.hi.alloc(static_cast<size_t>(a.rows) * idx.Kp, s);
-  if (plan.passes == 2) a.lo.alloc(static_cast<size_t>(a.rows) * idx.Kp, s);
-  add.alloc(static_cast<size_t>(pb.n_pairs), s);
-  count_launch();
-  pair_rows_kernel<<<blocks_for(a.rows * 32, 256), 256, 0, s>>>(q_rot, idx.centers_rot.data(), pb.pair_query.data(), pb.pair_list.data(),
-                                                                 pb.n_items.data() + 1, a.rows, idx.rot_dim, idx.Kp, ip, a.hi.data(),
-                                                                 a.lo.data(), add.data(), plan.path == scan_path::stream,
-                                                                 idx.metric == CosineExpanded);
-  B2_CUDA(cudaGetLastError());
-  return ip ? 1.0f : 2.0f;
-}
-
 // The LUT kernel for the search's LUT and distance dtypes, one CTA per pair slot.  The grid covers every slot: the live count
 // is on the device, and the slots past it (dropped pairs, garbage pair_query) exit at once.
 template <bool Store>
@@ -942,7 +880,7 @@ void ivf_pq_search(resources* res, const ivf_pq_index& idx, const cuvsIvfPqSearc
       return;
     }
     residual_rows a;
-    scale = pair_residual_rows(s, idx, q_rot.data(), pb, plan, a, add);
+    scale = pair_residual_rows(s, q_rot.data(), idx.centers_rot.data(), idx.rot_dim, idx.Kp, idx.metric, pb, plan.passes == 2, a, add);
     if (plan.store) item_segments(s, pb, seg_off);
     // probes of one query share a running bound on its k'-th best DISTANCE: d = add[slot] + scale * s
     if (k <= plan.KC) {  // the bound tracks a k-th best out of KC kept entries
