@@ -919,7 +919,7 @@ void kmeans_train(resources* res, const float* x, int64_t n, int d, int k, int n
 {
   auto s = res->stream;
   B2_EXPECTS(n >= 1 && k >= 1, "kmeans: empty input");
-  B2_EXPECTS(tc_supported(res->device, d), "kmeans: dim %d is not supported by the tensor-core assignment kernel yet (<= 128)", d);
+  B2_EXPECTS(tc_supported(res->device, d), "kmeans: dim %d is not supported: it pads to more than %d columns, the widest the tensor-core kernels take", d, kTcMaxK);
   if (init_from_data) {
     count_launch();
     strided_init_kernel<<<blocks_for(static_cast<int64_t>(k) * d, 256), 256, 0, s>>>(x, n, d, k, centers);

@@ -252,7 +252,7 @@ ivf_flat_index* ivf_flat_build(resources* res, const cuvsIvfFlatIndexParams& p, 
   const int d     = static_cast<int>(ds.shape[1]);
   B2_EXPECTS(n >= 1 && d >= 1, "empty dataset");
   B2_EXPECTS(p.n_lists >= 1 && static_cast<int64_t>(p.n_lists) <= n, "n_lists (%u) must be in [1, n_rows]", p.n_lists);
-  B2_EXPECTS(tc_supported(res->device, d), "ivf_flat: dim %d > 128 is not supported by this build yet", d);
+  B2_EXPECTS(tc_supported(res->device, d), "ivf_flat: dim %d is not supported: it pads to more than %d columns, the widest the tensor-core kernels take", d, kTcMaxK);
   auto idx               = std::make_unique<ivf_flat_index>();
   idx->device            = res->device;
   idx->metric            = p.metric;

@@ -21,7 +21,8 @@
 //   lut      pq_lut_scan_kernel — the reference's formulation restated for H100: one CTA per (query, probe),
 //            LUT[pq_dim x 2^bits] in shared memory (fp32 / fp16 / fp_8bit<5>), codes read with 128-bit loads, scores
 //            accumulated in subspace order (bit-identical to oracle/oracle.c for fp32).  It serves the searches the other
-//            two do not (an index with neither, k > 32 without a code stream) and CUVS_B200_PQ_PATH=lut.
+//            two do not (an index with neither, k > 32 without a code stream) and CUVS_B200_PQ_PATH=lut.  A LUT too large for
+//            shared memory goes to a global scratch, one slice per resident CTA (pq_lut_scan_gmem_kernel).
 // Each keeps the k' best per (query, probe) in its epilogue for k <= 64.  For k > 64 the stream and LUT kernels store every
 // score to a dense per-pair segment instead, and a segmented select takes each pair's k best.  Either way the probes of a
 // query are then merged into its k best.
@@ -309,23 +310,22 @@ __global__ void finish_ids_kernel(const uint32_t* __restrict__ pos, const int64_
 constexpr int kLutThreads = 128;
 constexpr int kLutBuf     = 256;  // candidate buffer (entries) per CTA
 
+// The work of one (query, probe) slot: build its LUT at `lut` (shared or global memory), then score the list's rows.
+// `work` is shared memory: the residual and q*c planes, then (select mode) the candidate and compaction buffers.
 // Store mode (k > 64, Store = true): no selection in the kernel.  The CTA writes the score of every row of its list, in list
 // order, to the pair's segment out_score[seg_off[slot] ...] (padding rows +inf); KC, out_pos and KCW are unused.
-template <typename LutT, typename OutT, bool Store = false>
-__global__ void __launch_bounds__(kLutThreads)
-pq_lut_scan_kernel(const float* __restrict__ q_rot, const float* __restrict__ centers_rot, const float* __restrict__ pq_centers,
-                   int per_cluster, const uint8_t* __restrict__ codes, const int64_t* __restrict__ list_offsets,
-                   const uint32_t* __restrict__ list_sizes, const uint32_t* __restrict__ pair_query,
-                   const uint32_t* __restrict__ pair_list, const int* __restrict__ n_live, int rot_dim, int pq_dim, int pq_len, int pq_bits, bool ip, bool cosine,
-                   int KC, float* __restrict__ out_score, uint32_t* __restrict__ out_pos, int KCW,
-                   const int64_t* __restrict__ seg_off)
+template <typename LutT, typename OutT, bool Store>
+__device__ __forceinline__ void
+pq_lut_scan_slot(int64_t slot, LutT* lut, unsigned char* work, const float* __restrict__ q_rot, const float* __restrict__ centers_rot,
+                 const float* __restrict__ pq_centers, int per_cluster, const uint8_t* __restrict__ codes,
+                 const int64_t* __restrict__ list_offsets, const uint32_t* __restrict__ list_sizes,
+                 const uint32_t* __restrict__ pair_query, const uint32_t* __restrict__ pair_list, int rot_dim, int pq_dim, int pq_len,
+                 int pq_bits, bool ip, bool cosine, int KC, float* __restrict__ out_score, uint32_t* __restrict__ out_pos, int KCW,
+                 const int64_t* __restrict__ seg_off)
 {
-  extern __shared__ __align__(16) unsigned char smem_raw[];
   const int book     = 1 << pq_bits;
   const int lut_size = pq_dim * book;
-  LutT* lut          = reinterpret_cast<LutT*>(smem_raw);
-  size_t off         = (static_cast<size_t>(lut_size) * sizeof(LutT) + 15) & ~size_t(15);
-  float* resid       = reinterpret_cast<float*>(smem_raw + off);              // [rot_dim] (L2: q-c ; IP: q)
+  float* resid       = reinterpret_cast<float*>(work);                          // [rot_dim] (L2: q-c ; IP: q)
   float* qc          = resid + rot_dim;                                        // [rot_dim] IP only: q*c
   float* bv          = qc + rot_dim;                                           // [kLutBuf] candidate scores
   uint32_t* bp       = reinterpret_cast<uint32_t*>(bv + kLutBuf);              // [kLutBuf] candidate rows
@@ -334,8 +334,6 @@ pq_lut_scan_kernel(const float* __restrict__ q_rot, const float* __restrict__ ce
   __shared__ int s_cnt;
   __shared__ float s_thr;
 
-  const int64_t slot = blockIdx.x;
-  if (slot >= *n_live) return;  // slots of probes that hit empty lists are never populated
   const uint32_t qi = pair_query[slot], l = pair_list[slot];
   const float* qr = q_rot + static_cast<int64_t>(qi) * rot_dim;
   const float* cr = centers_rot + static_cast<int64_t>(l) * rot_dim;
@@ -440,6 +438,44 @@ pq_lut_scan_kernel(const float* __restrict__ q_rot, const float* __restrict__ ce
     out_pos[slot * KCW + c]   = c < kept ? bp[c] : 0xffffffffu;
   }
 }
+
+#define B2_LUT_SCAN_PARAMS                                                                                                       \
+  const float *__restrict__ q_rot, const float *__restrict__ centers_rot, const float *__restrict__ pq_centers, int per_cluster, \
+    const uint8_t *__restrict__ codes, const int64_t *__restrict__ list_offsets, const uint32_t *__restrict__ list_sizes,       \
+    const uint32_t *__restrict__ pair_query, const uint32_t *__restrict__ pair_list, const int *__restrict__ n_live, int rot_dim, \
+    int pq_dim, int pq_len, int pq_bits, bool ip, bool cosine, int KC, float *__restrict__ out_score,                          \
+    uint32_t *__restrict__ out_pos, int KCW, const int64_t *__restrict__ seg_off
+#define B2_LUT_SCAN_ARGS                                                                                                         \
+  q_rot, centers_rot, pq_centers, per_cluster, codes, list_offsets, list_sizes, pair_query, pair_list, rot_dim, pq_dim, pq_len, \
+    pq_bits, ip, cosine, KC, out_score, out_pos, KCW, seg_off
+
+// LUT in shared memory, one CTA per slot.
+template <typename LutT, typename OutT, bool Store = false>
+__global__ void __launch_bounds__(kLutThreads) pq_lut_scan_kernel(B2_LUT_SCAN_PARAMS)
+{
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  const int lut_size = pq_dim * (1 << pq_bits);
+  const size_t off   = (static_cast<size_t>(lut_size) * sizeof(LutT) + 15) & ~size_t(15);
+  const int64_t slot = blockIdx.x;
+  if (slot >= *n_live) return;  // slots of probes that hit empty lists are never populated
+  pq_lut_scan_slot<LutT, OutT, Store>(slot, reinterpret_cast<LutT*>(smem_raw), smem_raw + off, B2_LUT_SCAN_ARGS);
+}
+
+// LUT in global memory, for LUTs that do not fit in shared memory (the reference's EnableSMemLut = false): the grid is the
+// resident grid, each CTA owns the slice lut_scratch[blockIdx.x * pq_dim * 2^bits ...] and walks the slots blockIdx.x,
+// blockIdx.x + gridDim.x, ...  The slot's work is the same code as above, so the scores are the same bits.
+template <typename LutT, typename OutT, bool Store = false>
+__global__ void __launch_bounds__(kLutThreads) pq_lut_scan_gmem_kernel(B2_LUT_SCAN_PARAMS, LutT* __restrict__ lut_scratch)
+{
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  LutT* lut = lut_scratch + static_cast<int64_t>(blockIdx.x) * (pq_dim << pq_bits);
+  for (int64_t slot = blockIdx.x; slot < *n_live; slot += gridDim.x) {
+    pq_lut_scan_slot<LutT, OutT, Store>(slot, lut, smem_raw, B2_LUT_SCAN_ARGS);
+    __syncthreads();  // the next slot overwrites the LUT and the shared buffers
+  }
+}
+#undef B2_LUT_SCAN_PARAMS
+#undef B2_LUT_SCAN_ARGS
 
 // ------------------------------------------------------------------ host helpers
 uint32_t calculate_pq_dim(uint32_t dim)
@@ -677,7 +713,7 @@ ivf_pq_index* ivf_pq_build(resources* res, const cuvsIvfPqIndexParams& p, const 
   const int d     = static_cast<int>(ds.shape[1]);
   B2_EXPECTS(n >= 1 && d >= 1, "empty dataset");
   B2_EXPECTS(p.n_lists >= 1 && static_cast<int64_t>(p.n_lists) <= n, "n_lists (%u) must be in [1, n_rows]", p.n_lists);
-  B2_EXPECTS(tc_supported(res->device, d), "ivf_pq: dim %d > 128 is not supported by this build yet", d);
+  B2_EXPECTS(tc_supported(res->device, d), "ivf_pq: dim %d is not supported: it pads to more than %d columns, the widest the tensor-core kernels take", d, kTcMaxK);
   auto idx    = std::make_unique<ivf_pq_index>();
   idx->device = res->device;
   init_shape(*idx, p, d);
@@ -794,32 +830,66 @@ scan_plan plan_scan(const ivf_pq_index& idx, const cuvsIvfPqSearchParams& sp, in
   return p;
 }
 
-// The LUT kernel for the search's LUT and distance dtypes, one CTA per pair slot.  The grid covers every slot: the live count
-// is on the device, and the slots past it (dropped pairs, garbage pair_query) exit at once.
+// The LUT kernel for the search's LUT and distance dtypes.  When the LUT fits in shared memory next to the kernel's buffers,
+// one CTA per pair slot: the grid covers every slot, the live count is on the device, and the slots past it (dropped pairs,
+// garbage pair_query) exit at once.  Otherwise the LUT goes to a global scratch with one slice per resident CTA (DESIGN.md §5).
 template <bool Store>
 void launch_lut_scan(cudaStream_t s, const ivf_pq_index& idx, const cuvsIvfPqSearchParams& sp, const float* q_rot, const probe_buckets& pb,
                      int KC, float* out_score, uint32_t* out_pos, int KCW, const int64_t* seg_off)
 {
-  const size_t lut_b = sp.lut_dtype == CUDA_R_32F ? 4 : (sp.lut_dtype == CUDA_R_16F ? 2 : 1);
-  const size_t smem  = ((static_cast<size_t>(idx.pq_dim) * idx.book() * lut_b + 15) & ~size_t(15)) + 2 * idx.rot_dim * sizeof(float) +
-                      (Store ? 0 : 4 * kLutBuf * sizeof(float));  // select mode: candidate and compaction buffers
-  B2_EXPECTS(smem <= 227 * 1024, "ivf_pq: LUT (%zu bytes) does not fit in shared memory; use a smaller lut_dtype", smem);
+  constexpr size_t kMaxSmem = 227 * 1024;
+  const size_t lut_b        = sp.lut_dtype == CUDA_R_32F ? 4 : (sp.lut_dtype == CUDA_R_16F ? 2 : 1);
+  const size_t lut_bytes    = static_cast<size_t>(idx.pq_dim) * idx.book() * lut_b;
+  // residual and q*c planes; select mode adds the candidate and compaction buffers
+  const size_t work = 2 * idx.rot_dim * sizeof(float) + (Store ? 0 : 4 * kLutBuf * sizeof(float));
+  const size_t smem = ((lut_bytes + 15) & ~size_t(15)) + work;
   const bool per_cl = idx.codebook_kind == CUVS_IVF_PQ_CODEBOOK_GEN_PER_CLUSTER;
-  auto run = [&](auto kern) {
-    B2_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
+  const bool ip = is_ip(idx.metric), cosine = idx.metric == CosineExpanded;
+  auto run = [&](auto lut_tag, auto out_tag) {
+    using LutT = decltype(lut_tag);
+    using OutT = decltype(out_tag);
+    if (smem <= kMaxSmem) {
+      auto kern = pq_lut_scan_kernel<LutT, OutT, Store>;
+      B2_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
+      timed_section ts("pq_scan", s);
+      count_launch();
+      kern<<<static_cast<unsigned>(pb.n_pairs), kLutThreads, smem, s>>>(
+        q_rot, idx.centers_rot.data(), idx.pq_centers.data(), per_cl, idx.codes.data(), idx.lists.d_offsets.data(), idx.lists.d_sizes.data(),
+        pb.pair_query.data(), pb.pair_list.data(), pb.n_items.data() + 1, idx.rot_dim, idx.pq_dim, idx.pq_len, idx.pq_bits, ip, cosine,
+        KC, out_score, out_pos, KCW, seg_off);
+      return;
+    }
+    auto kern = pq_lut_scan_gmem_kernel<LutT, OutT, Store>;
+    B2_EXPECTS(work <= kMaxSmem, "ivf_pq: the LUT kernel's buffers (%zu bytes at rot_dim %d) do not fit in shared memory", work, idx.rot_dim);
+    B2_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(work)));
+    int per_sm = 0;
+    B2_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, kLutThreads, work));
+    const int64_t grid = std::min<int64_t>(pb.n_pairs, static_cast<int64_t>(std::max(per_sm, 1)) * sm_count_of(idx.device));
+    if (grid == 0) return;
+    dbuf<LutT> scratch;
+    const size_t scratch_b  = static_cast<size_t>(grid) * lut_bytes;
+    const cudaError_t alloc = cudaMallocAsync(reinterpret_cast<void**>(&scratch.p), scratch_b, s);
+    if (alloc == cudaErrorMemoryAllocation) {
+      (void)cudaGetLastError();
+      B2_FAIL("ivf_pq: the LUT (%zu bytes) does not fit in shared memory, and device memory has no room for its global scratch "
+              "(%lld resident CTAs, %zu bytes)", lut_bytes, (long long)grid, scratch_b);
+    }
+    B2_CUDA(alloc);
+    scratch.n = static_cast<size_t>(grid) * idx.pq_dim * idx.book();
+    scratch.s = s;
     timed_section ts("pq_scan", s);
     count_launch();
-    kern<<<static_cast<unsigned>(pb.n_pairs), kLutThreads, smem, s>>>(
+    kern<<<static_cast<unsigned>(grid), kLutThreads, work, s>>>(
       q_rot, idx.centers_rot.data(), idx.pq_centers.data(), per_cl, idx.codes.data(), idx.lists.d_offsets.data(), idx.lists.d_sizes.data(),
-      pb.pair_query.data(), pb.pair_list.data(), pb.n_items.data() + 1, idx.rot_dim, idx.pq_dim, idx.pq_len, idx.pq_bits,
-      is_ip(idx.metric), idx.metric == CosineExpanded, KC, out_score, out_pos, KCW, seg_off);
+      pb.pair_query.data(), pb.pair_list.data(), pb.n_items.data() + 1, idx.rot_dim, idx.pq_dim, idx.pq_len, idx.pq_bits, ip, cosine,
+      KC, out_score, out_pos, KCW, seg_off, scratch.data());
   };
   const bool half_out = sp.internal_distance_dtype == CUDA_R_16F;
-  if (sp.lut_dtype == CUDA_R_32F) run(pq_lut_scan_kernel<float, float, Store>);
-  else if (sp.lut_dtype == CUDA_R_16F && !half_out) run(pq_lut_scan_kernel<__half, float, Store>);
-  else if (sp.lut_dtype == CUDA_R_16F && half_out) run(pq_lut_scan_kernel<__half, __half, Store>);
-  else if (!half_out) run(pq_lut_scan_kernel<uint8_t, float, Store>);
-  else run(pq_lut_scan_kernel<uint8_t, __half, Store>);
+  if (sp.lut_dtype == CUDA_R_32F) run(float{}, float{});
+  else if (sp.lut_dtype == CUDA_R_16F && !half_out) run(__half{}, float{});
+  else if (sp.lut_dtype == CUDA_R_16F && half_out) run(__half{}, __half{});
+  else if (!half_out) run(uint8_t{}, float{});
+  else run(uint8_t{}, __half{});
   B2_CUDA(cudaGetLastError());
 }
 
@@ -1151,7 +1221,7 @@ cuvsError_t cuvsIvfPqBuildPrecomputed(cuvsResources_t res, cuvsIvfPqIndexParams_
     const DLTensor& pc = pq_centers->dl_tensor;
     const DLTensor& ce = centers->dl_tensor;
     B2_EXPECTS(dl_is(pc, kDLFloat, 32) && dl_is(ce, kDLFloat, 32), "codebooks must be float32");
-    B2_EXPECTS(tc_supported(r->device, idx->dim), "ivf_pq: dim %d > 128 is not supported by this build yet", idx->dim);
+    B2_EXPECTS(tc_supported(r->device, idx->dim), "ivf_pq: dim %d is not supported: it pads to more than %d columns, the widest the tensor-core kernels take", idx->dim, kTcMaxK);
     const int64_t nb = idx->codebook_kind == CUVS_IVF_PQ_CODEBOOK_GEN_PER_CLUSTER ? idx->n_lists : idx->pq_dim;
     B2_EXPECTS(pc.ndim == 3 && pc.shape[0] == nb && pc.shape[1] == idx->pq_len && pc.shape[2] == idx->book(),
                "pq_centers must have extent [%lld, %d, %d]", (long long)nb, idx->pq_len, idx->book());

@@ -140,7 +140,7 @@ void predict(resources* r, const float* x, int64_t n, int d, const float* centro
              double* inertia)
 {
   auto s = r->stream;
-  B2_EXPECTS(tc_supported(r->device, d), "kmeans: dim %d > 128 is not supported by this build yet", d);
+  B2_EXPECTS(tc_supported(r->device, d), "kmeans: dim %d is not supported: it pads to more than %d columns, the widest the tensor-core kernels take", d, kTcMaxK);
   tc_rows_tmp xp;
   xp.build(s, x, n, d, true);
   dbuf<float> cn(static_cast<size_t>(k), s), xn(static_cast<size_t>(n), s), scores(static_cast<size_t>(n), s);
