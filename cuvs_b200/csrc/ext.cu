@@ -15,13 +15,58 @@ namespace {
 std::atomic<int> g_timing{0};
 std::atomic<long long> g_launches{0};
 thread_local int g_last_flagged = 0;
+// set_last_flagged_async: one pinned int and event per thread (for the device it was last used on), released when the thread
+// exits or moves to another device, after the copy into the int has landed.  Errors are ignored there: at process exit the
+// runtime may already be gone, and nothing is left to report to.
+struct pending_count {
+  int device        = -1;
+  int* host         = nullptr;
+  cudaEvent_t done  = nullptr;
+  bool pending      = false;
+  void release()
+  {
+    if (host == nullptr) return;
+    cudaEventSynchronize(done);
+    cudaEventDestroy(done);
+    cudaFreeHost(host);
+    host    = nullptr;
+    done    = nullptr;
+    device  = -1;
+    pending = false;
+  }
+  ~pending_count() { release(); }
+};
+thread_local pending_count g_pending;
 std::mutex g_mu;
 std::map<std::string, std::vector<std::pair<cudaEvent_t, cudaEvent_t>>> g_events;
 }  // namespace
 
 bool timing_enabled() { return g_timing.load(std::memory_order_relaxed) != 0; }
 void count_launch(int n) { g_launches.fetch_add(n, std::memory_order_relaxed); }
-void set_last_flagged(int n) { g_last_flagged = n; }
+void set_last_flagged(int n)
+{
+  g_last_flagged    = n;
+  g_pending.pending = false;
+}
+void set_last_flagged_async(const int* dev_count, cudaStream_t stream)
+{
+  int dev = 0;
+  B2_CUDA(cudaGetDevice(&dev));
+  auto& p = g_pending;
+  if (p.device != dev) {
+    if (p.pending) {  // the count of the search on the old device stays readable
+      B2_CUDA(cudaEventSynchronize(p.done));
+      g_last_flagged = *p.host;
+    }
+    p.release();
+    B2_CUDA(cudaMallocHost(&p.host, sizeof(int)));
+    B2_CUDA(cudaEventCreateWithFlags(&p.done, cudaEventDisableTiming));
+    p.device = dev;
+  }
+  B2_CUDA(cudaMemcpyAsync(p.host, dev_count, sizeof(int), cudaMemcpyDeviceToHost, stream));
+  B2_CUDA(cudaEventRecord(p.done, stream));
+  p.pending = true;
+}
 
 void timing_begin(const char*, cudaStream_t stream, cudaEvent_t* ev_start)
 {
@@ -67,6 +112,13 @@ double cuvsB200TimingTotalMs(const char* name, int* count)
   if (count) *count = n;
   return total;
 }
-int cuvsB200LastFlagged(void) { return g_last_flagged; }
+int cuvsB200LastFlagged(void)
+{
+  if (g_pending.pending && cudaEventSynchronize(g_pending.done) == cudaSuccess) {
+    g_last_flagged    = *g_pending.host;
+    g_pending.pending = false;
+  }
+  return g_last_flagged;
+}
 long long cuvsB200KernelLaunches(void) { return g_launches.load(); }
 }

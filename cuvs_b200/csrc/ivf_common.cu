@@ -272,7 +272,8 @@ __global__ void pair_rows_kernel(const float* __restrict__ q, const float* __res
 // out[q, p*KCW + c] = add[slot] + scale * s   (per-query concatenation of its probes' candidates; `empty` where there is none)
 __global__ void gather_cands_kernel(const float* __restrict__ cs, const uint32_t* __restrict__ cp,
                                     const uint32_t* __restrict__ slot_of, const float* __restrict__ add, float scale, float empty,
-                                    int64_t total, int KCW, float* __restrict__ out_score, uint32_t* __restrict__ out_pos)
+                                    int64_t total, int KCW, float* __restrict__ out_score, uint32_t* __restrict__ out_pos,
+                                    int L, float* __restrict__ last)
 {
   int64_t t = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x;
   if (t >= total) return;
@@ -291,6 +292,7 @@ __global__ void gather_cands_kernel(const float* __restrict__ cs, const uint32_t
   }
   out_score[t] = s;
   out_pos[t]   = p;
+  if (last != nullptr && c % L == L - 1) last[t / L] = s;
 }
 
 // ---- k > 64: dense per-pair score segments.  Live slot i, a pair of list l, owns scores[seg_off[i] .. + padded size of l):
@@ -779,12 +781,14 @@ float pair_residual_rows(cudaStream_t s, const float* q, const float* centers, i
 }
 
 void gather_probe_candidates(cudaStream_t s, const float* cs, const uint32_t* cp, const uint32_t* slot_of, const float* add,
-                             float scale, float empty, int64_t nq, int n_probes, int KCW, float* out_score, uint32_t* out_pos)
+                             float scale, float empty, int64_t nq, int n_probes, int KCW, float* out_score, uint32_t* out_pos,
+                             int L, float* last)
 {
   const int64_t total = nq * n_probes * KCW;
   if (total == 0) return;
   count_launch();
-  gather_cands_kernel<<<blocks_for(total, 256), 256, 0, s>>>(cs, cp, slot_of, add, scale, empty, total, KCW, out_score, out_pos);
+  gather_cands_kernel<<<blocks_for(total, 256), 256, 0, s>>>(cs, cp, slot_of, add, scale, empty, total, KCW, out_score, out_pos, L,
+                                                             last);
   B2_CUDA(cudaGetLastError());
 }
 

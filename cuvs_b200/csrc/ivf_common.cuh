@@ -90,9 +90,12 @@ float pair_residual_rows(cudaStream_t s, const float* q, const float* centers, i
 /**
  * Per query, concatenate the KCW candidates of each of its probes: out [nq, n_probes * KCW], value add[slot] + scale * score
  * (add null: 0).  Empty entries, of a dropped pair or with position 0xffffffff, become (`empty`, 0xffffffff).
+ * With `last`, the KCW entries of a pair are read as lists of L and the last value of every list is also written to
+ * last[q, p * (KCW / L) + j] (list j of probe p): what IVF-Flat's certificate reads of them.
  */
 void gather_probe_candidates(cudaStream_t s, const float* cs, const uint32_t* cp, const uint32_t* slot_of, const float* add,
-                             float scale, float empty, int64_t nq, int n_probes, int KCW, float* out_score, uint32_t* out_pos);
+                             float scale, float empty, int64_t nq, int n_probes, int KCW, float* out_score, uint32_t* out_pos,
+                             int L = 0, float* last = nullptr);
 
 /**
  * Per query: the k best (value, position) among its probes' candidates, value = add[slot] + scale * score, sorted

@@ -14,10 +14,12 @@
 //              fused top-k' epilogue — each list tile is read once per 128 probing queries, not once per query.
 //              k > 64: the same scan with the store epilogue writes every (pair, list row) score to the pair's dense
 //              segment, and a segmented select keeps each pair's kc2 = min(2k, 2048) best (the reference's non-fused
-//              formulation, ivf_flat_search.cuh:238-295).  32 < k <= 64: a certificate sends the queries whose column-half
-//              lists of 32 may have dropped a candidate through that path as well (step 5)
+//              formulation, ivf_flat_search.cuh:238-295)
 //   4. per query: gather the candidates of its probes, keep the best few by approximate score, re-score
 //      them exactly in fp32 (sum (q-x)^2 / q.x — the reference's fine-scan arithmetic) and emit ids.
+//   5. certificate: a query whose k-th exact distance is not safely below every row the candidates left out (the bf16 score's
+//      error budget) is searched again with every row of its probed lists scored exactly, so every query returns the
+//      oracle's answer over its probed lists.
 #include "common.hpp"
 #include "exact.cuh"
 #include "ivf_common.cuh"
@@ -58,6 +60,8 @@ struct ivf_flat_index {
   owned<__nv_bfloat16> hi;   // [rows_total, Kp] bf16 residuals x - c of each row's list centre (cosine: x/|x| - c/|c|)
   owned<__nv_bfloat16> hx;   // [rows_total, 16] half-norm plane: |x - c|^2/2 (0 for inner product), +inf on padding rows (scan_tc.cuh)
   // (cosine is scanned as L2 over the unit vectors, 2 - 2 q.x = |q - x|^2: the error then follows |q - c|, not |q| = 1)
+  owned<float> rn_max;       // [n_lists] max |x - c|^2 over the list's rows (the certificate's error budget)
+  owned<float> cn;           // [n_lists] |c|^2 of the fp32 centres (the inner-product budget)
   int Kp = 0;
 };
 
@@ -129,29 +133,247 @@ __global__ void drop_nonfinite_kernel(const float* __restrict__ score, uint32_t*
   if (i < n && !isfinite(score[i])) pos[i] = 0xffffffffu;
 }
 
-// 32 < k <= 64 certificate: each pair kept only the KC best rows of each column half of its list.  A half that came back full
-// may have dropped rows, all scoring no better than its last kept entry; when that entry is strictly better than the query's
-// kc2-th merged candidate, a dropped row could have made the cut, and the query is flagged (flags[nq] counts them).  Entries are
-// compared in the merged candidates' units, add[slot] + scale * score.
-__global__ void flag_truncated_halves_kernel(const float* __restrict__ cs, const uint32_t* __restrict__ cp,
-                                             const uint32_t* __restrict__ slot_of, const float* __restrict__ add, float scale,
-                                             const float* __restrict__ ms, int64_t nq, int n_probes, int KC, int KCW, int kc2,
-                                             int* __restrict__ flags)
+// rn_max[l] = max of rn over the rows of list l (padding rows hold 0); one warp per list
+__global__ void list_max_kernel(const float* __restrict__ rn, const int64_t* __restrict__ offsets, int64_t n_lists, float* __restrict__ out)
 {
-  int64_t q = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x;
+  const int64_t l = (blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x) >> 5;
+  const int lane  = threadIdx.x & 31;
+  if (l >= n_lists) return;
+  float m = 0.f;
+  for (int64_t r = offsets[l] + lane; r < offsets[l + 1]; r += 32) m = fmaxf(m, rn[r]);
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
+  if (lane == 0) out[l] = m;
+}
+
+// Error budget of the fine scan's approximate distance A = add + scale * score of a row x of a pair (q, list l) against the
+// exact fp32 distance F the re-score computes, in A's units (DESIGN.md §4, "Certificate").  Q = |q - c| (inner product: |q|),
+// R = max |x - c| over the list (rn_max), C = |c|:
+//   bf16 rounding of both residual rows        scale (2^-8 + 2^-16) Q R
+//   fp32 tensor-core accumulation over Kp + 16  scale (Kp + 20) 2^-22 (1.01 Q R + hn), hn = R^2 / 2 (L2, cosine) or 0
+//   fp32 rounding of add, rn, the sum and F     (2 dim + 16) 2^-23 (Q + R)^2, inner product (2 dim + 16) 2^-23 Q (2 C + R)
+//   cosine: unit rows and queries vs the exact  (2 dim + 16) 2^-21
+//     1 - q.x / (|q| |x|), taken twice
+// Each term bounds its rounding step as documented; how the MMA orders and rounds its fp32 sums inside one instruction is not,
+// so the budget is checked against the errors the scan makes (tests/test_ivf_flat_near_duplicates_gpu.py::budget_ratio,
+// DESIGN.md §4): they stay below 0.4 of it, and below 0.25 except where a row nearly repeats the query.
+struct flat_budget {
+  float c_bf, c_acc, c_fp, c_abs;
+  bool ip;
+  __device__ float eps(float Q, float R, float C) const
+  {
+    if (ip) return (c_bf + 1.01f * c_acc) * Q * R + c_fp * Q * (2.f * C + R);
+    return c_bf * Q * R + c_acc * (1.01f * Q * R + 0.5f * R * R) + c_fp * (Q + R) * (Q + R) + c_abs;
+  }
+};
+
+flat_budget make_budget(const ivf_flat_index& idx, float scale)
+{
+  flat_budget b;
+  b.ip    = idx.metric == InnerProduct;
+  b.c_bf  = scale * (1.f / 256.f + 1.f / 65536.f);
+  b.c_acc = scale * static_cast<float>(idx.Kp + 20) * (1.f / 4194304.f);
+  b.c_fp  = static_cast<float>(2 * idx.dim + 16) * (1.f / 8388608.f);
+  b.c_abs = idx.metric == CosineExpanded ? 4.f * b.c_fp : 0.f;
+  return b;
+}
+
+// The certificate (DESIGN.md §4).  Every row of the query's probed lists that is not among its kc2 merged candidates has A at
+// least `floor`, the minimum of
+//   * the kc2-th merged candidate (ms, sorted), for the rows the merge dropped;
+//   * the last entry of every full per-pair list (a column half of KC, or a pair's segment of kc2 at k > 64), for the rows a
+//     list dropped: last[q, p * nl + j] for list j of probe p (gather_probe_candidates), +inf where a list is not full;
+// and the rows the shared pruning bound rejected score above some full list's L-th entry, hence above `floor` too.  Such a row
+// has F >= floor - eps, so when the exact k-th distance (kth, in A's units) is strictly below floor - eps no row outside can
+// enter the top k, and the re-score of the candidates is the oracle's answer.  eps is the largest budget of the query's pairs,
+// except pairs whose every row is provably farther than kth (triangle inequality: |q - x| >= Q - R, or -q.x >= add - Q R).
+// Otherwise the query is flagged (flags[nq] counts them).  One warp per query, its lanes over the probes.
+__global__ void certify_kernel(const float* __restrict__ out_dist, int k, int fine, const float* __restrict__ ms, int kc2,
+                               const float* __restrict__ last, int nl, const uint32_t* __restrict__ probes,
+                               const uint32_t* __restrict__ slot_of, int n_probes, const float* __restrict__ add,
+                               const float* __restrict__ qn, const float* __restrict__ rn_max, const float* __restrict__ cn,
+                               flat_budget bud, int64_t nq, int* __restrict__ flags)
+{
+  const int64_t q = (blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x) >> 5;
+  const int lane  = threadIdx.x & 31;
   if (q >= nq) return;
-  const float cut = ms[q * kc2 + kc2 - 1];
-  int flag        = 0;
-  for (int p = 0; p < n_probes && !flag; ++p) {
+  const float kd = out_dist[q * k + k - 1];
+  // the exact k-th distance in A's units; a missing k-th neighbour (+-FLT_MAX) is FLT_MAX
+  const float kth = fine == InnerProduct ? -kd : (fine == CosineExpanded && kd < FLT_MAX ? 2.f * kd : kd);
+  float floor     = lane == 0 ? ms[q * kc2 + kc2 - 1] : INFINITY;
+  float eps       = 0.f;
+  const float qi  = bud.ip ? sqrtf(qn[q]) : 0.f;
+  for (int p = lane; p < n_probes; p += 32) {
     const uint32_t slot = slot_of[q * n_probes + p];
     if (slot == 0xffffffffu) continue;
-    for (int h = KC - 1; h < KCW; h += KC) {
-      const int64_t e = static_cast<int64_t>(slot) * KCW + h;
-      if (cp[e] != 0xffffffffu && add[slot] + scale * cs[e] < cut) flag = 1;
+    const float* g = last + (q * n_probes + p) * nl;
+    for (int j = 0; j < nl; ++j) floor = fminf(floor, g[j]);
+    const float a    = add[slot];
+    const uint32_t l = probes[q * n_probes + p];
+    const float R    = sqrtf(rn_max[l]);
+    const float Q    = bud.ip ? qi : sqrtf(fmaxf(a, 0.f));
+    const float e_p  = bud.eps(Q, R, bud.ip ? sqrtf(cn[l]) : 0.f);
+    const float lower = bud.ip ? a - Q * R - e_p : (Q > R ? (Q - R) * (Q - R) - e_p : -INFINITY);
+    if (lower > kth) continue;
+    eps = fmaxf(eps, e_p);
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    floor = fminf(floor, __shfl_xor_sync(0xffffffffu, floor, o));
+    eps   = fmaxf(eps, __shfl_xor_sync(0xffffffffu, eps, o));
+  }
+  if (lane != 0) return;
+  const int flag = kth < floor - eps ? 0 : 1;
+  flags[q]       = flag;
+  if (flag) atomicAdd(flags + nq, 1);
+}
+
+// The exact distance of row r to the query row qr with rescore_topk's arithmetic (exact.cu: fmaf over ascending components,
+// the `fine` metric), negated for inner product so that smaller is better.
+__device__ __forceinline__ float exact_key(const float* __restrict__ qr, const float* __restrict__ xr, int dim, float qn, float xn, int fine)
+{
+  float acc = 0.f;
+  if (fine == L2Unexpanded) {
+    for (int j = 0; j < dim; ++j) { const float t = qr[j] - xr[j]; acc = fmaf(t, t, acc); }
+  } else {
+    for (int j = 0; j < dim; ++j) acc = fmaf(qr[j], xr[j], acc);
+  }
+  return fine == InnerProduct ? -acc : (fine == CosineExpanded ? 1.0f - acc / (sqrtf(qn) * sqrtf(xn)) : acc);
+}
+
+__device__ __forceinline__ bool row_kept(int64_t id, const uint32_t* __restrict__ keep_bits, int64_t n_bits)
+{
+  return id != kPadId && (keep_bits == nullptr || (id >= 0 && id < n_bits && ((keep_bits[id >> 5] >> (id & 31)) & 1u)));
+}
+
+// k <= 64: the exact fallback on the device, the CTAs taking the queries in turn; they pass over a query the certificate
+// accepted, so the search needs no host round trip.  A flagged query scores every row of its probed lists with exact_key.  Rows better than the running
+// k-th best (distance, id) collect in shared memory, which is sorted and cut back to k whenever it may overflow; the k best by
+// (distance, id), rescore_topk's ranking, overwrite the query's output row (selection form; missing: pad id and +-FLT_MAX).
+constexpr int kFbThreads = 256, kFbCap = 1024;
+__global__ void __launch_bounds__(kFbThreads)
+exact_fallback_kernel(const int* __restrict__ flags, const uint32_t* __restrict__ probes, int n_probes, const int64_t* __restrict__ offsets,
+                      const float* __restrict__ q, int dim, const float* __restrict__ x, const float* __restrict__ qn,
+                      const float* __restrict__ xn, const int64_t* __restrict__ ids, int fine, const uint32_t* __restrict__ keep_bits,
+                      int64_t n_bits, int k, int64_t nq, int64_t* __restrict__ out_idx, float* __restrict__ out_dist)
+{
+  __shared__ float sd[kFbCap];
+  __shared__ int64_t si[kFbCap];
+  __shared__ int cnt;
+  __shared__ float thr_d;
+  __shared__ int64_t thr_i;
+  const bool ip = fine == InnerProduct;
+  auto compact = [&]() {  // sort the cnt entries by (distance, id), keep the k best and their k-th as the threshold
+    const int n = cnt;
+    for (int i = n + threadIdx.x; i < kFbCap; i += kFbThreads) { sd[i] = INFINITY; si[i] = INT64_MAX; }
+    __syncthreads();
+    for (int size = 2; size <= kFbCap; size <<= 1) {
+      for (int stride = size >> 1; stride > 0; stride >>= 1) {
+        for (int i = threadIdx.x; i < kFbCap / 2; i += kFbThreads) {
+          const int lo = (i / stride) * stride * 2 + (i % stride), hi = lo + stride;
+          const bool up = (lo & size) == 0;
+          const bool hi_first = sd[hi] < sd[lo] || (sd[hi] == sd[lo] && si[hi] < si[lo]);
+          if (hi_first == up) {
+            const float td = sd[lo]; sd[lo] = sd[hi]; sd[hi] = td;
+            const int64_t ti = si[lo]; si[lo] = si[hi]; si[hi] = ti;
+          }
+        }
+        __syncthreads();
+      }
+    }
+    if (threadIdx.x == 0) {
+      cnt = min(n, k);
+      if (n >= k) { thr_d = sd[k - 1]; thr_i = si[k - 1]; }
+    }
+    __syncthreads();
+  };
+  for (int64_t qi = blockIdx.x; qi < nq; qi += gridDim.x) {
+    if (!flags[qi]) continue;
+    __syncthreads();  // the previous query's rows are written
+    if (threadIdx.x == 0) { cnt = 0; thr_d = INFINITY; thr_i = INT64_MAX; }
+    __syncthreads();
+    const float* qr = q + qi * dim;
+    for (int p = 0; p < n_probes; ++p) {
+      const uint32_t l = probes[qi * n_probes + p];
+      if (l == 0xffffffffu) continue;
+      const int64_t r1 = offsets[l + 1];
+      for (int64_t base = offsets[l]; base < r1; base += kFbThreads) {
+        const int64_t r = base + threadIdx.x;
+        if (r < r1) {
+          const int64_t id = ids[r];
+          if (row_kept(id, keep_bits, n_bits)) {
+            const float d = exact_key(qr, x + r * dim, dim, qn[qi], xn[r], fine);
+            if (d < thr_d || (d == thr_d && id < thr_i)) {
+              const int at = atomicAdd(&cnt, 1);
+              sd[at] = d;
+              si[at] = id;
+            }
+          }
+        }
+        __syncthreads();
+        const bool full = cnt > kFbCap - kFbThreads;  // every thread reads it before any adds to it again
+        __syncthreads();
+        if (full) compact();
+      }
+    }
+    compact();
+    for (int j = threadIdx.x; j < k; j += kFbThreads) {
+      const bool have     = j < cnt;
+      out_idx[qi * k + j]  = have ? si[j] : INT64_MAX;
+      out_dist[qi * k + j] = have ? (ip ? -sd[j] : sd[j]) : (ip ? -FLT_MAX : FLT_MAX);
     }
   }
-  flags[q] = flag;
-  if (flag) atomicAdd(flags + nq, 1);
+}
+
+// k > 64: the exact fallback's scan.  The score of every (pair, list row) is the row's exact_key, so the segmented select keeps
+// each pair's k best by the very value the re-score recomputes.  Padding rows and rows the bitset hides
+// score +inf.  One CTA per live pair slot, one thread per row.
+__global__ void exact_segments_kernel(const float* __restrict__ q, int dim, const float* __restrict__ x, const float* __restrict__ qn,
+                                      const float* __restrict__ xn, const int64_t* __restrict__ ids, int fine,
+                                      const uint32_t* __restrict__ pair_query, const uint32_t* __restrict__ pair_list,
+                                      const int* __restrict__ n_live, const int64_t* __restrict__ offsets,
+                                      const int64_t* __restrict__ seg_off, const uint32_t* __restrict__ keep_bits, int64_t n_bits,
+                                      float* __restrict__ scores)
+{
+  const int64_t slot = blockIdx.x;
+  if (slot >= *n_live) return;
+  const int64_t qi = pair_query[slot];
+  const uint32_t l = pair_list[slot];
+  const float* qr  = q + qi * dim;
+  float* out       = scores + seg_off[slot];
+  for (int64_t r = offsets[l] + threadIdx.x; r < offsets[l + 1]; r += blockDim.x)
+    out[r - offsets[l]] = row_kept(ids[r], keep_bits, n_bits) ? exact_key(qr, x + r * dim, dim, qn[qi], xn[r], fine) : INFINITY;
+}
+
+// cuvsB200IvfFlatCandidates: per merged candidate (q, c) at index row pos, its source id (INT64_MAX for an empty slot) and the
+// budget of its own pair, the probe of q whose list holds the row (flat_budget::eps, as certify_kernel takes it).
+__global__ void candidate_budget_kernel(const uint32_t* __restrict__ pos, const int64_t* __restrict__ src_ids,
+                                        const int64_t* __restrict__ offsets, int64_t n_lists, const uint32_t* __restrict__ probes,
+                                        const uint32_t* __restrict__ slot_of, int n_probes, int kc2, const float* __restrict__ add,
+                                        const float* __restrict__ qn, const float* __restrict__ rn_max, const float* __restrict__ cn,
+                                        flat_budget bud, int64_t n, int64_t* __restrict__ ids, float* __restrict__ bound)
+{
+  const int64_t i = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x;
+  if (i >= n) return;
+  const uint32_t r = pos[i];
+  ids[i]           = r == 0xffffffffu ? INT64_MAX : src_ids[r];
+  float eps        = INFINITY;
+  if (r != 0xffffffffu) {
+    int64_t lo = 0, up = n_lists;  // the list holding row r: the last with offsets[l] <= r
+    while (up - lo > 1) {
+      const int64_t mid = (lo + up) >> 1;
+      if (offsets[mid] <= r) lo = mid;
+      else up = mid;
+    }
+    const int64_t q = i / kc2;
+    for (int p = 0; p < n_probes; ++p) {
+      const uint32_t slot = slot_of[q * n_probes + p];
+      if (slot == 0xffffffffu || probes[q * n_probes + p] != static_cast<uint32_t>(lo)) continue;
+      const float Q = bud.ip ? sqrtf(qn[q]) : sqrtf(fmaxf(add[slot], 0.f));
+      eps           = bud.eps(Q, sqrtf(rn_max[lo]), bud.ip ? sqrtf(cn[lo]) : 0.f);
+    }
+  }
+  bound[i] = eps;
 }
 
 // dst[dst_row(i)] = src[src_row(i)] for rows of `width` elements; a null row map is the identity
@@ -185,6 +407,8 @@ void refresh_tc_side(resources* res, ivf_flat_index& idx)
   idx.hx.alloc(static_cast<size_t>(std::max<int64_t>(R, 128)) * 16);
   idx.xn.alloc(static_cast<size_t>(std::max<int64_t>(R, 128)));
   idx.rn.alloc(static_cast<size_t>(std::max<int64_t>(R, 128)));
+  idx.rn_max.alloc(static_cast<size_t>(idx.n_lists));
+  B2_CUDA(cudaMemsetAsync(idx.rn_max.data(), 0, sizeof(float) * idx.n_lists, s));
   if (R == 0) return;
   row_norms(s, idx.data.data(), R, idx.dim, idx.dim, idx.xn.data());
   dbuf<float> scale;
@@ -198,6 +422,8 @@ void refresh_tc_side(resources* res, ivf_flat_index& idx)
                                                                 idx.hi.data(), idx.rn.data());
   dbuf<float> hn(static_cast<size_t>(R), s);
   half_norms_masked_kernel<<<blocks_for(R, 256), 256, 0, s>>>(idx.rn.data(), idx.ids.data(), R, !is_l2(scan_metric(idx)), hn.data());
+  count_launch();
+  list_max_kernel<<<blocks_for(idx.n_lists * 32, 256), 256, 0, s>>>(idx.rn.data(), idx.lists.d_offsets.data(), idx.n_lists, idx.rn_max.data());
   B2_CUDA(cudaGetLastError());
   tc_pack_half_norms(s, hn.data(), R, idx.hx.data());
 }
@@ -205,17 +431,18 @@ void refresh_tc_side(resources* res, ivf_flat_index& idx)
 void refresh_centers_tc(resources* res, ivf_flat_index& idx)
 {
   auto s = res->stream;
-  dbuf<float> cn(static_cast<size_t>(idx.n_lists), s);
-  row_norms(s, idx.centers.data(), idx.n_lists, idx.dim, idx.dim, cn.data());
+  idx.cn.alloc(static_cast<size_t>(idx.n_lists));
+  float* cn = idx.cn.data();
+  row_norms(s, idx.centers.data(), idx.n_lists, idx.dim, idx.dim, cn);
   dbuf<float> scale;
   if (idx.metric == CosineExpanded) {
     scale.alloc(static_cast<size_t>(idx.n_lists), s);
-    rsqrt_rows(s, cn.data(), idx.n_lists, scale.data());
+    rsqrt_rows(s, cn, idx.n_lists, scale.data());
     idx.centers_unit.alloc(static_cast<size_t>(idx.n_lists) * idx.dim);
     B2_CUDA(cudaMemcpyAsync(idx.centers_unit.data(), idx.centers.data(), sizeof(float) * idx.n_lists * idx.dim, cudaMemcpyDeviceToDevice, s));
     normalize_rows(s, idx.centers_unit.data(), idx.n_lists, idx.dim, idx.dim);
   }
-  idx.centers_tc.build(s, idx.centers.data(), idx.n_lists, idx.dim, is_l2(idx.metric) ? cn.data() : nullptr, true, scale.data());
+  idx.centers_tc.build(s, idx.centers.data(), idx.n_lists, idx.dim, is_l2(idx.metric) ? cn : nullptr, true, scale.data());
 }
 
 // Insert the rows of `t` (fp32 [n, dim], device or host) with ids new_ids[i] (device) or id0 + i, then refresh the derived
@@ -277,9 +504,18 @@ ivf_flat_index* ivf_flat_build(resources* res, const cuvsIvfFlatIndexParams& p, 
   return idx.release();
 }
 
-// store: take the k > 64 path at any k (the queries the 32 < k <= 64 certificate flags)
+// The merged candidates of a search and their error budget, as the certificate sees them (cuvsB200IvfFlatCandidates).
+struct flat_candidates {
+  int64_t* ids;  // [nq, kc2]
+  float* dist;   // [nq, kc2] approximate distance, add + scale * score
+  float* bound;  // [nq, kc2] error budget of each candidate's own pair
+};
+
+// exact: score every row of the probed lists exactly (the fallback of the queries the certificate flags).  dump: stop after
+// the certificate and copy its inputs out (one query batch).
 void ivf_flat_search(resources* res, const ivf_flat_index& idx, uint32_t n_probes, const DLTensor& qt, const DLTensor& nt,
-                     const DLTensor& dt, const uint32_t* keep_bits = nullptr, int64_t n_bits = 0, bool store = false)
+                     const DLTensor& dt, const uint32_t* keep_bits = nullptr, int64_t n_bits = 0, bool exact = false,
+                     const flat_candidates* dump = nullptr)
 {
   auto s           = res->stream;
   const int64_t nq = qt.shape[0];
@@ -290,9 +526,10 @@ void ivf_flat_search(resources* res, const ivf_flat_index& idx, uint32_t n_probe
   B2_EXPECTS(n_probes >= 1, "n_probes must be >= 1");
   if (nq == 0) return;
   n_probes         = std::min<uint32_t>(n_probes, idx.n_lists);
-  // k > 64 (DESIGN.md §4 "k > 64"): the scan stores every (pair, list row) score and a segmented select keeps kc2 per pair
-  const bool large_k = k > 64 || store;
-  const int large_kc = std::min(2 * k, kSelectMaxK);
+  // k > 64 (DESIGN.md §4 "k > 64"): the scan stores every (pair, list row) score and a segmented select keeps kc2 per pair.
+  // The exact fallback takes the same steps with exact scores, of which each pair needs only its k best.
+  const bool large_k = k > 64 || exact;
+  const int large_kc = exact ? k : std::min(2 * k, kSelectMaxK);
   // Query batching.  Per (query, probe) pair: the bf16 query residual row and its offset, 2 x KC candidate slots and their
   // per-query concatenation.  k > 64, per query: dense scores (bounded by its n_probes largest lists), each pair's kc2 best and their
   // per-query gather (8 + 8 bytes each), the gathered bf16 query rows, slot bookkeeping (32 bytes per pair) and the merged kc2.
@@ -301,8 +538,9 @@ void ivf_flat_search(resources* res, const ivf_flat_index& idx, uint32_t n_probe
                                              static_cast<int64_t>(n_probes) * (16 * large_kc + 2 * idx.Kp + 32) +
                                              static_cast<int64_t>(large_kc) * 8;
   const int64_t batch = query_batch_size(idx.Kp * 2 + 4 + 2 * 64 * 8 + 16, n_probes, large_k_bytes, "CUVS_B200_FLAT_LARGE_K_BUDGET_MB");
+  B2_EXPECTS(dump == nullptr || nq <= batch, "ivf_flat candidates: %lld queries do not fit one batch", (long long)nq);
   if (search_in_batches(batch, qt, nt, dt, [&](const DLTensor& qs, const DLTensor& ns, const DLTensor& ds) {
-        ivf_flat_search(res, idx, n_probes, qs, ns, ds, keep_bits, n_bits, store);
+        ivf_flat_search(res, idx, n_probes, qs, ns, ds, keep_bits, n_bits, exact);
       }))
     return;
   const float* q   = dl_ptr<float>(qt);
@@ -322,10 +560,11 @@ void ivf_flat_search(resources* res, const ivf_flat_index& idx, uint32_t n_probe
   dbuf<uint32_t> probes(static_cast<size_t>(nq) * n_probes, s);
   coarse_select(res, qp, idx.centers_tc, static_cast<int>(n_probes), probes.data(), nullptr);
 
-  // ---- 1b. bitset pre-filter (cuvs::neighbors::filtering::bitset_filter): one pass over the half-norm plane
+  // ---- 1b. bitset pre-filter (cuvs::neighbors::filtering::bitset_filter): one pass over the half-norm plane (the exact
+  // fallback reads the bitset itself)
   dbuf<__nv_bfloat16> hx_f;
   const __nv_bfloat16* hx = idx.hx.data();
-  if (keep_bits != nullptr && idx.lists.rows_total > 0) {
+  if (keep_bits != nullptr && idx.lists.rows_total > 0 && !exact) {
     const int64_t R = idx.lists.rows_total;
     dbuf<float> hn(static_cast<size_t>(R), s);
     hx_f.alloc(static_cast<size_t>(std::max<int64_t>(R, 128)) * 16, s);
@@ -341,30 +580,43 @@ void ivf_flat_search(resources* res, const ivf_flat_index& idx, uint32_t n_probe
   // The scan ranks rows by a ONE-pass bf16 score; the exact fp32 re-score below only sees what survives it.  Keep slack
   // between k and the per-list capacity (and the shared pruning bound, which tracks the KC-th best): a true top-k row whose
   // bf16 score ranks a few places late must still be a candidate.  k <= 10 -> 16 slots, k <= 32 -> 32 slots; the bound is
-  // only used when KC >= 1.5 k.
+  // only used when KC >= 1.5 k.  Step 5 certifies the result.
   // k > 64: no fused top-k (KC = 0, the store epilogue); each pair keeps its kc2 best from its dense score segment.
   const int KC    = large_k ? 0 : ((k + k / 2 <= 16) ? 16 : 32);
   const bool use_bound = !large_k && KC >= k + k / 2;
   int KCW         = KC * kTcListsPerItem;
   probe_buckets pb;
   bucket_probes(res, probes.data(), nq, static_cast<int>(n_probes), idx.n_lists, idx.lists.d_offsets.data(), KCW, pb);
+  cuvsDistanceType fine = idx.metric == InnerProduct ? InnerProduct : (idx.metric == CosineExpanded ? CosineExpanded : L2Unexpanded);
 
   // ---- 3. fine scan: per-pair query residuals (A) x list residuals (B).  Scores of different pairs compare as distances,
   // add[slot] + scale * score (pair_residual_rows); cosine scores the unit query as L2 (scan_metric).
-  const float* qf = q;
-  dbuf<float> q_unit;
-  if (idx.metric == CosineExpanded) {
-    q_unit.alloc(static_cast<size_t>(nq) * idx.dim, s);
-    B2_CUDA(cudaMemcpyAsync(q_unit.data(), q, sizeof(float) * nq * idx.dim, cudaMemcpyDeviceToDevice, s));
-    normalize_rows(s, q_unit.data(), nq, idx.dim, idx.dim);
-    qf = q_unit.data();
-  }
   residual_rows a;
   dbuf<float> add;
-  const float scale = pair_residual_rows(s, qf, residual_centers(idx), idx.dim, idx.Kp, scan_metric(idx), pb, false, a, add);
+  float scale = 1.f;
+  if (!exact) {
+    const float* qf = q;
+    dbuf<float> q_unit;
+    if (idx.metric == CosineExpanded) {
+      q_unit.alloc(static_cast<size_t>(nq) * idx.dim, s);
+      B2_CUDA(cudaMemcpyAsync(q_unit.data(), q, sizeof(float) * nq * idx.dim, cudaMemcpyDeviceToDevice, s));
+      normalize_rows(s, q_unit.data(), nq, idx.dim, idx.dim);
+      qf = q_unit.data();
+    }
+    scale = pair_residual_rows(s, qf, residual_centers(idx), idx.dim, idx.Kp, scan_metric(idx), pb, false, a, add);
+  }
   dbuf<float> cs;
   dbuf<uint32_t> cp;
-  if (large_k) {
+  if (exact) {
+    large_k_select(s, pb, idx.lists, nq, n_probes, large_kc, [&](float* scores, const int64_t* seg_off) {
+      count_launch();
+      exact_segments_kernel<<<static_cast<unsigned>(std::max<int64_t>(pb.n_pairs, 1)), 128, 0, s>>>(
+        q, idx.dim, idx.data.data(), qn.data(), idx.xn.data(), idx.ids.data(), int(fine), pb.pair_query.data(), pb.pair_list.data(),
+        pb.n_items.data() + 1, idx.lists.d_offsets.data(), seg_off, keep_bits, n_bits, scores);
+      B2_CUDA(cudaGetLastError());
+    }, cs, cp);
+    KCW = large_kc;
+  } else if (large_k) {
     // every (pair, list row) score goes to the pair's dense segment; each pair keeps its kc2 best rows
     large_k_select(s, pb, idx.lists, nq, n_probes, large_kc, [&](float* scores, const int64_t* seg_off) {
       item_segments(s, pb, seg_off);
@@ -394,8 +646,11 @@ void ivf_flat_search(resources* res, const ivf_flat_index& idx, uint32_t n_probe
   dbuf<float> gs(static_cast<size_t>(nq) * cand_w, s);
   dbuf<uint32_t> gp(static_cast<size_t>(nq) * cand_w, s);
   // empty entries +inf: FLT_MAX made the ivf_flat bench search ~3 % slower (DESIGN.md §4a)
-  gather_probe_candidates(s, cs.data(), cp.data(), pb.slot_of.data(), add.data(), scale, INFINITY, nq, static_cast<int>(n_probes), KCW, gs.data(),
-                          gp.data());
+  const int L = large_k ? KCW : KC;  // entries of one per-pair list
+  dbuf<float> last;
+  if (!exact) last.alloc(static_cast<size_t>(nq * cand_w / L), s);
+  gather_probe_candidates(s, cs.data(), cp.data(), pb.slot_of.data(), exact ? nullptr : add.data(), scale, INFINITY, nq,
+                          static_cast<int>(n_probes), KCW, gs.data(), gp.data(), L, last.data());
   const int kc2 = static_cast<int>(std::min<int64_t>(cand_w, large_k ? large_kc : std::max(32, 2 * k)));
   dbuf<float> ms(static_cast<size_t>(nq) * kc2, s);
   dbuf<uint32_t> mp(static_cast<size_t>(nq) * kc2, s);
@@ -407,26 +662,54 @@ void ivf_flat_search(resources* res, const ivf_flat_index& idx, uint32_t n_probe
     drop_nonfinite_kernel<<<blocks_for(nq * kc2, 256), 256, 0, s>>>(ms.data(), mp.data(), nq * kc2);
     B2_CUDA(cudaGetLastError());
   }
-  cuvsDistanceType fine = idx.metric == InnerProduct ? InnerProduct : (idx.metric == CosineExpanded ? CosineExpanded : L2Unexpanded);
   rescore_topk(s, q, nq, idx.dim, idx.data.data(), idx.dim, idx.dim, qn.data(), idx.xn.data(), fine, mp.data(), nullptr, kc2,
                idx.ids.data(), k, out_idx, out_dist, INT64_MAX, approx_map{}, nullptr, nullptr);
-  postprocess_distances(s, out_dist, nq * k, idx.metric);
+  if (exact) {
+    postprocess_distances(s, out_dist, nq * k, idx.metric);
+    return;
+  }
 
-  // ---- 5. 32 < k <= 64: queries whose pairs may have dropped a candidate (a full column half, flag_truncated_halves_kernel)
-  // are searched again on the store path, whose per-pair selection has no per-half limit.  k <= 32 keeps KC >= k per half.
-  if (large_k || k <= 32) return;
+  // ---- 5. certificate (certify_kernel): the queries whose k-th exact distance is not safely below every row the bf16
+  // candidates left out are searched again with exact scores and their rows written back
   dbuf<int> flags(static_cast<size_t>(nq) + 1, s);
   B2_CUDA(cudaMemsetAsync(flags.data() + nq, 0, sizeof(int), s));
   count_launch();
-  flag_truncated_halves_kernel<<<blocks_for(nq, 256), 256, 0, s>>>(cs.data(), cp.data(), pb.slot_of.data(), add.data(), scale, ms.data(),
-                                                                   nq, static_cast<int>(n_probes), KC, KCW, kc2, flags.data());
+  certify_kernel<<<blocks_for(nq * 32, 256), 256, 0, s>>>(out_dist, k, int(fine), ms.data(), kc2, last.data(), KCW / L,
+                                                         probes.data(), pb.slot_of.data(), static_cast<int>(n_probes),
+                                                         add.data(), qn.data(), idx.rn_max.data(), idx.cn.data(), make_budget(idx, scale),
+                                                         nq, flags.data());
   B2_CUDA(cudaGetLastError());
-  std::vector<int> hflags(static_cast<size_t>(nq) + 1);
-  B2_CUDA(cudaMemcpyAsync(hflags.data(), flags.data(), sizeof(int) * (nq + 1), cudaMemcpyDeviceToHost, s));
+  if (dump) {
+    count_launch();
+    candidate_budget_kernel<<<blocks_for(nq * kc2, 256), 256, 0, s>>>(mp.data(), idx.ids.data(), idx.lists.d_offsets.data(), idx.n_lists,
+                                                                      probes.data(), pb.slot_of.data(), static_cast<int>(n_probes), kc2,
+                                                                      add.data(), qn.data(), idx.rn_max.data(), idx.cn.data(),
+                                                                      make_budget(idx, scale), nq * kc2, dump->ids, dump->bound);
+    B2_CUDA(cudaGetLastError());
+    B2_CUDA(cudaMemcpyAsync(dump->dist, ms.data(), sizeof(float) * nq * kc2, cudaMemcpyDeviceToDevice, s));
+    B2_CUDA(cudaStreamSynchronize(s));
+    return;
+  }
+  if (!large_k) {
+    count_launch();
+    exact_fallback_kernel<<<static_cast<unsigned>(std::min<int64_t>(nq, 1024)), kFbThreads, 0, s>>>(
+      flags.data(), probes.data(), static_cast<int>(n_probes), idx.lists.d_offsets.data(), q, idx.dim, idx.data.data(), qn.data(),
+      idx.xn.data(), idx.ids.data(), int(fine), keep_bits, n_bits, k, nq, out_idx, out_dist);
+    B2_CUDA(cudaGetLastError());
+    postprocess_distances(s, out_dist, nq * k, idx.metric);
+    set_last_flagged_async(flags.data() + nq, s);
+    return;
+  }
+  // k > 64: the flagged queries are gathered and searched again with exact scores (exact_segments_kernel)
+  postprocess_distances(s, out_dist, nq * k, idx.metric);
+  int n_flagged = 0;
+  B2_CUDA(cudaMemcpyAsync(&n_flagged, flags.data() + nq, sizeof(int), cudaMemcpyDeviceToHost, s));
   B2_CUDA(cudaStreamSynchronize(s));
-  const int64_t n_flagged = hflags[nq];
-  set_last_flagged(static_cast<int>(n_flagged));
+  set_last_flagged(n_flagged);
   if (n_flagged == 0) return;
+  std::vector<int> hflags(static_cast<size_t>(nq));
+  B2_CUDA(cudaMemcpyAsync(hflags.data(), flags.data(), sizeof(int) * nq, cudaMemcpyDeviceToHost, s));
+  B2_CUDA(cudaStreamSynchronize(s));
   std::vector<int64_t> hrows;
   hrows.reserve(static_cast<size_t>(n_flagged));
   for (int64_t i = 0; i < nq; ++i)
@@ -541,6 +824,38 @@ cuvsError_t cuvsB200IvfFlatSetCenters(cuvsResources_t res, cuvsIvfFlatIndex_t in
   });
 }
 cuvsError_t cuvsB200IvfFlatGetSize(cuvsIvfFlatIndex_t index, int64_t* size) { return guarded([=] { *size = flat_of(index).lists.size; }); }
+
+cuvsError_t cuvsB200IvfFlatCandidates(cuvsResources_t res, cuvsIvfFlatIndex_t index, uint32_t n_probes, int k, DLManagedTensor* queries,
+                                      DLManagedTensor* cand_ids, DLManagedTensor* cand_dist, DLManagedTensor* bound)
+{
+  return guarded([=] {
+    auto r    = as_res(res);
+    auto& idx = flat_of(index);
+    B2_EXPECTS(queries && cand_ids && cand_dist && bound, "null argument");
+    const DLTensor& q  = queries->dl_tensor;
+    const DLTensor& ci = cand_ids->dl_tensor;
+    const DLTensor& cd = cand_dist->dl_tensor;
+    const DLTensor& b  = bound->dl_tensor;
+    B2_EXPECTS(dl_is(q, kDLFloat, 32) && dl_is_device(q) && dl_is_c_contiguous(q) && q.ndim == 2 && q.shape[1] == idx.dim, "bad queries");
+    B2_EXPECTS(k >= 1 && k <= 64, "k must be in [1, 64]");
+    const int64_t nq = q.shape[0];
+    const int kc2    = std::max(32, 2 * k);
+    B2_EXPECTS(dl_is(ci, kDLInt, 64) && dl_is(cd, kDLFloat, 32) && dl_is(b, kDLFloat, 32) && dl_is_device(ci) && dl_is_device(cd) &&
+                 dl_is_device(b) && ci.ndim == 2 && cd.ndim == 2 && ci.shape[0] == nq && cd.shape[0] == nq && ci.shape[1] == kc2 &&
+                 cd.shape[1] == kc2 && b.ndim == 2 && b.shape[0] == nq && b.shape[1] == kc2 && dl_is_c_contiguous(ci) &&
+                 dl_is_c_contiguous(cd) && dl_is_c_contiguous(b),
+               "cand_ids / cand_dist / bound must be [nq, max(32, 2k)] int64 / float32 / float32, on the device");
+    B2_EXPECTS(static_cast<int64_t>(std::min(n_probes, idx.n_lists)) * 2 * (k + k / 2 <= 16 ? 16 : 32) >= kc2, "n_probes too small for kc2");
+    dbuf<int64_t> ni(static_cast<size_t>(nq) * k, r->stream);
+    dbuf<float> nd(static_cast<size_t>(nq) * k, r->stream);
+    int64_t shape[2] = {nq, k};
+    DLTensor nt{}, dt{};
+    nt.data = ni.data(); nt.device = q.device; nt.ndim = 2; nt.dtype = DLDataType{kDLInt, 64, 1}; nt.shape = shape;
+    dt.data = nd.data(); dt.device = q.device; dt.ndim = 2; dt.dtype = DLDataType{kDLFloat, 32, 1}; dt.shape = shape;
+    flat_candidates c{dl_ptr<int64_t>(ci), dl_ptr<float>(cd), dl_ptr<float>(b)};
+    ivf_flat_search(r, idx, n_probes, q, nt, dt, nullptr, 0, false, &c);
+  });
+}
 
 cuvsError_t cuvsIvfFlatBuild(cuvsResources_t res, cuvsIvfFlatIndexParams_t params, DLManagedTensor* dataset, cuvsIvfFlatIndex_t index)
 {

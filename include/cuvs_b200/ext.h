@@ -23,8 +23,8 @@ CUVS_EXPORT void cuvsB200TimingReset(void);
  * and returns their summed duration in milliseconds; *count receives the number of launches. */
 CUVS_EXPORT double cuvsB200TimingTotalMs(const char* name, int* count);
 
-/* Number of queries of the calling thread's last cuvsBruteForceSearch that failed the candidate
- * certificate and were recomputed on the exact path, and the number of kernels that search launched. */
+/* Number of queries of the calling thread's last cuvsBruteForceSearch (or last IVF-Flat query batch) that failed the
+ * candidate certificate and were recomputed on the exact path, and the number of kernels that search launched. */
 CUVS_EXPORT int cuvsB200LastFlagged(void);
 CUVS_EXPORT long long cuvsB200KernelLaunches(void);
 
@@ -43,6 +43,14 @@ CUVS_EXPORT cuvsError_t cuvsB200IvfFlatGetSize(cuvsIvfFlatIndex_t index, int64_t
 /* Replace the coarse centres of an (empty) index — used by the list-sharded multi-GPU build so that every rank
  * partitions the data with bit-identical centres (trained on one rank, broadcast over NCCL). centers: [n_lists, dim] f32. */
 CUVS_EXPORT cuvsError_t cuvsB200IvfFlatSetCenters(cuvsResources_t res, cuvsIvfFlatIndex_t index, DLManagedTensor* centers);
+/* IVF-Flat fine-scan candidates of a search at k (1..64) with n_probes, as its certificate sees them (DESIGN.md §4): per
+ * query the kc2 = cand_ids.shape[1] merged candidates (kc2 must be max(32, 2k)) by their approximate distance in the scan's
+ * units (|q - x|^2 for L2, 2 (1 - cos) for cosine, -q.x for inner product; INT64_MAX / +inf for empty slots), and for each
+ * the error budget of its own (query, list) pair against the exact fp32 distance (+inf for empty slots).  queries: f32
+ * device [nq, dim], one query batch. */
+CUVS_EXPORT cuvsError_t cuvsB200IvfFlatCandidates(cuvsResources_t res, cuvsIvfFlatIndex_t index, uint32_t n_probes, int k,
+                                                  DLManagedTensor* queries, DLManagedTensor* cand_ids /*[nq, kc2] i64*/,
+                                                  DLManagedTensor* cand_dist /*[nq, kc2] f32*/, DLManagedTensor* bound /*[nq, kc2] f32*/);
 
 /* IVF-PQ: which fine-scan kernel cuvsIvfPqSearch will use on this index by default, and the device bytes the index holds.
  * *path: bit 1 (value 2) = the index holds the code stream (code-streaming wgmma scan, scan_pq.cu), bit 0 (value 1) = it holds
