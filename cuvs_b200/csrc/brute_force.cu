@@ -10,10 +10,10 @@
 //   1. candidate scan on wgmma (scan_tc.cu): s = |x|^2/2 - q.x with split-bf16 products, a
 //      register top-k' per query row per dataset split, no distance matrix in HBM;
 //   2. merge of the per-split lists (select_k.cu);
-//   3. exact fp32 re-scoring of the k' candidates in the oracle's arithmetic (exact.cu), which
-//      also evaluates a certificate: if the k-th exact distance is not strictly below the worst
+//   3. exact fp32 re-scoring of the k' candidates in the oracle's arithmetic (exact.cu);
+//   4. a certificate (bf_certify_kernel): if the k-th exact distance is not strictly below the worst
 //      candidate's approximate distance minus the error budget, the query is flagged;
-//   4. flagged queries (ties / duplicates at the k' boundary) are recomputed by the exact SIMT
+//   5. flagged queries (ties / duplicates at the k' boundary) are recomputed by the exact SIMT
 //      path.  Result: identical to oracle/oracle.c::oracle_knn, bit for bit.
 // Filtered search and shapes the tensor-core kernel does not cover (dim > 2048, k > 64)
 // run on the exact SIMT path.
@@ -71,12 +71,6 @@ __global__ void transpose_kernel(const float* __restrict__ in, float* __restrict
   int64_t r = t / d;
   int c     = static_cast<int>(t % d);
   out[t]    = in[static_cast<int64_t>(c) * n + r];
-}
-
-__global__ void rsqrt_kernel(const float* __restrict__ xn, float* __restrict__ out, int64_t n)
-{
-  int64_t i = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x;
-  if (i < n) out[i] = xn[i] > 0.f ? 1.0f / sqrtf(xn[i]) : 0.f;
 }
 
 __global__ void max_kernel(const float* __restrict__ v, int64_t n, float* __restrict__ out)
@@ -174,8 +168,7 @@ static bf_index* bf_build(resources* res, const DLTensor& ds, cuvsDistanceType m
     const float* scale = nullptr;
     if (metric == CosineExpanded) {
       idx->inv_norm.alloc(static_cast<size_t>(idx->n));
-      rsqrt_kernel<<<static_cast<unsigned>((idx->n + 255) / 256), 256, 0, stream>>>(idx->norms.data(), idx->inv_norm.data(), idx->n);
-      B2_CUDA(cudaGetLastError());
+      rsqrt_rows(stream, idx->norms.data(), idx->n, idx->inv_norm.data());
       scale = idx->inv_norm.data();
     }
     tc_split_planes(stream, idx->data, idx->n, idx->d, idx->d, idx->Kp, idx->hi.data(), idx->lo.data(), idx->rows_pad, scale);
@@ -260,9 +253,7 @@ static void bf_tc_candidates(resources* res, const bf_index& idx, const float* q
   dbuf<float> qscale;
   if (idx.metric == CosineExpanded) {
     qscale.alloc(static_cast<size_t>(nq), stream);
-    rsqrt_kernel<<<static_cast<unsigned>((nq + 255) / 256), 256, 0, stream>>>(out.qn.data(), qscale.data(), nq);
-    B2_CUDA(cudaGetLastError());
-    count_launch();
+    rsqrt_rows(stream, out.qn.data(), nq, qscale.data());
   }
   dbuf<__nv_bfloat16> qhi(static_cast<size_t>(nq_pad) * idx.Kp, stream), qlo(static_cast<size_t>(nq_pad) * idx.Kp, stream);
   tc_split_planes(stream, q, nq, idx.d, idx.d, idx.Kp, qhi.data(), qlo.data(), nq_pad, qscale.data());
@@ -301,6 +292,13 @@ static void bf_tc_candidates(resources* res, const bf_index& idx, const float* q
   }
 }
 
+/** How a raw scan score s of the tensor-core engine maps to the metric's selection form, and the
+ *  error budget of that approximation:  A = sa*s + sb*|q|^2 + sc,  eps = eps_rel * (eq*|q|^2 + ec). */
+struct approx_map {
+  float sa = 1.f, sb = 0.f, sc = 0.f;
+  float eps_rel = 0.f, eq = 0.f, ec = 0.f;
+};
+
 static approx_map bf_approx_map(const bf_index& idx)
 {
   approx_map am;
@@ -312,6 +310,54 @@ static approx_map bf_approx_map(const bf_index& idx)
   else if (idx.metric == CosineExpanded) { am.sa = 1.f; am.sc = 1.f; am.eq = 0.f; am.ec = 2.f; }
   else { am.sa = 2.f; am.sb = 1.f; am.eq = 1.f; am.ec = idx.xn_max; }
   return am;
+}
+
+// The certificate (DESIGN.md §3), one warp per query: flags[q] = 1 (flags[nq] counts them) unless the exact k-th distance
+// out_dist[q, k-1] (selection form, before postprocess_distances) beats the worst approximate score A of the rows outside the
+// candidates by more than eps_rel * (eq |q|^2 + ec).  Such rows exist when the candidate list is full and score worse than its
+// worst entry; with a floor (raw engine units, +inf: none), the bound of the rows that never entered a list, also worse than it.
+__global__ void bf_certify_kernel(const float* __restrict__ cand_score, const uint32_t* __restrict__ cand_pos, int kc,
+                                  const float* __restrict__ approx_floor, const float* __restrict__ qn,
+                                  const float* __restrict__ out_dist, int k, approx_map amap, bool select_min, int64_t nq,
+                                  int* __restrict__ flags)
+{
+  const int64_t qi = (blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x) >> 5;
+  const int lane   = threadIdx.x & 31;
+  if (qi >= nq) return;
+  const float qnv    = qn[qi];
+  float worst_approx = select_min ? -FLT_MAX : FLT_MAX;
+  int n_valid        = 0;
+  for (int c = lane; c < kc; c += 32) {
+    if (cand_pos[qi * kc + c] == 0xffffffffu) continue;
+    ++n_valid;
+    float a      = amap.sa * cand_score[qi * kc + c] + amap.sb * qnv + amap.sc;
+    worst_approx = select_min ? fmaxf(worst_approx, a) : fminf(worst_approx, a);
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    n_valid += __shfl_xor_sync(0xffffffffu, n_valid, o);
+    float t = __shfl_xor_sync(0xffffffffu, worst_approx, o);
+    worst_approx = select_min ? fmaxf(worst_approx, t) : fminf(worst_approx, t);
+  }
+  if (lane != 0) return;
+  const float kth = out_dist[qi * k + k - 1];
+  int flag        = 0;
+  bool outside    = n_valid == kc;  // candidate list is full: rows outside it exist (dropped by the merge to kc)
+  if (approx_floor != nullptr) {
+    const float fl = approx_floor[qi];
+    if (fl < FLT_MAX) {
+      const float a = amap.sa * fl + amap.sb * qnv + amap.sc;
+      worst_approx  = !outside ? a : (select_min ? fminf(worst_approx, a) : fmaxf(worst_approx, a));
+      outside       = true;
+    }
+  }
+  if (outside) {
+    float eps = amap.eps_rel * (amap.eq * qnv + amap.ec);
+    bool ok   = select_min ? (kth < worst_approx - eps) : (kth > worst_approx + eps);
+    flag      = ok ? 0 : 1;
+  }
+  flags[qi] = flag;
+  if (flag) atomicAdd(flags + nq, 1);
 }
 
 static void bf_search(resources* res, const bf_index& idx, const DLTensor& qt, const DLTensor& nt, const DLTensor& dt,
@@ -368,36 +414,26 @@ static void bf_search(resources* res, const bf_index& idx, const DLTensor& qt, c
   const int KCm = k <= 24 ? KC : (k <= 48 ? 64 : 96);
   bf_cands cand;
   bf_tc_candidates(res, idx, q, nq, KC, cand, KCm);
-  const float* m_score  = cand.score.data();
-  const uint32_t* m_pos = cand.pos.data();
-  dbuf<float>& qn       = cand.qn;
 
-  // ---- exact re-scoring + certificate
-  const approx_map am = bf_approx_map(idx);
+  // ---- exact re-scoring
+  const bool need_xn = (idx.metric == L2Expanded || idx.metric == L2SqrtExpanded || idx.metric == CosineExpanded);
+  rescore_topk(stream, q, nq, idx.d, idx.data, idx.d, idx.d, cand.qn.data(), need_xn ? idx.norms.data() : nullptr, idx.metric,
+               cand.pos.data(), cand.width, nullptr, k, out_idx, out_dist, -1);
+
+  // ---- certificate, and the exact path for flagged queries (rare: exact ties / duplicates at the k' boundary)
   dbuf<int> flags(static_cast<size_t>(nq) + 1, stream);
   B2_CUDA(cudaMemsetAsync(flags.data() + nq, 0, sizeof(int), stream));
-  const bool need_xn = (idx.metric == L2Expanded || idx.metric == L2SqrtExpanded || idx.metric == CosineExpanded);
-  rescore_topk(stream, q, nq, idx.d, idx.data, idx.d, idx.d, qn.data(), need_xn ? idx.norms.data() : nullptr, idx.metric,
-               m_pos, m_score, cand.width, nullptr, k, out_idx, out_dist, -1, am, flags.data(), flags.data() + nq, cand.floor.data());
-
-  // ---- certified fallback for flagged queries (rare: exact ties / duplicates at the k' boundary)
-  int n_flagged = 0;
-  B2_CUDA(cudaMemcpyAsync(&n_flagged, flags.data() + nq, sizeof(int), cudaMemcpyDeviceToHost, stream));
-  B2_CUDA(cudaStreamSynchronize(stream));
-  set_last_flagged(n_flagged);
-  if (n_flagged > 0) {
-    std::vector<int> hflags(static_cast<size_t>(nq));
-    B2_CUDA(cudaMemcpyAsync(hflags.data(), flags.data(), sizeof(int) * nq, cudaMemcpyDeviceToHost, stream));
-    B2_CUDA(cudaStreamSynchronize(stream));
-    int64_t i = 0;
-    while (i < nq) {
-      if (!hflags[i]) { ++i; continue; }
-      int64_t j = i;
-      while (j < nq && hflags[j]) ++j;  // contiguous run of flagged queries
-      search_exact(res, idx, q + i * idx.d, j - i, i, k, out_idx + i * k, out_dist + i * k, filter_view{});
-      i = j;
-    }
-  }
+  count_launch();
+  bf_certify_kernel<<<blocks_for(nq * 32, 256), 256, 0, stream>>>(cand.score.data(), cand.pos.data(), cand.width, cand.floor.data(),
+                                                                  cand.qn.data(), out_dist, k, bf_approx_map(idx), select_min, nq,
+                                                                  flags.data());
+  B2_CUDA(cudaGetLastError());
+  // search_exact answers every query on its own, and these run unfiltered, so the gathered rows get the same bits
+  rerun_flagged(stream, flags.data(), nq, k, out_idx, out_dist, [&](const int64_t* rows, int64_t n, int64_t* fi, float* fd) {
+    dbuf<float> fq(static_cast<size_t>(n) * idx.d, stream);
+    copy_rows(stream, q, rows, fq.data(), nullptr, n, idx.d);
+    search_exact(res, idx, fq.data(), n, 0, k, fi, fd, filter_view{});
+  });
   postprocess_distances(stream, out_dist, nq * k, idx.metric);
 }
 

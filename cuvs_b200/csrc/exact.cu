@@ -5,9 +5,11 @@
 //   post-selection sqrt       cpp/src/neighbors/detail/knn_brute_force.cuh:468-479
 #include "common.hpp"
 #include "exact.cuh"
+#include "exact_device.cuh"
 #include "timing.hpp"
 
 #include <cfloat>
+#include <vector>
 
 namespace b200 {
 namespace {
@@ -53,21 +55,6 @@ __device__ __forceinline__ bool keep_sample(const filter_view& f, int64_t q, int
   if (f.kind == 0) return true;
   int64_t bit = f.kind == 1 ? j : q * f.n_samples + j;
   return (f.bits[bit >> 5] >> (bit & 31)) & 1u;
-}
-
-__device__ __forceinline__ float finish_distance(float acc, float qn, float xn, int metric)
-{
-  switch (metric) {
-    case L2Expanded:
-    case L2SqrtExpanded: {
-      float val = fmaf(-2.0f, acc, qn + xn);
-      if (!(val > 0.0f)) val = 0.0f;
-      if (val * val < 1e-6f && qn == xn) val = 0.0f;
-      return val;
-    }
-    case CosineExpanded: return 1.0f - acc / (sqrtf(qn) * sqrtf(xn));
-    default: return acc;  // InnerProduct, L2Unexpanded (acc already holds the sum of squares)
-  }
 }
 
 constexpr int TM = 64, TN = 64, TK = 16;
@@ -147,13 +134,10 @@ constexpr int kMaxCandBlock = 2048;  // one CTA per query
 __global__ void __launch_bounds__(128) rescore_kernel(const float* __restrict__ q, int64_t nq, int64_t ldq,
                                                        const float* __restrict__ x, int64_t ldx, int d,
                                                        const float* __restrict__ qn, const float* __restrict__ xn,
-                                                       int metric, const uint32_t* __restrict__ cand_pos,
-                                                       const float* __restrict__ cand_score, int kc,
+                                                       int metric, const uint32_t* __restrict__ cand_pos, int kc,
                                                        const int64_t* __restrict__ src_ids, int k,
                                                        int64_t* __restrict__ out_idx, float* __restrict__ out_dist,
-                                                       int64_t pad_id, approx_map amap,
-                                                       int* __restrict__ flags, int* __restrict__ n_flagged,
-                                                       const float* __restrict__ approx_floor)
+                                                       int64_t pad_id)
 {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   const int warps = blockDim.x >> 5, wid = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -165,63 +149,22 @@ __global__ void __launch_bounds__(128) rescore_kernel(const float* __restrict__ 
   const bool select_min = metric != InnerProduct;
   const float* qr       = q + qi * ldq;
   const float qnv       = qn ? qn[qi] : 0.f;
-  const bool sqdiff     = (metric == L2Unexpanded || metric == L2SqrtUnexpanded);
-  const bool vec4       = ((d & 3) == 0) && ((ldx & 3) == 0) && ((ldq & 3) == 0) &&
-                    ((reinterpret_cast<uintptr_t>(x) & 15) == 0) && ((reinterpret_cast<uintptr_t>(q) & 15) == 0);
+  const bool vec4       = exact_vec4(q, ldq, x, ldx, d);
 
-  float worst_approx = select_min ? -FLT_MAX : FLT_MAX;
-  int n_valid        = 0;
   for (int c = lane; c < kc; c += 32) {
     uint32_t pos = cand_pos[qi * kc + c];
     float dist   = select_min ? FLT_MAX : -FLT_MAX;
     int64_t id   = INT64_MAX;
     if (pos != 0xffffffffu) {
-      const float* xr = x + static_cast<int64_t>(pos) * ldx;
-      float acc       = 0.f;
-      if (vec4) {
-        const float4* x4 = reinterpret_cast<const float4*>(xr);
-        const float4* q4 = reinterpret_cast<const float4*>(qr);
-        for (int kk = 0; kk < d / 4; ++kk) {
-          float4 a = q4[kk], b = x4[kk];
-          if (sqdiff) {
-            float t;
-            t = a.x - b.x; acc = fmaf(t, t, acc);
-            t = a.y - b.y; acc = fmaf(t, t, acc);
-            t = a.z - b.z; acc = fmaf(t, t, acc);
-            t = a.w - b.w; acc = fmaf(t, t, acc);
-          } else {
-            acc = fmaf(a.x, b.x, acc);
-            acc = fmaf(a.y, b.y, acc);
-            acc = fmaf(a.z, b.z, acc);
-            acc = fmaf(a.w, b.w, acc);
-          }
-        }
-      } else {
-        for (int kk = 0; kk < d; ++kk) {
-          if (sqdiff) { float t = qr[kk] - xr[kk]; acc = fmaf(t, t, acc); }
-          else acc = fmaf(qr[kk], xr[kk], acc);
-        }
-      }
-      dist = finish_distance(acc, qnv, xn ? xn[pos] : 0.f, metric);
+      const float acc = exact_accumulate(qr, x + static_cast<int64_t>(pos) * ldx, d, vec4, metric);
+      dist            = finish_distance(acc, qnv, xn ? xn[pos] : 0.f, metric);
       id   = src_ids ? src_ids[pos] : static_cast<int64_t>(pos);
-      ++n_valid;
-      if (cand_score) {
-        float a      = amap.sa * cand_score[qi * kc + c] + amap.sb * qnv + amap.sc;
-        worst_approx = select_min ? fmaxf(worst_approx, a) : fminf(worst_approx, a);
-      }
     }
     sd[c] = dist;
     si[c] = id;
   }
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) {
-    n_valid += __shfl_xor_sync(0xffffffffu, n_valid, o);
-    float t = __shfl_xor_sync(0xffffffffu, worst_approx, o);
-    worst_approx = select_min ? fmaxf(worst_approx, t) : fminf(worst_approx, t);
-  }
   __syncwarp();
   // rank by (distance, id, slot): unique ranks even among empty slots
-  float kth = select_min ? FLT_MAX : -FLT_MAX;
   for (int c = lane; c < kc; c += 32) {
     float dv = sd[c];
     int64_t iv = si[c];
@@ -236,47 +179,17 @@ __global__ void __launch_bounds__(128) rescore_kernel(const float* __restrict__ 
       bool valid = iv != INT64_MAX;
       out_idx[qi * k + rank]  = valid ? iv : pad_id;
       out_dist[qi * k + rank] = dv;
-      if (rank == k - 1) kth = dv;
     }
   }
   for (int j = kc + lane; j < k; j += 32) {  // k > kc: pad
     out_idx[qi * k + j]  = pad_id;
     out_dist[qi * k + j] = select_min ? FLT_MAX : -FLT_MAX;
   }
-  if (flags) {
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) {
-      float t = __shfl_xor_sync(0xffffffffu, kth, o);
-      kth     = select_min ? fminf(kth, t) : fmaxf(kth, t);
-    }
-    if (lane == 0) {
-      int flag = 0;
-      bool outside = n_valid == kc;  // candidate list is full: rows outside it exist (dropped by the merge to kc)
-      if (approx_floor != nullptr && cand_score) {
-        // a second bound, in raw engine units, on the rows that never entered a candidate list (brute force with k above the
-        // fused list length: such rows are bounded by the lists' own worst entries, not by the merged set's); +inf = none
-        const float fl = approx_floor[qi];
-        if (fl < FLT_MAX) {
-          const float a = amap.sa * fl + amap.sb * qnv + amap.sc;
-          worst_approx  = !outside ? a : (select_min ? fminf(worst_approx, a) : fmaxf(worst_approx, a));
-          outside       = true;
-        }
-      }
-      if (outside && cand_score) {
-        float eps = amap.eps_rel * (amap.eq * qnv + amap.ec);
-        bool ok   = select_min ? (kth < worst_approx - eps) : (kth > worst_approx + eps);
-        flag      = ok ? 0 : 1;
-      }
-      flags[qi] = flag;
-      if (flag && n_flagged) atomicAdd(n_flagged, 1);
-    }
-  }
 }
 
 // More candidates than one warp's shared memory holds (refine with 257..2048 candidates): one CTA per query.  Every candidate
-// is scored by one thread with rescore_kernel's arithmetic (same fmaf order, same vec4 rule), then the kc entries are sorted by
-// rescore_kernel's ranking rule, (distance, id, slot), with a bitonic sort over kpow2 entries; the padding entries (slot >= kc)
-// rank last.
+// is scored by one thread with exact_accumulate, as in rescore_kernel, then the kc entries are sorted by rescore_kernel's
+// ranking rule, (distance, id, slot), with a bitonic sort over kpow2 entries; the padding entries (slot >= kc) rank last.
 __global__ void __launch_bounds__(256) rescore_block_kernel(const float* __restrict__ q, int64_t ldq, const float* __restrict__ x,
                                                              int64_t ldx, int d, const float* __restrict__ qn,
                                                              const float* __restrict__ xn, int metric,
@@ -292,41 +205,14 @@ __global__ void __launch_bounds__(256) rescore_block_kernel(const float* __restr
   const bool select_min = metric != InnerProduct;
   const float* qr       = q + qi * ldq;
   const float qnv       = qn ? qn[qi] : 0.f;
-  const bool sqdiff     = (metric == L2Unexpanded || metric == L2SqrtUnexpanded);
-  const bool vec4       = ((d & 3) == 0) && ((ldx & 3) == 0) && ((ldq & 3) == 0) &&
-                    ((reinterpret_cast<uintptr_t>(x) & 15) == 0) && ((reinterpret_cast<uintptr_t>(q) & 15) == 0);
+  const bool vec4       = exact_vec4(q, ldq, x, ldx, d);
   for (int c = threadIdx.x; c < kpow2; c += blockDim.x) {
     float dist = select_min ? FLT_MAX : -FLT_MAX;
     int64_t id = INT64_MAX;
     const uint32_t pos = c < kc ? cand_pos[qi * kc + c] : 0xffffffffu;
     if (pos != 0xffffffffu) {
-      const float* xr = x + static_cast<int64_t>(pos) * ldx;
-      float acc       = 0.f;
-      if (vec4) {
-        const float4* x4 = reinterpret_cast<const float4*>(xr);
-        const float4* q4 = reinterpret_cast<const float4*>(qr);
-        for (int kk = 0; kk < d / 4; ++kk) {
-          float4 a = q4[kk], b = x4[kk];
-          if (sqdiff) {
-            float t;
-            t = a.x - b.x; acc = fmaf(t, t, acc);
-            t = a.y - b.y; acc = fmaf(t, t, acc);
-            t = a.z - b.z; acc = fmaf(t, t, acc);
-            t = a.w - b.w; acc = fmaf(t, t, acc);
-          } else {
-            acc = fmaf(a.x, b.x, acc);
-            acc = fmaf(a.y, b.y, acc);
-            acc = fmaf(a.z, b.z, acc);
-            acc = fmaf(a.w, b.w, acc);
-          }
-        }
-      } else {
-        for (int kk = 0; kk < d; ++kk) {
-          if (sqdiff) { float t = qr[kk] - xr[kk]; acc = fmaf(t, t, acc); }
-          else acc = fmaf(qr[kk], xr[kk], acc);
-        }
-      }
-      dist = finish_distance(acc, qnv, xn ? xn[pos] : 0.f, metric);
+      const float acc = exact_accumulate(qr, x + static_cast<int64_t>(pos) * ldx, d, vec4, metric);
+      dist            = finish_distance(acc, qnv, xn ? xn[pos] : 0.f, metric);
       id   = src_ids ? src_ids[pos] : static_cast<int64_t>(pos);
     }
     sd[c] = dist;
@@ -335,27 +221,12 @@ __global__ void __launch_bounds__(256) rescore_block_kernel(const float* __restr
   }
   __syncthreads();
   // a before b in the ranking (slots are unique, so this is a strict total order)
-  auto before = [&](float da, int64_t ia, int ca, float db, int64_t ib, int cb) {
-    const bool pa = ca >= kc, pb = cb >= kc;
+  block_bitonic_sort(sd, si, sc, kpow2, [&](int a, int b) {
+    const bool pa = sc[a] >= kc, pb = sc[b] >= kc;
     if (pa != pb) return pb;
-    if (da != db) return select_min ? da < db : da > db;
-    return ia != ib ? ia < ib : ca < cb;
-  };
-  for (int size = 2; size <= kpow2; size <<= 1) {
-    for (int stride = size >> 1; stride > 0; stride >>= 1) {
-      for (int i = threadIdx.x; i < (kpow2 >> 1); i += blockDim.x) {
-        const int lo = (i / stride) * (stride << 1) + (i % stride), hi = lo + stride;
-        const bool up = (lo & size) == 0;
-        const bool swap = before(sd[hi], si[hi], sc[hi], sd[lo], si[lo], sc[lo]) == up;
-        if (swap) {
-          const float td = sd[lo]; sd[lo] = sd[hi]; sd[hi] = td;
-          const int64_t ti = si[lo]; si[lo] = si[hi]; si[hi] = ti;
-          const int tc = sc[lo]; sc[lo] = sc[hi]; sc[hi] = tc;
-        }
-      }
-      __syncthreads();
-    }
-  }
+    if (sd[a] != sd[b]) return select_min ? sd[a] < sd[b] : sd[a] > sd[b];
+    return si[a] != si[b] ? si[a] < si[b] : sc[a] < sc[b];
+  });
   for (int j = threadIdx.x; j < k; j += blockDim.x) {
     const int64_t iv = si[j];
     out_idx[qi * k + j]  = iv != INT64_MAX ? iv : pad_id;
@@ -371,6 +242,17 @@ __global__ void postprocess_kernel(float* dist, int64_t count, int metric)
   if (metric == L2SqrtExpanded || metric == L2SqrtUnexpanded) {
     if (v != FLT_MAX) dist[i] = sqrtf(fmaxf(v, 0.f));
   }
+}
+
+// dst[dst_row(i)] = src[src_row(i)] for rows of `width` elements; a null row map is the identity
+template <typename T>
+__global__ void copy_rows_kernel(const T* __restrict__ src, const int64_t* __restrict__ src_rows, T* __restrict__ dst,
+                                 const int64_t* __restrict__ dst_rows, int64_t n, int64_t width)
+{
+  int64_t t = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x;
+  if (t >= n * width) return;
+  const int64_t i = t / width, j = t % width;
+  dst[(dst_rows ? dst_rows[i] : i) * width + j] = src[(src_rows ? src_rows[i] : i) * width + j];
 }
 
 }  // namespace
@@ -420,14 +302,12 @@ void exact_distance_tile(cudaStream_t stream, const float* q, int64_t nq, int64_
 }
 
 void rescore_topk(cudaStream_t stream, const float* q, int64_t nq, int64_t ldq, const float* x, int64_t ldx, int d,
-                  const float* qn, const float* xn, cuvsDistanceType metric, const uint32_t* cand_pos,
-                  const float* cand_score, int kc, const int64_t* src_ids, int k, int64_t* out_idx, float* out_dist,
-                  int64_t pad_id, const approx_map& amap, int* flags, int* n_flagged, const float* approx_floor)
+                  const float* qn, const float* xn, cuvsDistanceType metric, const uint32_t* cand_pos, int kc,
+                  const int64_t* src_ids, int k, int64_t* out_idx, float* out_dist, int64_t pad_id)
 {
   if (nq == 0) return;
   if (kc > kMaxCand) {
     B2_EXPECTS(kc <= kMaxCandBlock && k <= kc, "rescore_topk: candidate count %d out of range", kc);
-    B2_EXPECTS(cand_score == nullptr && flags == nullptr, "rescore_topk: the certificate takes at most %d candidates", kMaxCand);
     int kpow2 = 1;
     while (kpow2 < kc) kpow2 <<= 1;
     const size_t smem = static_cast<size_t>(kpow2) * (sizeof(int64_t) + sizeof(float) + sizeof(int));
@@ -442,9 +322,45 @@ void rescore_topk(cudaStream_t stream, const float* q, int64_t nq, int64_t ldq, 
   size_t smem     = static_cast<size_t>(warps) * kc * (sizeof(float) + sizeof(int64_t));
   count_launch();
   rescore_kernel<<<static_cast<unsigned>((nq + warps - 1) / warps), warps * 32, smem, stream>>>(
-    q, nq, ldq, x, ldx, d, qn, xn, int(metric), cand_pos, cand_score, kc, src_ids, k, out_idx, out_dist, pad_id, amap,
-    flags, n_flagged, approx_floor);
+    q, nq, ldq, x, ldx, d, qn, xn, int(metric), cand_pos, kc, src_ids, k, out_idx, out_dist, pad_id);
   B2_CUDA(cudaGetLastError());
+}
+
+template <typename T>
+void copy_rows(cudaStream_t s, const T* src, const int64_t* src_rows, T* dst, const int64_t* dst_rows, int64_t n, int64_t width)
+{
+  if (n == 0) return;
+  count_launch();
+  copy_rows_kernel<T><<<blocks_for(n * width, 256), 256, 0, s>>>(src, src_rows, dst, dst_rows, n, width);
+  B2_CUDA(cudaGetLastError());
+}
+template void copy_rows<float>(cudaStream_t, const float*, const int64_t*, float*, const int64_t*, int64_t, int64_t);
+template void copy_rows<int64_t>(cudaStream_t, const int64_t*, const int64_t*, int64_t*, const int64_t*, int64_t, int64_t);
+template void copy_rows<uint32_t>(cudaStream_t, const uint32_t*, const int64_t*, uint32_t*, const int64_t*, int64_t, int64_t);
+
+void rerun_flagged(cudaStream_t s, const int* flags, int64_t nq, int k, int64_t* out_idx, float* out_dist,
+                   const std::function<void(const int64_t* rows, int64_t n, int64_t* idx, float* dist)>& answer)
+{
+  int n_flagged = 0;
+  B2_CUDA(cudaMemcpyAsync(&n_flagged, flags + nq, sizeof(int), cudaMemcpyDeviceToHost, s));
+  B2_CUDA(cudaStreamSynchronize(s));
+  set_last_flagged(n_flagged);
+  if (n_flagged == 0) return;
+  std::vector<int> hflags(static_cast<size_t>(nq));
+  B2_CUDA(cudaMemcpyAsync(hflags.data(), flags, sizeof(int) * nq, cudaMemcpyDeviceToHost, s));
+  B2_CUDA(cudaStreamSynchronize(s));
+  std::vector<int64_t> hrows;
+  hrows.reserve(static_cast<size_t>(n_flagged));
+  for (int64_t i = 0; i < nq; ++i)
+    if (hflags[i]) hrows.push_back(i);
+  dbuf<int64_t> rows(static_cast<size_t>(n_flagged), s);
+  B2_CUDA(cudaMemcpyAsync(rows.data(), hrows.data(), sizeof(int64_t) * n_flagged, cudaMemcpyHostToDevice, s));
+  dbuf<int64_t> fi(static_cast<size_t>(n_flagged) * k, s);
+  dbuf<float> fd(static_cast<size_t>(n_flagged) * k, s);
+  answer(rows.data(), n_flagged, fi.data(), fd.data());
+  copy_rows(s, fi.data(), nullptr, out_idx, rows.data(), n_flagged, k);
+  copy_rows(s, fd.data(), nullptr, out_dist, rows.data(), n_flagged, k);
+  B2_CUDA(cudaStreamSynchronize(s));  // hrows is host memory read by the copy above
 }
 
 void postprocess_distances(cudaStream_t stream, float* dist, int64_t count, cuvsDistanceType metric)

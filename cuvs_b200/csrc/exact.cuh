@@ -7,6 +7,7 @@
 #pragma once
 #include <cuda_runtime.h>
 #include <cstdint>
+#include <functional>
 
 #include <cuvs/distance/distance.h>
 
@@ -38,31 +39,28 @@ void exact_distance_tile(cudaStream_t stream, const float* q, int64_t nq, int64_
                          int64_t ldx, int d, const float* qn, const float* xn, cuvsDistanceType metric, float* out,
                          int64_t ldo, filter_view filt, int64_t q_row0);
 
-/** How a raw scan score s of the tensor-core engine maps to the metric's selection form, and the
- *  error budget of that approximation:  A = sa*s + sb*|q|^2 + sc,  eps = eps_rel * (eq*|q|^2 + ec). */
-struct approx_map {
-  float sa = 1.f, sb = 0.f, sc = 0.f;
-  float eps_rel = 0.f, eq = 0.f, ec = 0.f;
-};
-
 /**
  * Re-score candidates exactly and keep the best k per query.
  *   cand_pos [nq, kc]  uint32 row positions into x (0xffffffff = empty slot)
  *   src_ids            optional int64 map position -> source id (null: identity)
  * Output rows are sorted best-first, ties towards the smaller *source id*; missing entries get
- * id `pad_id` and +/-FLT_MAX.  When `cand_score` (approximate selection-form scores of the
- * candidates = raw engine scores mapped through `amap`, same layout, sorted or not) and `flags` are given, flags[i] is set to 1 unless the
- * k-th exact distance is strictly better than (worst candidate approx score -/+ eps_i), where
- * eps_i comes from `amap` (for L2: eps_rel * (|q_i|^2 + max_j |x_j|^2)): the certificate that no non-candidate can
- * belong to the exact top-k (DESIGN.md §3).
- * kc <= 256 runs one warp per query; 256 < kc <= 2048 (no certificate: cand_score and flags null, k <= kc) one CTA per
- * query with the same arithmetic and ranking.
+ * id `pad_id` and +/-FLT_MAX.  kc <= 256 runs one warp per query; 256 < kc <= 2048 (k <= kc) one CTA per query with the
+ * same arithmetic and ranking.
  */
 void rescore_topk(cudaStream_t stream, const float* q, int64_t nq, int64_t ldq, const float* x, int64_t ldx, int d,
-                  const float* qn, const float* xn, cuvsDistanceType metric, const uint32_t* cand_pos,
-                  const float* cand_score, int kc, const int64_t* src_ids, int k, int64_t* out_idx, float* out_dist,
-                  int64_t pad_id, const struct approx_map& amap, int* flags, int* n_flagged,
-                  const float* approx_floor = nullptr /* [nq] raw engine score no row outside the candidates can beat */);
+                  const float* qn, const float* xn, cuvsDistanceType metric, const uint32_t* cand_pos, int kc,
+                  const int64_t* src_ids, int k, int64_t* out_idx, float* out_dist, int64_t pad_id);
+
+/** dst[dst_rows[i]] = src[src_rows[i]] for n rows of `width` elements (a null row map is the identity).  T: float, int64_t,
+ *  uint32_t. */
+template <typename T>
+void copy_rows(cudaStream_t s, const T* src, const int64_t* src_rows, T* dst, const int64_t* dst_rows, int64_t n, int64_t width);
+
+/** The exact fallback of a certified search: flags [nq + 1] (device) marks the queries a certificate rejected and flags[nq]
+ *  counts them (recorded by set_last_flagged).  answer(rows, n, idx, dist) writes the k results of the n flagged rows (device,
+ *  ascending) to idx / dist [n, k], which replace those rows of out_idx / out_dist [nq, k].  Synchronises the stream. */
+void rerun_flagged(cudaStream_t s, const int* flags, int64_t nq, int k, int64_t* out_idx, float* out_dist,
+                   const std::function<void(const int64_t* rows, int64_t n, int64_t* idx, float* dist)>& answer);
 
 /** In-place sqrt (L2Sqrt*) or sign/offset fix-ups applied after selection. */
 void postprocess_distances(cudaStream_t stream, float* dist, int64_t count, cuvsDistanceType metric);

@@ -22,6 +22,7 @@
 //      oracle's answer over its probed lists.
 #include "common.hpp"
 #include "exact.cuh"
+#include "exact_device.cuh"
 #include "ivf_common.cuh"
 #include "ivf_lists.cuh"
 #include "npy_io.hpp"
@@ -74,6 +75,8 @@ const float* residual_centers(const ivf_flat_index& idx)
 }
 // The metric the scan ranks by: cosine ranks as L2 over unit vectors.
 cuvsDistanceType scan_metric(const ivf_flat_index& idx) { return idx.metric == CosineExpanded ? L2Expanded : idx.metric; }
+// The metric the exact re-score computes: the reference's fine-scan arithmetic, sum (q - x)^2, for every L2 metric.
+cuvsDistanceType fine_metric(const ivf_flat_index& idx) { return is_ip(idx.metric) ? idx.metric : L2Unexpanded; }
 
 // One warp per list row: hi = bf16(x * scale - c_l) and rn = |x * scale - c_l|^2 (fp32), with l the row's list (the last with
 // offsets[l] <= row) and scale = row_scale[row] (null: 1).  Padding rows get a zero residual.
@@ -228,28 +231,16 @@ __global__ void certify_kernel(const float* __restrict__ out_dist, int k, int fi
   if (flag) atomicAdd(flags + nq, 1);
 }
 
-// The exact distance of row r to the query row qr with rescore_topk's arithmetic (exact.cu: fmaf over ascending components,
-// the `fine` metric), negated for inner product so that smaller is better.
-__device__ __forceinline__ float exact_key(const float* __restrict__ qr, const float* __restrict__ xr, int dim, float qn, float xn, int fine)
-{
-  float acc = 0.f;
-  if (fine == L2Unexpanded) {
-    for (int j = 0; j < dim; ++j) { const float t = qr[j] - xr[j]; acc = fmaf(t, t, acc); }
-  } else {
-    for (int j = 0; j < dim; ++j) acc = fmaf(qr[j], xr[j], acc);
-  }
-  return fine == InnerProduct ? -acc : (fine == CosineExpanded ? 1.0f - acc / (sqrtf(qn) * sqrtf(xn)) : acc);
-}
-
 __device__ __forceinline__ bool row_kept(int64_t id, const uint32_t* __restrict__ keep_bits, int64_t n_bits)
 {
   return id != kPadId && (keep_bits == nullptr || (id >= 0 && id < n_bits && ((keep_bits[id >> 5] >> (id & 31)) & 1u)));
 }
 
 // k <= 64: the exact fallback on the device, the CTAs taking the queries in turn; they pass over a query the certificate
-// accepted, so the search needs no host round trip.  A flagged query scores every row of its probed lists with exact_key.  Rows better than the running
-// k-th best (distance, id) collect in shared memory, which is sorted and cut back to k whenever it may overflow; the k best by
-// (distance, id), rescore_topk's ranking, overwrite the query's output row (selection form; missing: pad id and +-FLT_MAX).
+// accepted, so the search needs no host round trip.  A flagged query scores every row of its probed lists exactly, negated for
+// inner product so that smaller is better.  Rows better than the running k-th best (distance, id) collect in shared memory,
+// which is sorted and cut back to k whenever it may overflow; the k best by (distance, id), rescore_topk's ranking, overwrite
+// the query's output row (selection form; missing: pad id and +-FLT_MAX).
 constexpr int kFbThreads = 256, kFbCap = 1024;
 __global__ void __launch_bounds__(kFbThreads)
 exact_fallback_kernel(const int* __restrict__ flags, const uint32_t* __restrict__ probes, int n_probes, const int64_t* __restrict__ offsets,
@@ -267,20 +258,7 @@ exact_fallback_kernel(const int* __restrict__ flags, const uint32_t* __restrict_
     const int n = cnt;
     for (int i = n + threadIdx.x; i < kFbCap; i += kFbThreads) { sd[i] = INFINITY; si[i] = INT64_MAX; }
     __syncthreads();
-    for (int size = 2; size <= kFbCap; size <<= 1) {
-      for (int stride = size >> 1; stride > 0; stride >>= 1) {
-        for (int i = threadIdx.x; i < kFbCap / 2; i += kFbThreads) {
-          const int lo = (i / stride) * stride * 2 + (i % stride), hi = lo + stride;
-          const bool up = (lo & size) == 0;
-          const bool hi_first = sd[hi] < sd[lo] || (sd[hi] == sd[lo] && si[hi] < si[lo]);
-          if (hi_first == up) {
-            const float td = sd[lo]; sd[lo] = sd[hi]; sd[hi] = td;
-            const int64_t ti = si[lo]; si[lo] = si[hi]; si[hi] = ti;
-          }
-        }
-        __syncthreads();
-      }
-    }
+    block_bitonic_sort(sd, si, nullptr, kFbCap, [&](int a, int b) { return sd[a] < sd[b] || (sd[a] == sd[b] && si[a] < si[b]); });
     if (threadIdx.x == 0) {
       cnt = min(n, k);
       if (n >= k) { thr_d = sd[k - 1]; thr_i = si[k - 1]; }
@@ -302,7 +280,9 @@ exact_fallback_kernel(const int* __restrict__ flags, const uint32_t* __restrict_
         if (r < r1) {
           const int64_t id = ids[r];
           if (row_kept(id, keep_bits, n_bits)) {
-            const float d = exact_key(qr, x + r * dim, dim, qn[qi], xn[r], fine);
+            // scalar reads: the float4 form makes this kernel spill, and both give the same bits
+            const float e = finish_distance(exact_accumulate(qr, x + r * dim, dim, false, fine), qn[qi], xn[r], fine);
+            const float d = ip ? -e : e;
             if (d < thr_d || (d == thr_d && id < thr_i)) {
               const int at = atomicAdd(&cnt, 1);
               sd[at] = d;
@@ -325,9 +305,9 @@ exact_fallback_kernel(const int* __restrict__ flags, const uint32_t* __restrict_
   }
 }
 
-// k > 64: the exact fallback's scan.  The score of every (pair, list row) is the row's exact_key, so the segmented select keeps
-// each pair's k best by the very value the re-score recomputes.  Padding rows and rows the bitset hides
-// score +inf.  One CTA per live pair slot, one thread per row.
+// k > 64: the exact fallback's scan.  The score of every (pair, list row) is the row's exact distance (negated for inner
+// product), so the segmented select keeps each pair's k best by the very value the re-score recomputes.  Padding rows and rows
+// the bitset hides score +inf.  One CTA per live pair slot, one thread per row.
 __global__ void exact_segments_kernel(const float* __restrict__ q, int dim, const float* __restrict__ x, const float* __restrict__ qn,
                                       const float* __restrict__ xn, const int64_t* __restrict__ ids, int fine,
                                       const uint32_t* __restrict__ pair_query, const uint32_t* __restrict__ pair_list,
@@ -341,8 +321,12 @@ __global__ void exact_segments_kernel(const float* __restrict__ q, int dim, cons
   const uint32_t l = pair_list[slot];
   const float* qr  = q + qi * dim;
   float* out       = scores + seg_off[slot];
-  for (int64_t r = offsets[l] + threadIdx.x; r < offsets[l + 1]; r += blockDim.x)
-    out[r - offsets[l]] = row_kept(ids[r], keep_bits, n_bits) ? exact_key(qr, x + r * dim, dim, qn[qi], xn[r], fine) : INFINITY;
+  const bool vec4  = exact_vec4(q, dim, x, dim, dim);
+  for (int64_t r = offsets[l] + threadIdx.x; r < offsets[l + 1]; r += blockDim.x) {
+    if (!row_kept(ids[r], keep_bits, n_bits)) { out[r - offsets[l]] = INFINITY; continue; }
+    const float v = finish_distance(exact_accumulate(qr, x + r * dim, dim, vec4, fine), qn[qi], xn[r], fine);
+    out[r - offsets[l]] = fine == InnerProduct ? -v : v;
+  }
 }
 
 // cuvsB200IvfFlatCandidates: per merged candidate (q, c) at index row pos, its source id (INT64_MAX for an empty slot) and the
@@ -374,26 +358,6 @@ __global__ void candidate_budget_kernel(const uint32_t* __restrict__ pos, const 
     }
   }
   bound[i] = eps;
-}
-
-// dst[dst_row(i)] = src[src_row(i)] for rows of `width` elements; a null row map is the identity
-template <typename T>
-__global__ void copy_rows_kernel(const T* __restrict__ src, const int64_t* __restrict__ src_rows, T* __restrict__ dst,
-                                 const int64_t* __restrict__ dst_rows, int64_t n, int64_t width)
-{
-  int64_t t = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x;
-  if (t >= n * width) return;
-  const int64_t i = t / width, j = t % width;
-  dst[(dst_rows ? dst_rows[i] : i) * width + j] = src[(src_rows ? src_rows[i] : i) * width + j];
-}
-
-template <typename T>
-void copy_rows(cudaStream_t s, const T* src, const int64_t* src_rows, T* dst, const int64_t* dst_rows, int64_t n, int64_t width)
-{
-  if (n == 0) return;
-  count_launch();
-  copy_rows_kernel<T><<<blocks_for(n * width, 256), 256, 0, s>>>(src, src_rows, dst, dst_rows, n, width);
-  B2_CUDA(cudaGetLastError());
 }
 
 // The scan's side of the list rows (DESIGN.md §4): bf16 residuals against the row's list centre and their half norms.  Rebuilt
@@ -511,10 +475,46 @@ struct flat_candidates {
   float* bound;  // [nq, kc2] error budget of each candidate's own pair
 };
 
-// exact: score every row of the probed lists exactly (the fallback of the queries the certificate flags).  dump: stop after
-// the certificate and copy its inputs out (one query batch).
+// k > 64: the exact fallback.  The k > 64 steps with exact scores over the lists the nq queries q probe (probes [nq, n_probes],
+// the search's own: its coarse selection is exact per query), written postprocessed to out_idx / out_dist [nq, k].  A query's
+// workspace here (kc = k) is no larger than in the search (kc = min(2k, 2048)), so the flagged queries of a batch fit its budget.
+void exact_probed_search(resources* res, const ivf_flat_index& idx, const float* q, int64_t nq, const uint32_t* probes,
+                         uint32_t n_probes, const uint32_t* keep_bits, int64_t n_bits, int k, int64_t* out_idx, float* out_dist)
+{
+  auto s                     = res->stream;
+  const cuvsDistanceType fine = fine_metric(idx);
+  dbuf<float> qn(static_cast<size_t>(nq), s);
+  row_norms(s, q, nq, idx.dim, idx.dim, qn.data());
+  probe_buckets pb;
+  bucket_probes(res, probes, nq, static_cast<int>(n_probes), idx.n_lists, idx.lists.d_offsets.data(), 0, pb);
+  dbuf<float> cs;
+  dbuf<uint32_t> cp;
+  large_k_select(s, pb, idx.lists, nq, n_probes, k, [&](float* scores, const int64_t* seg_off) {
+    count_launch();
+    exact_segments_kernel<<<static_cast<unsigned>(std::max<int64_t>(pb.n_pairs, 1)), 128, 0, s>>>(
+      q, idx.dim, idx.data.data(), qn.data(), idx.xn.data(), idx.ids.data(), int(fine), pb.pair_query.data(), pb.pair_list.data(),
+      pb.n_items.data() + 1, idx.lists.d_offsets.data(), seg_off, keep_bits, n_bits, scores);
+    B2_CUDA(cudaGetLastError());
+  }, cs, cp);
+  const int64_t cand_w = static_cast<int64_t>(n_probes) * k;
+  dbuf<float> gs(static_cast<size_t>(nq) * cand_w, s);
+  dbuf<uint32_t> gp(static_cast<size_t>(nq) * cand_w, s);
+  gather_probe_candidates(s, cs.data(), cp.data(), pb.slot_of.data(), nullptr, 1.f, INFINITY, nq, static_cast<int>(n_probes), k,
+                          gs.data(), gp.data());
+  dbuf<float> ms(static_cast<size_t>(nq) * k, s);
+  dbuf<uint32_t> mp(static_cast<size_t>(nq) * k, s);
+  select_k(s, gs.data(), gp.data(), IDX_U32, nq, cand_w, cand_w, k, ms.data(), mp.data(), IDX_U32, true);
+  count_launch();
+  drop_nonfinite_kernel<<<blocks_for(nq * k, 256), 256, 0, s>>>(ms.data(), mp.data(), nq * k);
+  B2_CUDA(cudaGetLastError());
+  rescore_topk(s, q, nq, idx.dim, idx.data.data(), idx.dim, idx.dim, qn.data(), idx.xn.data(), fine, mp.data(), k, idx.ids.data(), k,
+               out_idx, out_dist, INT64_MAX);
+  postprocess_distances(s, out_dist, nq * k, idx.metric);
+}
+
+// dump: stop after the certificate and copy its inputs out (one query batch).
 void ivf_flat_search(resources* res, const ivf_flat_index& idx, uint32_t n_probes, const DLTensor& qt, const DLTensor& nt,
-                     const DLTensor& dt, const uint32_t* keep_bits = nullptr, int64_t n_bits = 0, bool exact = false,
+                     const DLTensor& dt, const uint32_t* keep_bits = nullptr, int64_t n_bits = 0,
                      const flat_candidates* dump = nullptr)
 {
   auto s           = res->stream;
@@ -527,9 +527,8 @@ void ivf_flat_search(resources* res, const ivf_flat_index& idx, uint32_t n_probe
   if (nq == 0) return;
   n_probes         = std::min<uint32_t>(n_probes, idx.n_lists);
   // k > 64 (DESIGN.md §4 "k > 64"): the scan stores every (pair, list row) score and a segmented select keeps kc2 per pair.
-  // The exact fallback takes the same steps with exact scores, of which each pair needs only its k best.
-  const bool large_k = k > 64 || exact;
-  const int large_kc = exact ? k : std::min(2 * k, kSelectMaxK);
+  const bool large_k = k > 64;
+  const int large_kc = std::min(2 * k, kSelectMaxK);
   // Query batching.  Per (query, probe) pair: the bf16 query residual row and its offset, 2 x KC candidate slots and their
   // per-query concatenation.  k > 64, per query: dense scores (bounded by its n_probes largest lists), each pair's kc2 best and their
   // per-query gather (8 + 8 bytes each), the gathered bf16 query rows, slot bookkeeping (32 bytes per pair) and the merged kc2.
@@ -540,7 +539,7 @@ void ivf_flat_search(resources* res, const ivf_flat_index& idx, uint32_t n_probe
   const int64_t batch = query_batch_size(idx.Kp * 2 + 4 + 2 * 64 * 8 + 16, n_probes, large_k_bytes, "CUVS_B200_FLAT_LARGE_K_BUDGET_MB");
   B2_EXPECTS(dump == nullptr || nq <= batch, "ivf_flat candidates: %lld queries do not fit one batch", (long long)nq);
   if (search_in_batches(batch, qt, nt, dt, [&](const DLTensor& qs, const DLTensor& ns, const DLTensor& ds) {
-        ivf_flat_search(res, idx, n_probes, qs, ns, ds, keep_bits, n_bits, exact);
+        ivf_flat_search(res, idx, n_probes, qs, ns, ds, keep_bits, n_bits);
       }))
     return;
   const float* q   = dl_ptr<float>(qt);
@@ -564,7 +563,7 @@ void ivf_flat_search(resources* res, const ivf_flat_index& idx, uint32_t n_probe
   // fallback reads the bitset itself)
   dbuf<__nv_bfloat16> hx_f;
   const __nv_bfloat16* hx = idx.hx.data();
-  if (keep_bits != nullptr && idx.lists.rows_total > 0 && !exact) {
+  if (keep_bits != nullptr && idx.lists.rows_total > 0) {
     const int64_t R = idx.lists.rows_total;
     dbuf<float> hn(static_cast<size_t>(R), s);
     hx_f.alloc(static_cast<size_t>(std::max<int64_t>(R, 128)) * 16, s);
@@ -587,14 +586,14 @@ void ivf_flat_search(resources* res, const ivf_flat_index& idx, uint32_t n_probe
   int KCW         = KC * kTcListsPerItem;
   probe_buckets pb;
   bucket_probes(res, probes.data(), nq, static_cast<int>(n_probes), idx.n_lists, idx.lists.d_offsets.data(), KCW, pb);
-  cuvsDistanceType fine = idx.metric == InnerProduct ? InnerProduct : (idx.metric == CosineExpanded ? CosineExpanded : L2Unexpanded);
+  const cuvsDistanceType fine = fine_metric(idx);
 
   // ---- 3. fine scan: per-pair query residuals (A) x list residuals (B).  Scores of different pairs compare as distances,
   // add[slot] + scale * score (pair_residual_rows); cosine scores the unit query as L2 (scan_metric).
   residual_rows a;
   dbuf<float> add;
   float scale = 1.f;
-  if (!exact) {
+  {
     const float* qf = q;
     dbuf<float> q_unit;
     if (idx.metric == CosineExpanded) {
@@ -607,16 +606,7 @@ void ivf_flat_search(resources* res, const ivf_flat_index& idx, uint32_t n_probe
   }
   dbuf<float> cs;
   dbuf<uint32_t> cp;
-  if (exact) {
-    large_k_select(s, pb, idx.lists, nq, n_probes, large_kc, [&](float* scores, const int64_t* seg_off) {
-      count_launch();
-      exact_segments_kernel<<<static_cast<unsigned>(std::max<int64_t>(pb.n_pairs, 1)), 128, 0, s>>>(
-        q, idx.dim, idx.data.data(), qn.data(), idx.xn.data(), idx.ids.data(), int(fine), pb.pair_query.data(), pb.pair_list.data(),
-        pb.n_items.data() + 1, idx.lists.d_offsets.data(), seg_off, keep_bits, n_bits, scores);
-      B2_CUDA(cudaGetLastError());
-    }, cs, cp);
-    KCW = large_kc;
-  } else if (large_k) {
+  if (large_k) {
     // every (pair, list row) score goes to the pair's dense segment; each pair keeps its kc2 best rows
     large_k_select(s, pb, idx.lists, nq, n_probes, large_kc, [&](float* scores, const int64_t* seg_off) {
       item_segments(s, pb, seg_off);
@@ -647,9 +637,8 @@ void ivf_flat_search(resources* res, const ivf_flat_index& idx, uint32_t n_probe
   dbuf<uint32_t> gp(static_cast<size_t>(nq) * cand_w, s);
   // empty entries +inf: FLT_MAX made the ivf_flat bench search ~3 % slower (DESIGN.md §4a)
   const int L = large_k ? KCW : KC;  // entries of one per-pair list
-  dbuf<float> last;
-  if (!exact) last.alloc(static_cast<size_t>(nq * cand_w / L), s);
-  gather_probe_candidates(s, cs.data(), cp.data(), pb.slot_of.data(), exact ? nullptr : add.data(), scale, INFINITY, nq,
+  dbuf<float> last(static_cast<size_t>(nq * cand_w / L), s);
+  gather_probe_candidates(s, cs.data(), cp.data(), pb.slot_of.data(), add.data(), scale, INFINITY, nq,
                           static_cast<int>(n_probes), KCW, gs.data(), gp.data(), L, last.data());
   const int kc2 = static_cast<int>(std::min<int64_t>(cand_w, large_k ? large_kc : std::max(32, 2 * k)));
   dbuf<float> ms(static_cast<size_t>(nq) * kc2, s);
@@ -662,12 +651,8 @@ void ivf_flat_search(resources* res, const ivf_flat_index& idx, uint32_t n_probe
     drop_nonfinite_kernel<<<blocks_for(nq * kc2, 256), 256, 0, s>>>(ms.data(), mp.data(), nq * kc2);
     B2_CUDA(cudaGetLastError());
   }
-  rescore_topk(s, q, nq, idx.dim, idx.data.data(), idx.dim, idx.dim, qn.data(), idx.xn.data(), fine, mp.data(), nullptr, kc2,
-               idx.ids.data(), k, out_idx, out_dist, INT64_MAX, approx_map{}, nullptr, nullptr);
-  if (exact) {
-    postprocess_distances(s, out_dist, nq * k, idx.metric);
-    return;
-  }
+  rescore_topk(s, q, nq, idx.dim, idx.data.data(), idx.dim, idx.dim, qn.data(), idx.xn.data(), fine, mp.data(), kc2,
+               idx.ids.data(), k, out_idx, out_dist, INT64_MAX);
 
   // ---- 5. certificate (certify_kernel): the queries whose k-th exact distance is not safely below every row the bf16
   // candidates left out are searched again with exact scores and their rows written back
@@ -700,33 +685,15 @@ void ivf_flat_search(resources* res, const ivf_flat_index& idx, uint32_t n_probe
     set_last_flagged_async(flags.data() + nq, s);
     return;
   }
-  // k > 64: the flagged queries are gathered and searched again with exact scores (exact_segments_kernel)
+  // k > 64: the flagged queries are answered again by exact_probed_search over the lists they probed
   postprocess_distances(s, out_dist, nq * k, idx.metric);
-  int n_flagged = 0;
-  B2_CUDA(cudaMemcpyAsync(&n_flagged, flags.data() + nq, sizeof(int), cudaMemcpyDeviceToHost, s));
-  B2_CUDA(cudaStreamSynchronize(s));
-  set_last_flagged(n_flagged);
-  if (n_flagged == 0) return;
-  std::vector<int> hflags(static_cast<size_t>(nq));
-  B2_CUDA(cudaMemcpyAsync(hflags.data(), flags.data(), sizeof(int) * nq, cudaMemcpyDeviceToHost, s));
-  B2_CUDA(cudaStreamSynchronize(s));
-  std::vector<int64_t> hrows;
-  hrows.reserve(static_cast<size_t>(n_flagged));
-  for (int64_t i = 0; i < nq; ++i)
-    if (hflags[i]) hrows.push_back(i);
-  dbuf<int64_t> rows(static_cast<size_t>(n_flagged), s);
-  B2_CUDA(cudaMemcpyAsync(rows.data(), hrows.data(), sizeof(int64_t) * n_flagged, cudaMemcpyHostToDevice, s));
-  dbuf<float> fq(static_cast<size_t>(n_flagged) * idx.dim, s), fd(static_cast<size_t>(n_flagged) * k, s);
-  dbuf<int64_t> fi(static_cast<size_t>(n_flagged) * k, s);
-  copy_rows(s, q, rows.data(), fq.data(), nullptr, n_flagged, idx.dim);
-  dl_row_slice sq(qt, 0, n_flagged), si(nt, 0, n_flagged), sd(dt, 0, n_flagged);
-  sq.t.data = fq.data();
-  si.t.data = fi.data();
-  sd.t.data = fd.data();
-  ivf_flat_search(res, idx, n_probes, sq.t, si.t, sd.t, keep_bits, n_bits, true);
-  copy_rows(s, fi.data(), nullptr, out_idx, rows.data(), n_flagged, k);
-  copy_rows(s, fd.data(), nullptr, out_dist, rows.data(), n_flagged, k);
-  B2_CUDA(cudaStreamSynchronize(s));  // hrows is host memory read by the copy above
+  rerun_flagged(s, flags.data(), nq, k, out_idx, out_dist, [&](const int64_t* rows, int64_t n, int64_t* fi, float* fd) {
+    dbuf<float> fq(static_cast<size_t>(n) * idx.dim, s);
+    dbuf<uint32_t> fp(static_cast<size_t>(n) * n_probes, s);
+    copy_rows(s, q, rows, fq.data(), nullptr, n, idx.dim);
+    copy_rows(s, probes.data(), rows, fp.data(), nullptr, n, int64_t(n_probes));
+    exact_probed_search(res, idx, fq.data(), n, fp.data(), n_probes, keep_bits, n_bits, k, fi, fd);
+  });
 }
 
 }  // namespace
@@ -853,7 +820,7 @@ cuvsError_t cuvsB200IvfFlatCandidates(cuvsResources_t res, cuvsIvfFlatIndex_t in
     nt.data = ni.data(); nt.device = q.device; nt.ndim = 2; nt.dtype = DLDataType{kDLInt, 64, 1}; nt.shape = shape;
     dt.data = nd.data(); dt.device = q.device; dt.ndim = 2; dt.dtype = DLDataType{kDLFloat, 32, 1}; dt.shape = shape;
     flat_candidates c{dl_ptr<int64_t>(ci), dl_ptr<float>(cd), dl_ptr<float>(b)};
-    ivf_flat_search(r, idx, n_probes, q, nt, dt, nullptr, 0, false, &c);
+    ivf_flat_search(r, idx, n_probes, q, nt, dt, nullptr, 0, &c);
   });
 }
 

@@ -68,7 +68,7 @@ extern "C" cuvsError_t cuvsRefine(cuvsResources_t res, DLManagedTensor* dataset_
     }
     timed_section ts("refine", s);
     rescore_topk(s, dl_ptr<float>(q), nq, d, dl_ptr<float>(ds), d, d, need_norms ? qn.data() : nullptr, need_norms ? xn.data() : nullptr,
-                 fine, pos.data(), nullptr, n_cand, nullptr, k, dl_ptr<int64_t>(oi), dl_ptr<float>(od), -1, approx_map{}, nullptr, nullptr);
+                 fine, pos.data(), n_cand, nullptr, k, dl_ptr<int64_t>(oi), dl_ptr<float>(od), -1);
     postprocess_distances(s, dl_ptr<float>(od), nq * k, fine);
   });
 }
