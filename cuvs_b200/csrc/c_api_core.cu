@@ -22,6 +22,18 @@ __global__ void widen_kernel(const T* __restrict__ in, int64_t n, float* __restr
   if (i < n) out[i] = static_cast<float>(in[i]);
 }
 
+void widen_async(cudaStream_t s, const void* in, DLDataType dt, int64_t count, float* out)
+{
+  if (count == 0) return;
+  const unsigned grid = static_cast<unsigned>((count + 255) / 256);
+  count_launch();
+  if (dt.code == kDLFloat && dt.bits == 16) widen_kernel<__half><<<grid, 256, 0, s>>>(static_cast<const __half*>(in), count, out);
+  else if (dt.code == kDLInt && dt.bits == 8) widen_kernel<int8_t><<<grid, 256, 0, s>>>(static_cast<const int8_t*>(in), count, out);
+  else if (dt.code == kDLUInt && dt.bits == 8) widen_kernel<uint8_t><<<grid, 256, 0, s>>>(static_cast<const uint8_t*>(in), count, out);
+  else B2_FAIL("widen_async: unsupported dtype code %d bits %d", int(dt.code), int(dt.bits));
+  B2_CUDA(cudaGetLastError());
+}
+
 void widen_to_f32(resources* res, const DLTensor& src, f32_matrix& out)
 {
   B2_EXPECTS(src.ndim == 2 && dl_is_c_contiguous(src), "matrix must be a row-major 2-D tensor");
@@ -45,14 +57,7 @@ void widen_to_f32(resources* res, const DLTensor& src, f32_matrix& out)
     B2_CUDA(cudaMemcpyAsync(stage.data(), in, static_cast<size_t>(count) * esize, cudaMemcpyHostToDevice, s));
     in = stage.data();
   }
-  if (count) {
-    const unsigned grid = static_cast<unsigned>((count + 255) / 256);
-    count_launch();
-    if (dl_is(src, kDLFloat, 16)) widen_kernel<__half><<<grid, 256, 0, s>>>(static_cast<const __half*>(in), count, out.own.data());
-    else if (dl_is(src, kDLInt, 8)) widen_kernel<int8_t><<<grid, 256, 0, s>>>(static_cast<const int8_t*>(in), count, out.own.data());
-    else widen_kernel<uint8_t><<<grid, 256, 0, s>>>(static_cast<const uint8_t*>(in), count, out.own.data());
-    B2_CUDA(cudaGetLastError());
-  }
+  widen_async(s, in, src.dtype, count, out.own.data());
   out.t.data        = out.own.data();
   out.t.byte_offset = 0;
   out.t.dtype       = DLDataType{kDLFloat, 32, 1};

@@ -239,6 +239,8 @@ inline bool dl_is_dataset_dtype(const DLTensor& t)
   return dl_is(t, kDLFloat, 32) || dl_is(t, kDLFloat, 16) || dl_is(t, kDLInt, 8) || dl_is(t, kDLUInt, 8);
 }
 void widen_to_f32(struct resources* res, const DLTensor& src, f32_matrix& out);
+/** out[i] = float(in[i]) for `count` device elements of type `dt` (float16, int8 or uint8), stream-ordered. */
+void widen_async(cudaStream_t s, const void* in, DLDataType dt, int64_t count, float* out);
 
 /** Fill a caller-provided DLManagedTensor as a non-owning row-major view (used by index getters). */
 void dl_fill_view(DLManagedTensor* out, void* data, int device, DLDataType dt, int ndim, const int64_t* shape);

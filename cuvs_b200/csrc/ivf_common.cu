@@ -873,8 +873,16 @@ dbuf<float> train_subsample(cudaStream_t s, const DLTensor& ds, uint32_t n_lists
   const int64_t stride = std::max<int64_t>(1, n / n_train);
   n_train = std::min(n_train, (n + stride - 1) / stride);
   dbuf<float> train(static_cast<size_t>(n_train) * d, s);
-  B2_CUDA(cudaMemcpy2DAsync(train.data(), sizeof(float) * d, dl_ptr<float>(ds), sizeof(float) * d * stride, sizeof(float) * d, n_train,
-                            cudaMemcpyDefault, s));
+  if (dl_is(ds, kDLFloat, 32)) {
+    B2_CUDA(cudaMemcpy2DAsync(train.data(), sizeof(float) * d, dl_ptr<float>(ds), sizeof(float) * d * stride, sizeof(float) * d, n_train,
+                              cudaMemcpyDefault, s));
+    return train;
+  }
+  // a narrower type: only the sample is widened
+  const size_t row = static_cast<size_t>(d) * (ds.dtype.bits / 8);
+  dbuf<uint8_t> raw(static_cast<size_t>(n_train) * row, s);
+  B2_CUDA(cudaMemcpy2DAsync(raw.data(), row, dl_ptr<uint8_t>(ds), row * stride, row, n_train, cudaMemcpyDefault, s));
+  widen_async(s, raw.data(), ds.dtype, n_train * d, train.data());
   return train;
 }
 

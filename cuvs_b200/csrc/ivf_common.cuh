@@ -135,7 +135,8 @@ void item_segments(cudaStream_t s, probe_buckets& pb, const int64_t* seg_off);
 int64_t large_k_rows_per_query(const list_layout& lists, uint32_t n_probes);
 
 /**
- * Training rows of an IVF build: an evenly strided subsample of the rows of `ds` (fp32 [n, d], device or host), every
+ * Training rows of an IVF build: an evenly strided subsample of the rows of `ds` ([n, d], device or host; float16, int8 and
+ * uint8 rows are widened after sampling), every
  * stride-th row from row 0.  About fraction x n rows (fraction clamped to [0, 1]), at least n_lists, at most
  * max(n_lists x 1024, 2^18) (ivf_flat_build.cuh:430-455 uses the same rule).  n_train receives the row count.
  */

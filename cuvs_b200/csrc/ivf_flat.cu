@@ -20,6 +20,9 @@
 //   5. certificate: a query whose k-th exact distance is not safely below every row the candidates left out (the bf16 score's
 //      error budget) is searched again with every row of its probed lists scored exactly, so every query returns the
 //      oracle's answer over its probed lists.
+// int8 / uint8 indexes in L2 or inner product keep their rows as bytes and scan them on the integer tensor cores, whose scores
+// are exact: steps 3-4 rank by exact integer keys and need no re-score or certificate (ivf_flat_search_i8, DESIGN.md §4
+// "Row types").
 #include "common.hpp"
 #include "exact.cuh"
 #include "exact_device.cuh"
@@ -32,9 +35,12 @@
 #include <cuvs/neighbors/ivf_flat.h>
 #include <cuvs_b200/ext.h>
 
+#include <cuda_fp16.h>
+
 #include <algorithm>
 #include <cfloat>
 #include <cmath>
+#include <cstring>
 #include <fstream>
 #include <memory>
 #include <vector>
@@ -64,9 +70,152 @@ struct ivf_flat_index {
   owned<float> rn_max;       // [n_lists] max |x - c|^2 over the list's rows (the certificate's error budget)
   owned<float> cn;           // [n_lists] |c|^2 of the fp32 centres (the inner-product budget)
   int Kp = 0;
+  // 8-bit lists (row_type kRowS8 / kRowU8; DESIGN.md §4 "Row types"): data, hi, hx, xn, rn and rn_max stay empty
+  int row_type = 0;
+  owned<uint8_t> rows8;      // [rows_total, Kp8] the rows' bytes, zero padding rows and columns
+  owned<int> norms8;         // [rows_total] exact |x|^2, kI8PadNorm on padding rows
+  int Kp8 = 0;
 };
 
 namespace {
+
+// How an index stores its list rows: fp32 (float32 and float16 datasets, and cosine on 8-bit ones), or the 8-bit rows themselves.
+constexpr int kRowF32 = 0, kRowS8 = 1, kRowU8 = 2;
+int row_type_for(DLDataType t, cuvsDistanceType metric)
+{
+  if (metric == CosineExpanded || t.bits != 8) return kRowF32;  // a cosine distance is no integer function of the rows
+  return t.code == kDLInt ? kRowS8 : kRowU8;
+}
+
+// 8-bit rows from a widened chunk x (integer values as fp32): one thread per byte of a padded row, written to row dst_rows[r]
+__global__ void narrow_rows_kernel(const float* __restrict__ x, int64_t n, int dim, int Kp8, const int64_t* __restrict__ dst_rows,
+                                   uint8_t* __restrict__ out)
+{
+  const int64_t t = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x;
+  if (t >= n * Kp8) return;
+  const int64_t r = t / Kp8;
+  const int j     = static_cast<int>(t % Kp8);
+  const int64_t o = dst_rows[r];
+  if (o < 0) return;
+  out[o * Kp8 + j] = j < dim ? static_cast<uint8_t>(static_cast<int>(x[r * dim + j])) : uint8_t(0);
+}
+
+// norms[r] = |x_r|^2 exactly, or kI8PadNorm on padding rows and on rows the bitset (bit = 1 keeps; null: all) hides.  One warp
+// per row.
+template <bool U8>
+__global__ void i8_norms_kernel(const uint8_t* __restrict__ rows, int64_t n, int Kp8, const int64_t* __restrict__ ids,
+                                const uint32_t* __restrict__ keep_bits, int64_t n_bits, int* __restrict__ norms)
+{
+  const int64_t r = (blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x) >> 5;
+  const int lane  = threadIdx.x & 31;
+  if (r >= n) return;
+  int acc = 0;
+  for (int j = lane; j < Kp8; j += 32) {
+    const int v = U8 ? static_cast<int>(rows[r * Kp8 + j]) : static_cast<int>(static_cast<int8_t>(rows[r * Kp8 + j]));
+    acc += v * v;
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
+  if (lane != 0) return;
+  const int64_t id = ids[r];
+  const bool keep  = id != kPadId && (keep_bits == nullptr || (id >= 0 && id < n_bits && ((keep_bits[id >> 5] >> (id & 31)) & 1u)));
+  norms[r]         = keep ? acc : kI8PadNorm;
+}
+
+// The A rows of an 8-bit scan: the bytes of each pair slot's query (slots past the live pairs: zero), 16 per thread
+__global__ void pair_query_bytes_kernel(const float* __restrict__ q, int dim, int Kp8, const uint32_t* __restrict__ pair_query,
+                                        const int* __restrict__ n_live, int64_t rows, uint8_t* __restrict__ out)
+{
+  const int64_t t = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x;
+  const int w     = Kp8 / 16;
+  if (t >= rows * w) return;
+  const int64_t slot = t / w;
+  const int j0       = static_cast<int>(t % w) * 16;
+  uint32_t v[4]      = {0, 0, 0, 0};
+  if (slot < *n_live) {
+    const float* qr = q + static_cast<int64_t>(pair_query[slot]) * dim;
+#pragma unroll
+    for (int b = 0; b < 16; ++b)
+      if (j0 + b < dim) v[b >> 2] |= (static_cast<uint32_t>(static_cast<int>(qr[j0 + b])) & 0xffu) << (8 * (b & 3));
+  }
+  reinterpret_cast<uint4*>(out)[t] = make_uint4(v[0], v[1], v[2], v[3]);
+}
+
+// exact |q|^2 of a query row holding integer values; every thread of the block calls it and gets the sum
+__device__ int block_query_norm(const float* __restrict__ qr, int dim)
+{
+  __shared__ int part[32];
+  int acc = 0;
+  for (int j = threadIdx.x; j < dim; j += blockDim.x) {
+    const int v = static_cast<int>(qr[j]);
+    acc += v * v;
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
+  if ((threadIdx.x & 31) == 0) part[threadIdx.x >> 5] = acc;
+  __syncthreads();
+  int total = 0;
+  for (int w = 0; w < static_cast<int>(blockDim.x >> 5); ++w) total += part[w];
+  return total;
+}
+
+// a merged candidate that names a row: not an empty slot (FLT_MAX or +inf, position 0xffffffff) nor a row the filter hid (+inf)
+__device__ __forceinline__ bool i8_live(float key, uint32_t pos) { return pos != 0xffffffffu && __float_as_uint(key) < 0x7f000000u; }
+// the exact distance of a key's score s, rounded once: |q - x|^2 = s + |q|^2 (L2), q.x = -s (inner product)
+__device__ __forceinline__ float i8_distance(float key, int qn, bool ip)
+{
+  const int s = tc_i8_score(key);
+  return ip ? __int2float_rn(-s) : __int2float_rn(s + qn);
+}
+
+// 8-bit search, one block per query: its kc2 merged candidates (key, position), sorted by key, give the k best by (distance, id).
+// Equal keys are equal distances, so a candidate's rank is the number of candidates ahead of its run of equal keys plus the
+// members of the run with a smaller id.  Missing slots: (INT64_MAX, +-FLT_MAX).
+__global__ void i8_finish_kernel(const float* __restrict__ ms, const uint32_t* __restrict__ mp, int kc2, const int64_t* __restrict__ ids,
+                                 const float* __restrict__ q, int dim, bool ip, int k, int64_t* __restrict__ out_idx,
+                                 float* __restrict__ out_dist)
+{
+  const int64_t qi    = blockIdx.x;
+  const int qn        = block_query_norm(q + qi * dim, dim);
+  const float* key    = ms + qi * kc2;
+  const uint32_t* pos = mp + qi * kc2;
+  for (int j = threadIdx.x; j < k; j += blockDim.x) {
+    out_idx[qi * k + j]  = INT64_MAX;
+    out_dist[qi * k + j] = ip ? -FLT_MAX : FLT_MAX;
+  }
+  __syncthreads();
+  for (int j = threadIdx.x; j < kc2; j += blockDim.x) {
+    const float kj = key[j];
+    if (!i8_live(kj, pos[j])) continue;
+    const int64_t id = ids[pos[j]];
+    int lo = j;
+    while (lo > 0 && key[lo - 1] == kj) --lo;
+    int rank = lo;
+    for (int i = lo; i < kc2 && key[i] == kj && rank < k; ++i)
+      if (i != j && i8_live(key[i], pos[i]) && ids[pos[i]] < id) ++rank;
+    if (rank >= k) continue;
+    out_idx[qi * k + rank]  = id;
+    out_dist[qi * k + rank] = i8_distance(kj, qn, ip);
+  }
+}
+
+// cuvsB200IvfFlatCandidates on an 8-bit index: the kc2 merged candidates with their exact distances in the scan's units
+// (|q - x|^2, or -q.x) and, as their bound, half an ulp of that distance, the only error left being its rounding to fp32.
+__global__ void i8_candidates_kernel(const float* __restrict__ ms, const uint32_t* __restrict__ mp, int kc2, const int64_t* __restrict__ ids,
+                                     const float* __restrict__ q, int dim, bool ip, int64_t* __restrict__ out_ids,
+                                     float* __restrict__ out_dist, float* __restrict__ out_bound)
+{
+  const int64_t qi = blockIdx.x;
+  const int qn     = block_query_norm(q + qi * dim, dim);
+  for (int j = threadIdx.x; j < kc2; j += blockDim.x) {
+    const int64_t i = qi * kc2 + j;
+    const bool live = i8_live(ms[i], mp[i]);
+    const float d   = live ? i8_distance(ms[i], qn, ip) : INFINITY;
+    out_ids[i]      = live ? ids[mp[i]] : INT64_MAX;
+    out_dist[i]     = ip && live ? -d : d;
+    out_bound[i]    = live ? fmaxf(fabsf(d), 1.f) * 0x1p-24f : INFINITY;
+  }
+}
 
 // The centres the scan's residuals are taken from: the unit centres for cosine (the rows and queries are unit there too).
 const float* residual_centers(const ivf_flat_index& idx)
@@ -392,6 +541,22 @@ void refresh_tc_side(resources* res, ivf_flat_index& idx)
   tc_pack_half_norms(s, hn.data(), R, idx.hx.data());
 }
 
+// The scan's side of 8-bit list rows: their exact norms (kI8PadNorm on padding rows).  Rebuilt whenever the rows change.
+void refresh_i8_side(resources* res, ivf_flat_index& idx)
+{
+  const int64_t R = idx.lists.rows_total;
+  idx.norms8.alloc(static_cast<size_t>(std::max<int64_t>(R, 128)));
+  if (R == 0) return;
+  count_launch();
+  if (idx.row_type == kRowU8)
+    i8_norms_kernel<true><<<blocks_for(R * 32, 256), 256, 0, res->stream>>>(idx.rows8.data(), R, idx.Kp8, idx.ids.data(), nullptr, 0,
+                                                                            idx.norms8.data());
+  else
+    i8_norms_kernel<false><<<blocks_for(R * 32, 256), 256, 0, res->stream>>>(idx.rows8.data(), R, idx.Kp8, idx.ids.data(), nullptr, 0,
+                                                                             idx.norms8.data());
+  B2_CUDA(cudaGetLastError());
+}
+
 void refresh_centers_tc(resources* res, ivf_flat_index& idx)
 {
   auto s = res->stream;
@@ -409,8 +574,9 @@ void refresh_centers_tc(resources* res, ivf_flat_index& idx)
   idx.centers_tc.build(s, idx.centers.data(), idx.n_lists, idx.dim, is_l2(idx.metric) ? cn : nullptr, true, scale.data());
 }
 
-// Insert the rows of `t` (fp32 [n, dim], device or host) with ids new_ids[i] (device) or id0 + i, then refresh the derived
-// rows once.  A cosine row is labelled from its unit bf16 planes, as a cosine query is in the coarse search.
+// Insert the rows of `t` ([n, dim], device or host: fp32, or int8 / uint8 for an index of that row type) with ids new_ids[i]
+// (device) or id0 + i, then refresh the derived rows once.  A cosine row is labelled from its unit bf16 planes, as a cosine
+// query is in the coarse search.  8-bit rows are labelled from a widened chunk at a time and stored as bytes.
 void ivf_flat_extend(resources* res, ivf_flat_index& idx, const DLTensor& t, const int64_t* new_ids, int64_t id0)
 {
   auto s = res->stream;
@@ -430,8 +596,25 @@ void ivf_flat_extend(resources* res, ivf_flat_index& idx, const DLTensor& t, con
   auto write = [&](const float* x, int64_t n, uint32_t*, const int64_t* dst_rows, float* data) {
     scatter_rows(s, x, n, int64_t(idx.dim), dst_rows, data);
   };
+  if (idx.row_type != kRowF32) {
+    auto write8 = [&](const float* x, int64_t n, uint32_t*, const int64_t* dst_rows, uint8_t* rows) {
+      count_launch();
+      narrow_rows_kernel<<<blocks_for(n * idx.Kp8, 256), 256, 0, s>>>(x, n, idx.dim, idx.Kp8, dst_rows, rows);
+      B2_CUDA(cudaGetLastError());
+    };
+    insert_rows<uint8_t>(res, t, idx.lists, idx.rows8, idx.Kp8, idx.ids, new_ids, id0, label, write8);
+    refresh_i8_side(res, idx);
+    return;
+  }
   insert_rows<float>(res, t, idx.lists, idx.data, idx.dim, idx.ids, new_ids, id0, label, write);
   refresh_tc_side(res, idx);
+}
+
+// The derived rows of the index's row type
+void refresh_rows(resources* res, ivf_flat_index& idx)
+{
+  if (idx.row_type != kRowF32) refresh_i8_side(res, idx);
+  else refresh_tc_side(res, idx);
 }
 
 ivf_flat_index* ivf_flat_build(resources* res, const cuvsIvfFlatIndexParams& p, const DLTensor& ds)
@@ -453,6 +636,9 @@ ivf_flat_index* ivf_flat_build(resources* res, const cuvsIvfFlatIndexParams& p, 
   idx->adaptive_centers  = p.adaptive_centers;
   idx->kmeans_n_iters    = p.kmeans_n_iters;
   idx->kmeans_trainset_fraction = p.kmeans_trainset_fraction;
+  idx->row_type          = row_type_for(ds.dtype, p.metric);
+  idx->Kp8               = tc_pad_k_i8(d);
+  B2_EXPECTS(idx->row_type != kRowF32 || dl_is(ds, kDLFloat, 32), "ivf_flat_build: float16 rows, and 8-bit rows of a cosine index, must be widened to float32 first");
   auto s = res->stream;
 
   int64_t n_train   = 0;
@@ -464,7 +650,7 @@ ivf_flat_index* ivf_flat_build(resources* res, const cuvsIvfFlatIndexParams& p, 
   std::vector<int64_t> zero(p.n_lists, 0);
   idx->lists.set_sizes(s, zero);
   if (p.add_data_on_build) ivf_flat_extend(res, *idx, ds, nullptr, 0);
-  else refresh_tc_side(res, *idx);
+  else refresh_rows(res, *idx);
   return idx.release();
 }
 
@@ -512,6 +698,122 @@ void exact_probed_search(resources* res, const ivf_flat_index& idx, const float*
   postprocess_distances(s, out_dist, nq * k, idx.metric);
 }
 
+// Search of an 8-bit index (DESIGN.md §4 "Row types").  q [nq, dim] fp32 holds the queries' integer values.  The coarse search
+// is the fp32 one; the fine scan multiplies the pairs' query bytes with the list bytes on the integer tensor cores and ranks by
+// exact keys (tc_i8_key), so the merged candidates are the exact best of the probed lists: no re-score, no certificate.
+//   want <= 16 (32 at Kp8 = 128): the fused epilogue, lists of KC >= want per column half; each holds every row of its half
+//   that can be among the query's want best, and the shared pruning bound stops at each list's want-th key.
+//   otherwise: the store scan and the segmented select keep each pair's want best, which hold the query's want best.
+// want is k, or the kc2 candidates cuvsB200IvfFlatCandidates asks for (dump).
+void ivf_flat_search_i8(resources* res, const ivf_flat_index& idx, uint32_t n_probes, const DLTensor& qt, const DLTensor& nt,
+                        const DLTensor& dt, const uint32_t* keep_bits, int64_t n_bits, const flat_candidates* dump)
+{
+  auto s           = res->stream;
+  const int64_t nq = qt.shape[0];
+  const int k      = static_cast<int>(nt.shape[1]);
+  const int want   = dump ? std::max(32, 2 * k) : k;
+  const int KC     = want <= 16 ? 16 : (want <= 32 && idx.Kp8 == 128 ? 32 : 0);
+  // Query batching.  Per pair: its query bytes, the bound slot, 2 x KC candidates (score, position) and their per-query gather.
+  // Store scan, per query: dense scores over its n_probes largest lists, each pair's want best and their gather (16 bytes each),
+  // pair bookkeeping, and the merged want.
+  const int64_t store_bytes = KC != 0 ? 0
+                                      : large_k_rows_per_query(idx.lists, n_probes) * 4 +
+                                          static_cast<int64_t>(n_probes) * (16 * want + idx.Kp8 + 32) + static_cast<int64_t>(want) * 8;
+  const int64_t batch = query_batch_size(idx.Kp8 + 4 + 2 * 32 * 8 + 16, n_probes, store_bytes, "CUVS_B200_FLAT_LARGE_K_BUDGET_MB");
+  B2_EXPECTS(dump == nullptr || nq <= batch, "ivf_flat candidates: %lld queries do not fit one batch", (long long)nq);
+  if (search_in_batches(batch, qt, nt, dt, [&](const DLTensor& qs, const DLTensor& ns, const DLTensor& ds) {
+        ivf_flat_search_i8(res, idx, n_probes, qs, ns, ds, keep_bits, n_bits, nullptr);
+      }))
+    return;
+  const float* q   = dl_ptr<float>(qt);
+  const bool ip    = idx.metric == InnerProduct;
+
+  // ---- 1. coarse (as for fp32 rows)
+  tc_rows_tmp qp;
+  qp.build(s, q, nq, idx.dim, true, 0, nullptr);
+  dbuf<uint32_t> probes(static_cast<size_t>(nq) * n_probes, s);
+  coarse_select(res, qp, idx.centers_tc, static_cast<int>(n_probes), probes.data(), nullptr);
+
+  // ---- 1b. bitset pre-filter: hidden rows get the padding norm and score +inf
+  const int64_t R  = idx.lists.rows_total;
+  const int* norms = idx.norms8.data();
+  dbuf<int> norms_f;
+  if (keep_bits != nullptr && R > 0) {
+    norms_f.alloc(static_cast<size_t>(std::max<int64_t>(R, 128)), s);
+    count_launch();
+    if (idx.row_type == kRowU8)
+      i8_norms_kernel<true><<<blocks_for(R * 32, 256), 256, 0, s>>>(idx.rows8.data(), R, idx.Kp8, idx.ids.data(), keep_bits, n_bits, norms_f.data());
+    else
+      i8_norms_kernel<false><<<blocks_for(R * 32, 256), 256, 0, s>>>(idx.rows8.data(), R, idx.Kp8, idx.ids.data(), keep_bits, n_bits, norms_f.data());
+    B2_CUDA(cudaGetLastError());
+    norms = norms_f.data();
+  }
+
+  // ---- 2. pairs by list, and their query bytes
+  const int KCW = KC * kTcListsPerItem;
+  probe_buckets pb;
+  bucket_probes(res, probes.data(), nq, static_cast<int>(n_probes), idx.n_lists, idx.lists.d_offsets.data(), KCW, pb);
+  const int64_t a_rows = pb.n_pairs + 128;
+  dbuf<uint8_t> a(static_cast<size_t>(a_rows) * idx.Kp8, s);
+  count_launch();
+  pair_query_bytes_kernel<<<blocks_for(a_rows * idx.Kp8 / 16, 256), 256, 0, s>>>(q, idx.dim, idx.Kp8, pb.pair_query.data(), pb.n_items.data() + 1,
+                                                                            a_rows, a.data());
+  B2_CUDA(cudaGetLastError());
+
+  // ---- 3. fine scan on the integer tensor cores
+  const bool u8       = idx.row_type == kRowU8;
+  const int64_t b_rows = std::max<int64_t>(R, 128);
+  dbuf<float> cs;
+  dbuf<uint32_t> cp;
+  int L = KCW;  // candidates per pair
+  if (KC == 0) {
+    large_k_select(s, pb, idx.lists, nq, n_probes, want, [&](float* scores, const int64_t* seg_off) {
+      item_segments(s, pb, seg_off);
+      timed_section ts("ivf_flat_scan", s);
+      tc_scan_i8(s, res->device, u8, a.data(), a_rows, idx.rows8.data(), b_rows, idx.Kp8, norms, !ip, pb.items.data(), pb.max_items,
+                 pb.n_items.data(), 0, scores, nullptr, 0);
+    }, cs, cp);
+    L = want;
+  } else {
+    cs.alloc(static_cast<size_t>(pb.n_pairs) * KCW, s);
+    cp.alloc(static_cast<size_t>(pb.n_pairs) * KCW, s);
+    dbuf<int> bkeys(static_cast<size_t>(nq), s);
+    B2_CUDA(cudaMemsetAsync(bkeys.data(), tc_bound_init_byte, sizeof(int) * nq, s));
+    tc_bound bnd;
+    bnd.keys = bkeys.data();
+    bnd.idx  = pb.pair_query.data();
+    bnd.kth  = want < KC ? want : 0;
+    timed_section ts("ivf_flat_scan", s);
+    tc_scan_i8(s, res->device, u8, a.data(), a_rows, idx.rows8.data(), b_rows, idx.Kp8, norms, !ip, pb.items.data(), pb.max_items,
+               pb.n_items.data(), KC, cs.data(), cp.data(), KCW, &bnd);
+  }
+
+  // ---- 4. per query: the want best keys of its pairs, then the k best by (distance, id)
+  const int64_t cand_w = static_cast<int64_t>(n_probes) * L;
+  dbuf<float> gs(static_cast<size_t>(nq) * cand_w, s);
+  dbuf<uint32_t> gp(static_cast<size_t>(nq) * cand_w, s);
+  gather_probe_candidates(s, cs.data(), cp.data(), pb.slot_of.data(), nullptr, 1.f, INFINITY, nq, static_cast<int>(n_probes), L,
+                          gs.data(), gp.data());
+  const int kc2 = static_cast<int>(std::min<int64_t>(cand_w, want));
+  dbuf<float> ms(static_cast<size_t>(nq) * kc2, s);
+  dbuf<uint32_t> mp(static_cast<size_t>(nq) * kc2, s);
+  select_k(s, gs.data(), gp.data(), IDX_U32, nq, cand_w, cand_w, kc2, ms.data(), mp.data(), IDX_U32, true);
+  count_launch();
+  if (dump) {
+    B2_EXPECTS(kc2 == want, "ivf_flat candidates: n_probes too small for %d candidates", want);
+    i8_candidates_kernel<<<static_cast<unsigned>(nq), 256, 0, s>>>(ms.data(), mp.data(), kc2, idx.ids.data(), q, idx.dim, ip, dump->ids,
+                                                                   dump->dist, dump->bound);
+    B2_CUDA(cudaGetLastError());
+    B2_CUDA(cudaStreamSynchronize(s));
+    return;
+  }
+  i8_finish_kernel<<<static_cast<unsigned>(nq), 256, 0, s>>>(ms.data(), mp.data(), kc2, idx.ids.data(), q, idx.dim, ip, k,
+                                                             dl_ptr<int64_t>(nt), dl_ptr<float>(dt));
+  B2_CUDA(cudaGetLastError());
+  postprocess_distances(s, dl_ptr<float>(dt), nq * k, idx.metric);
+  set_last_flagged(0);
+}
+
 // dump: stop after the certificate and copy its inputs out (one query batch).
 void ivf_flat_search(resources* res, const ivf_flat_index& idx, uint32_t n_probes, const DLTensor& qt, const DLTensor& nt,
                      const DLTensor& dt, const uint32_t* keep_bits = nullptr, int64_t n_bits = 0,
@@ -526,6 +828,7 @@ void ivf_flat_search(resources* res, const ivf_flat_index& idx, uint32_t n_probe
   B2_EXPECTS(n_probes >= 1, "n_probes must be >= 1");
   if (nq == 0) return;
   n_probes         = std::min<uint32_t>(n_probes, idx.n_lists);
+  if (idx.row_type != kRowF32) return ivf_flat_search_i8(res, idx, n_probes, qt, nt, dt, keep_bits, n_bits, dump);
   // k > 64 (DESIGN.md §4 "k > 64"): the scan stores every (pair, list row) score and a segmented select keeps kc2 per pair.
   const bool large_k = k > 64;
   const int large_kc = std::min(2 * k, kSelectMaxK);
@@ -832,9 +1135,15 @@ cuvsError_t cuvsIvfFlatBuild(cuvsResources_t res, cuvsIvfFlatIndexParams_t param
     const DLTensor& ds = dataset->dl_tensor;
     B2_EXPECTS(dl_is_dataset_dtype(ds), "Unsupported dataset DLtensor dtype: %d and bits: %d", ds.dtype.code, ds.dtype.bits);
     if (index->addr) { delete reinterpret_cast<ivf_flat_index*>(index->addr); index->addr = 0; }
-    f32_matrix w;  // float16 / int8 / uint8 datasets (c/src/neighbors/ivf_flat.cpp dtype switch) are widened to fp32 rows
-    widen_to_f32(r, ds, w);
-    index->addr  = reinterpret_cast<uintptr_t>(ivf_flat_build(r, *params, w.t));
+    // int8 / uint8 datasets in L2 or inner product keep their type; float16 ones, and 8-bit ones for cosine, are widened to fp32
+    // rows (c/src/neighbors/ivf_flat.cpp dtype switch)
+    if (row_type_for(ds.dtype, params->metric) != kRowF32) {
+      index->addr = reinterpret_cast<uintptr_t>(ivf_flat_build(r, *params, ds));
+    } else {
+      f32_matrix w;
+      widen_to_f32(r, ds, w);
+      index->addr = reinterpret_cast<uintptr_t>(ivf_flat_build(r, *params, w.t));
+    }
     index->dtype = ds.dtype;
   });
 }
@@ -866,9 +1175,17 @@ cuvsError_t cuvsIvfFlatSearch(cuvsResources_t res, cuvsIvfFlatSearchParams_t par
       keep   = dl_ptr<uint32_t>(ft->dl_tensor);
       n_bits = ft->dl_tensor.shape[0] * 32;
     }
-    f32_matrix w;
-    widen_to_f32(r, queries, w);
-    ivf_flat_search(r, idx, params->n_probes, w.t, neighbors, distances, keep, n_bits);
+    // narrower queries are widened into stream-ordered memory: no device-wide synchronisation per search
+    B2_EXPECTS(dl_is_dataset_dtype(queries), "Unsupported queries DLtensor dtype: %d and bits: %d", queries.dtype.code, queries.dtype.bits);
+    DLTensor qv = queries;
+    dbuf<float> qw;
+    if (!dl_is(queries, kDLFloat, 32)) {
+      qw.alloc(static_cast<size_t>(std::max<int64_t>(queries.shape[0] * queries.shape[1], 1)), r->stream);
+      widen_async(r->stream, dl_ptr<void>(queries), queries.dtype, queries.shape[0] * queries.shape[1], qw.data());
+      qv.data  = qw.data();
+      qv.dtype = DLDataType{kDLFloat, 32, 1};
+    }
+    ivf_flat_search(r, idx, params->n_probes, qv, neighbors, distances, keep, n_bits);
   });
 }
 
@@ -881,9 +1198,16 @@ cuvsError_t cuvsIvfFlatExtend(cuvsResources_t res, DLManagedTensor* new_vectors,
     B2_EXPECTS(dl_is_dataset_dtype(new_vectors->dl_tensor), "Unsupported new_vectors DLtensor dtype: %d and bits: %d",
                new_vectors->dl_tensor.dtype.code, new_vectors->dl_tensor.dtype.bits);
     f32_matrix wv;
-    widen_to_f32(r, new_vectors->dl_tensor, wv);
+    if (idx.row_type != kRowF32) {  // 8-bit lists take rows of their own type
+      const DLTensor& nv = new_vectors->dl_tensor;
+      B2_EXPECTS(nv.dtype.code == index->dtype.code && nv.dtype.bits == 8, "type mismatch between index and new_vectors");
+      B2_EXPECTS(nv.ndim == 2 && dl_is_c_contiguous(nv), "matrix must be a row-major 2-D tensor");
+      wv.t = nv;
+    } else {
+      widen_to_f32(r, new_vectors->dl_tensor, wv);
+    }
     const DLTensor& v = wv.t;
-    B2_EXPECTS(dl_is(v, kDLFloat, 32) && v.ndim == 2 && v.shape[1] == idx.dim && dl_is_c_contiguous(v), "new_vectors must be [n, dim] row-major");
+    B2_EXPECTS(v.ndim == 2 && v.shape[1] == idx.dim && dl_is_c_contiguous(v), "new_vectors must be [n, dim] row-major");
     dbuf<int64_t> ids_buf;
     // reference: new ids continue after the current size when none are given
     ivf_flat_extend(r, idx, v, device_ids(r, new_indices, v.shape[0], ids_buf), idx.lists.size);
@@ -891,15 +1215,53 @@ cuvsError_t cuvsIvfFlatExtend(cuvsResources_t res, DLManagedTensor* new_vectors,
 }
 
 // cuVS index file, serialization version 4 (cpp/src/neighbors/ivf_flat/ivf_flat_serialize.cuh:25-84; per-list records
-// cpp/src/neighbors/ivf_list.cuh:108-133): the 4-byte dtype tag "<f4\0", then NPY records (npy_io.hpp) —
+// cpp/src/neighbors/ivf_list.cuh:108-133): the 4-byte dtype tag of the index's type ("<f4\0", "<e2\0", "|i1\0", "|u1\0": the
+// kind and size the reader dispatches on, c/src/neighbors/ivf_flat.cpp:307-325), then NPY records (npy_io.hpp) —
 //   version i4 = 4, size i8, dim u4, n_lists u4, metric i4, adaptive_centers u1, conservative_memory_allocation u1,
 //   centers f4 [n_lists, dim], has_norms u1 (+ center_norms f4 [n_lists] for L2), list_sizes u4 [n_lists], then per list:
-//   capacity u4 = size rounded up to 32 and (capacity > 0) data f4 [capacity, dim] in the reference's interleaved layout
-//   (groups of 32 rows, element (r, k) at (r/32)*32*dim + (k/veclen)*32*veclen + (r%32)*veclen + k%veclen, veclen = 4 when
-//   dim % 4 == 0 else 1: ivf_flat.hpp:184-201) and indices i8 [capacity] (-1 = kInvalidRecord on the padding rows).
+//   capacity u4 = size rounded up to 32 and (capacity > 0) data [capacity, dim] of the index's type ('<f4', '<f2', '|i1',
+//   '|u1') in the reference's interleaved layout (groups of 32 rows, element (r, k) at (r/32)*32*dim + (k/veclen)*32*veclen +
+//   (r%32)*veclen + k%veclen, veclen = 16 / sizeof(T) when dim is a multiple of it, else 1: ivf_flat.hpp:184-201, 284-293) and
+//   indices i8 [capacity] (-1 = kInvalidRecord on the padding rows).
 namespace {
 
-inline int flat_veclen(int dim) { return dim % 4 == 0 ? 4 : 1; }
+// an index file's element type: its tag, the descr of its data records and the element size
+struct flat_file_type {
+  const char* tag;
+  const char* descr;
+  int size;
+};
+flat_file_type flat_file_type_of(DLDataType t)
+{
+  if (t.code == kDLFloat) return t.bits == 32 ? flat_file_type{"<f4", "<f4", 4} : flat_file_type{"<e2", "<f2", 2};
+  return t.code == kDLInt ? flat_file_type{"|i1", "|i1", 1} : flat_file_type{"|u1", "|u1", 1};
+}
+// the type a tag or a data record names by its kind and size (float16 is kind 'e' to the reference and 'f' to NumPy); bits 0:
+// none of the four
+DLDataType flat_dtype_of(char kind, int size)
+{
+  if (kind == 'f' && size == 4) return DLDataType{kDLFloat, 32, 1};
+  if ((kind == 'e' || kind == 'f') && size == 2) return DLDataType{kDLFloat, 16, 1};
+  if (kind == 'i' && size == 1) return DLDataType{kDLInt, 8, 1};
+  if (kind == 'u' && size == 1) return DLDataType{kDLUInt, 8, 1};
+  return DLDataType{kDLFloat, 0, 1};
+}
+inline int flat_veclen(int dim, int size) { return dim % (16 / size) == 0 ? 16 / size : 1; }
+inline int64_t interleaved_at(int64_t r, int k, int dim, int vl) { return (r / 32) * 32 * dim + (k / vl) * 32 * vl + (r % 32) * vl + k % vl; }
+
+// fp32 storage value <-> file element of `size` bytes of type t (the values are the type's: the conversions are exact)
+void put_element(DLDataType t, float v, uint8_t* out)
+{
+  if (t.bits == 32) std::memcpy(out, &v, 4);
+  else if (t.bits == 16) { const __half h = __float2half_rn(v); std::memcpy(out, &h, 2); }
+  else *out = static_cast<uint8_t>(static_cast<int>(v));
+}
+float get_element(DLDataType t, const uint8_t* in)
+{
+  if (t.bits == 32) { float v; std::memcpy(&v, in, 4); return v; }
+  if (t.bits == 16) { __half h; std::memcpy(&h, in, 2); return __half2float(h); }
+  return t.code == kDLInt ? static_cast<float>(static_cast<int8_t>(*in)) : static_cast<float>(*in);
+}
 
 }  // namespace
 
@@ -910,8 +1272,8 @@ cuvsError_t cuvsIvfFlatSerialize(cuvsResources_t res, const char* filename, cuvs
     auto& idx = flat_of(index);
     std::ofstream os(filename, std::ios::out | std::ios::binary);
     B2_EXPECTS(bool(os), "Cannot open file %s", filename);
-    const char tag[4] = {'<', 'f', '4', 0};
-    os.write(tag, 4);
+    const flat_file_type ft = flat_file_type_of(index->dtype);
+    os.write(ft.tag, 4);  // three characters and the terminating zero
     npy::write_scalar<int32_t>(os, 4);
     npy::write_scalar<int64_t>(os, idx.lists.size);
     npy::write_scalar<uint32_t>(os, static_cast<uint32_t>(idx.dim));
@@ -937,23 +1299,34 @@ cuvsError_t cuvsIvfFlatSerialize(cuvsResources_t res, const char* filename, cuvs
     std::vector<uint32_t> sizes(idx.n_lists);
     for (uint32_t l = 0; l < idx.n_lists; ++l) sizes[l] = static_cast<uint32_t>(idx.lists.h_sizes[l]);
     npy::write_array<uint32_t>(os, sizes.data(), {static_cast<int64_t>(idx.n_lists)});
-    std::vector<float> rows, inter;
+    const bool native = idx.row_type != kRowF32;
+    const int dim = idx.dim, es = ft.size, vl = flat_veclen(dim, es);
+    std::vector<float> rows;
+    std::vector<uint8_t> rows8, inter;
     std::vector<int64_t> ids;
-    const int dim = idx.dim, vl = flat_veclen(dim);
     for (uint32_t l = 0; l < idx.n_lists; ++l) {
-      const int64_t sz = idx.lists.h_sizes[l], cap = (sz + 31) / 32 * 32;
+      const int64_t sz = idx.lists.h_sizes[l], cap = (sz + 31) / 32 * 32, row0 = idx.lists.h_offsets[l];
       npy::write_scalar<uint32_t>(os, static_cast<uint32_t>(cap));
       if (!cap) continue;
-      rows.resize(static_cast<size_t>(sz) * dim);
       ids.assign(static_cast<size_t>(cap), int64_t(-1));
-      inter.assign(static_cast<size_t>(cap) * dim, 0.f);
-      B2_CUDA(cudaMemcpyAsync(rows.data(), idx.data.data() + idx.lists.h_offsets[l] * dim, rows.size() * sizeof(float), cudaMemcpyDeviceToHost, r->stream));
-      B2_CUDA(cudaMemcpyAsync(ids.data(), idx.ids.data() + idx.lists.h_offsets[l], static_cast<size_t>(sz) * sizeof(int64_t), cudaMemcpyDeviceToHost, r->stream));
+      inter.assign(static_cast<size_t>(cap) * dim * es, 0);
+      B2_CUDA(cudaMemcpyAsync(ids.data(), idx.ids.data() + row0, static_cast<size_t>(sz) * sizeof(int64_t), cudaMemcpyDeviceToHost, r->stream));
+      if (native) {
+        rows8.resize(static_cast<size_t>(sz) * idx.Kp8);
+        B2_CUDA(cudaMemcpyAsync(rows8.data(), idx.rows8.data() + row0 * idx.Kp8, rows8.size(), cudaMemcpyDeviceToHost, r->stream));
+      } else {
+        rows.resize(static_cast<size_t>(sz) * dim);
+        B2_CUDA(cudaMemcpyAsync(rows.data(), idx.data.data() + row0 * dim, rows.size() * sizeof(float), cudaMemcpyDeviceToHost, r->stream));
+      }
       B2_CUDA(cudaStreamSynchronize(r->stream));
       for (int64_t rr = 0; rr < sz; ++rr)
-        for (int k = 0; k < dim; ++k)
-          inter[static_cast<size_t>((rr / 32) * 32 * dim + (k / vl) * 32 * vl + (rr % 32) * vl + k % vl)] = rows[static_cast<size_t>(rr) * dim + k];
-      npy::write_array<float>(os, inter.data(), {cap, dim});
+        for (int k = 0; k < dim; ++k) {
+          uint8_t* o = inter.data() + interleaved_at(rr, k, dim, vl) * es;
+          if (native) *o = rows8[static_cast<size_t>(rr) * idx.Kp8 + k];
+          else put_element(index->dtype, rows[static_cast<size_t>(rr) * dim + k], o);
+        }
+      npy::write_header(os, ft.descr, {cap, dim});
+      os.write(reinterpret_cast<const char*>(inter.data()), static_cast<std::streamsize>(inter.size()));
       npy::write_array<int64_t>(os, ids.data(), {cap});
     }
     B2_EXPECTS(bool(os), "Error writing %s", filename);
@@ -969,7 +1342,9 @@ cuvsError_t cuvsIvfFlatDeserialize(cuvsResources_t res, const char* filename, cu
     B2_EXPECTS(bool(is), "Cannot open file %s", filename);
     char tag[4]{};
     B2_EXPECTS(bool(is.read(tag, 4)), "ivf_flat::deserialize: failed to read dtype prefix");
-    B2_EXPECTS(tag[0] == '<' && tag[1] == 'f' && tag[2] == '4', "ivf_flat::deserialize: serialized dtype prefix does not match requested type");
+    const DLDataType dtype = flat_dtype_of(tag[1], tag[2] - '0');
+    B2_EXPECTS(dtype.bits != 0 && (tag[0] == '<' || tag[0] == '|' || tag[0] == '='),
+               "ivf_flat::deserialize: unsupported dtype prefix '%.3s' in the index file", tag);
     const int ver = npy::read_scalar<int32_t>(is, filename);
     B2_EXPECTS(ver == 4, "serialization version mismatch, expected %d, got %d ", 4, ver);
     const int64_t n_rows = npy::read_scalar<int64_t>(is, filename);
@@ -979,6 +1354,8 @@ cuvsError_t cuvsIvfFlatDeserialize(cuvsResources_t res, const char* filename, cu
     idx->n_lists  = npy::read_scalar<uint32_t>(is, filename);
     idx->metric   = static_cast<cuvsDistanceType>(npy::read_scalar<int32_t>(is, filename));
     idx->adaptive_centers = npy::read_scalar<uint8_t>(is, filename) != 0;
+    idx->row_type = row_type_for(dtype, idx->metric);
+    idx->Kp8      = tc_pad_k_i8(idx->dim);
     (void)npy::read_scalar<uint8_t>(is, filename);  // conservative_memory_allocation: an allocation policy, nothing to restore
     std::vector<float> c(static_cast<size_t>(idx->n_lists) * idx->dim);
     npy::read_array<float>(is, c.data(), static_cast<int64_t>(c.size()), filename);
@@ -996,32 +1373,48 @@ cuvsError_t cuvsIvfFlatDeserialize(cuvsResources_t res, const char* filename, cu
     idx->lists.set_sizes(r->stream, sizes);
     B2_EXPECTS(idx->lists.size == n_rows, "ivf_flat::deserialize: list sizes sum to %lld, header says %lld rows", (long long)idx->lists.size,
                (long long)n_rows);
-    alloc_list_storage(r->stream, idx->lists, idx->dim, idx->data, idx->ids);
-    std::vector<float> rows, inter;
+    const bool native = idx->row_type != kRowF32;
+    if (native) alloc_list_storage(r->stream, idx->lists, idx->Kp8, idx->rows8, idx->ids);
+    else alloc_list_storage(r->stream, idx->lists, idx->dim, idx->data, idx->ids);
+    const int es = dtype.bits / 8, dim = idx->dim, vl = flat_veclen(dim, es);
+    std::vector<float> rows;
+    std::vector<uint8_t> rows8, inter;
     std::vector<int64_t> ids;
-    const int dim = idx->dim, vl = flat_veclen(dim);
     for (uint32_t l = 0; l < idx->n_lists; ++l) {
       const int64_t cap = npy::read_scalar<uint32_t>(is, filename);
-      const int64_t sz  = sizes[l];
+      const int64_t sz  = sizes[l], row0 = idx->lists.h_offsets[l];
       B2_EXPECTS(cap >= sz, "ivf_flat::deserialize: list %u stores %lld rows, list_sizes says %lld", l, (long long)cap, (long long)sz);
       if (!cap) continue;
-      inter.resize(static_cast<size_t>(cap) * dim);
+      const npy::header h = npy::read_header(is, filename);
+      const DLDataType rt = flat_dtype_of(h.descr.size() >= 3 ? h.descr[1] : '?', h.item_size());
+      B2_EXPECTS(rt.code == dtype.code && rt.bits == dtype.bits && !h.fortran && h.count() == cap * dim,
+                 "ivf_flat::deserialize: list %u holds %lld elements of '%s', the file's type '%.3s' needs %lld", l, (long long)h.count(),
+                 h.descr.c_str(), tag, (long long)(cap * dim));
+      inter.resize(static_cast<size_t>(cap) * dim * es);
+      is.read(reinterpret_cast<char*>(inter.data()), static_cast<std::streamsize>(inter.size()));
+      B2_EXPECTS(bool(is), "%s: truncated file", filename);
       ids.resize(static_cast<size_t>(cap));
-      npy::read_array<float>(is, inter.data(), cap * dim, filename);
       npy::read_array<int64_t>(is, ids.data(), cap, filename);
       if (!sz) continue;
-      rows.resize(static_cast<size_t>(sz) * dim);
-      for (int64_t rr = 0; rr < sz; ++rr)
-        for (int k = 0; k < dim; ++k)
-          rows[static_cast<size_t>(rr) * dim + k] = inter[static_cast<size_t>((rr / 32) * 32 * dim + (k / vl) * 32 * vl + (rr % 32) * vl + k % vl)];
-      B2_CUDA(cudaMemcpyAsync(idx->data.data() + idx->lists.h_offsets[l] * dim, rows.data(), rows.size() * sizeof(float), cudaMemcpyHostToDevice, r->stream));
-      B2_CUDA(cudaMemcpyAsync(idx->ids.data() + idx->lists.h_offsets[l], ids.data(), static_cast<size_t>(sz) * sizeof(int64_t), cudaMemcpyHostToDevice, r->stream));
+      if (native) {
+        rows8.assign(static_cast<size_t>(sz) * idx->Kp8, 0);
+        for (int64_t rr = 0; rr < sz; ++rr)
+          for (int k = 0; k < dim; ++k) rows8[static_cast<size_t>(rr) * idx->Kp8 + k] = inter[interleaved_at(rr, k, dim, vl)];
+        B2_CUDA(cudaMemcpyAsync(idx->rows8.data() + row0 * idx->Kp8, rows8.data(), rows8.size(), cudaMemcpyHostToDevice, r->stream));
+      } else {
+        rows.resize(static_cast<size_t>(sz) * dim);
+        for (int64_t rr = 0; rr < sz; ++rr)
+          for (int k = 0; k < dim; ++k)
+            rows[static_cast<size_t>(rr) * dim + k] = get_element(dtype, inter.data() + interleaved_at(rr, k, dim, vl) * es);
+        B2_CUDA(cudaMemcpyAsync(idx->data.data() + row0 * dim, rows.data(), rows.size() * sizeof(float), cudaMemcpyHostToDevice, r->stream));
+      }
+      B2_CUDA(cudaMemcpyAsync(idx->ids.data() + row0, ids.data(), static_cast<size_t>(sz) * sizeof(int64_t), cudaMemcpyHostToDevice, r->stream));
       B2_CUDA(cudaStreamSynchronize(r->stream));
     }
-    refresh_tc_side(r, *idx);
+    refresh_rows(r, *idx);
     if (index->addr) delete reinterpret_cast<ivf_flat_index*>(index->addr);
     index->addr  = reinterpret_cast<uintptr_t>(idx.release());
-    index->dtype = DLDataType{kDLFloat, 32, 1};
+    index->dtype = dtype;
   });
 }
 

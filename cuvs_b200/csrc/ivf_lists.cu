@@ -106,22 +106,35 @@ void place_rows(cudaStream_t s, const uint32_t* labels, int64_t n, const list_la
   B2_CUDA(cudaStreamSynchronize(s));  // `base` is a host vector
 }
 
-// rows of `t` in device-resident chunks of at most 512 MiB (host tensors are staged through one reusable buffer)
+// rows of `t` as fp32 device-resident chunks of at most 512 MiB (host tensors are staged through one reusable buffer; int8 and
+// uint8 rows are widened one chunk at a time)
 template <typename Fn>
 void for_device_chunks(resources* res, const DLTensor& t, Fn&& fn)
 {
   const int64_t n = t.shape[0];
   const int d     = static_cast<int>(t.shape[1]);
-  const float* p  = dl_ptr<float>(t);
   const int64_t chunk = std::max<int64_t>(1, (int64_t(1) << 27) / std::max(d, 1));  // 512 MiB of floats per step
-  const bool dev = dl_is_device(t) && t.device.device_type != kDLCUDAHost;
+  const bool dev  = dl_is_device(t) && t.device.device_type != kDLCUDAHost;
+  const bool f32  = dl_is(t, kDLFloat, 32);
+  const size_t es = t.dtype.bits / 8;
   dbuf<float> buf;
-  if (!dev) buf.alloc(static_cast<size_t>(std::min(n, chunk)) * d, res->stream);
+  dbuf<uint8_t> raw;
+  if (!dev || !f32) buf.alloc(static_cast<size_t>(std::min(n, chunk)) * d, res->stream);
+  if (!dev && !f32) raw.alloc(static_cast<size_t>(std::min(n, chunk)) * d * es, res->stream);
   for (int64_t r0 = 0; r0 < n; r0 += chunk) {
     int64_t rows = std::min(chunk, n - r0);
-    if (dev) fn(p + r0 * d, rows, r0);
-    else {
-      B2_CUDA(cudaMemcpyAsync(buf.data(), p + r0 * d, sizeof(float) * rows * d, cudaMemcpyHostToDevice, res->stream));
+    const uint8_t* src = dl_ptr<uint8_t>(t) + r0 * d * es;
+    if (f32 && dev) {
+      fn(reinterpret_cast<const float*>(src), rows, r0);
+    } else if (f32) {
+      B2_CUDA(cudaMemcpyAsync(buf.data(), src, sizeof(float) * rows * d, cudaMemcpyHostToDevice, res->stream));
+      fn(buf.data(), rows, r0);
+    } else {
+      if (!dev) {
+        B2_CUDA(cudaMemcpyAsync(raw.data(), src, es * rows * d, cudaMemcpyHostToDevice, res->stream));
+        src = raw.data();
+      }
+      widen_async(res->stream, src, t.dtype, rows * d, buf.data());
       fn(buf.data(), rows, r0);
     }
   }
@@ -222,6 +235,7 @@ void insert_rows(resources* res, const DLTensor& t, list_layout& lists, owned<T>
 template void alloc_list_storage<float>(cudaStream_t, const list_layout&, int64_t, owned<float>&, owned<int64_t>&);
 template void alloc_list_storage<uint8_t>(cudaStream_t, const list_layout&, int64_t, owned<uint8_t>&, owned<int64_t>&);
 template void scatter_rows<float>(cudaStream_t, const float*, int64_t, int64_t, const int64_t*, float*);
+template void scatter_rows<uint8_t>(cudaStream_t, const uint8_t*, int64_t, int64_t, const int64_t*, uint8_t*);
 template void insert_rows<float>(resources*, const DLTensor&, list_layout&, owned<float>&, int64_t, owned<int64_t>&, const int64_t*, int64_t,
                                  const label_chunk_fn&, const write_chunk_fn<float>&);
 template void insert_rows<uint8_t>(resources*, const DLTensor&, list_layout&, owned<uint8_t>&, int64_t, owned<int64_t>&, const int64_t*,

@@ -44,7 +44,7 @@ template <typename T>
 using write_chunk_fn = std::function<void(const float* x, int64_t n, uint32_t* labels, const int64_t* dst_rows, T* payload)>;
 
 /**
- * Appends the rows of `t` (fp32 [n, dim], device or host) to the lists, with ids new_ids[i] (device; null: id0 + i), and
+ * Appends the rows of `t` ([n, dim], device or host: fp32, or int8 / uint8 widened one chunk at a time) to the lists, with ids new_ids[i] (device; null: id0 + i), and
  * replaces `lists`, `payload` [rows_total, width] and `ids` with the grown storage.  The rows go through the device in
  * chunks of at most 512 MiB (host rows are staged through one buffer), twice, so that the lists are laid out once for the
  * whole insertion: (1) `label` names each row's list and the rows are counted per list; (2) the old rows move to the new

@@ -171,5 +171,34 @@ __device__ __forceinline__ void wgmma_bf16<128>(float (&d)[64], uint64_t adesc, 
     : "l"(adesc), "l"(bdesc), "r"(scale_d));
 }
 
+// D[64 x 128] (+)= A[64 x 32] * B[128 x 32]^T over 8-bit integers (U8: unsigned, else signed), both K-major in shared memory
+// (one K = 32 step is 32 bytes, as one bf16 K = 16 step), D s32 in registers with wgmma_bf16<128>'s fragment layout.  Integer
+// sums are exact.
+template <bool U8>
+__device__ __forceinline__ void wgmma_i8_128(uint32_t (&d)[64], uint64_t adesc, uint64_t bdesc, uint32_t scale_d)
+{
+#define B2_I8_ARGS                                                                                                          \
+  : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]), "+r"(d[8]), "+r"(d[9]),        \
+    "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15]), "+r"(d[16]), "+r"(d[17]), "+r"(d[18]),           \
+    "+r"(d[19]), "+r"(d[20]), "+r"(d[21]), "+r"(d[22]), "+r"(d[23]), "+r"(d[24]), "+r"(d[25]), "+r"(d[26]), "+r"(d[27]),           \
+    "+r"(d[28]), "+r"(d[29]), "+r"(d[30]), "+r"(d[31]), "+r"(d[32]), "+r"(d[33]), "+r"(d[34]), "+r"(d[35]), "+r"(d[36]),           \
+    "+r"(d[37]), "+r"(d[38]), "+r"(d[39]), "+r"(d[40]), "+r"(d[41]), "+r"(d[42]), "+r"(d[43]), "+r"(d[44]), "+r"(d[45]),           \
+    "+r"(d[46]), "+r"(d[47]), "+r"(d[48]), "+r"(d[49]), "+r"(d[50]), "+r"(d[51]), "+r"(d[52]), "+r"(d[53]), "+r"(d[54]),           \
+    "+r"(d[55]), "+r"(d[56]), "+r"(d[57]), "+r"(d[58]), "+r"(d[59]), "+r"(d[60]), "+r"(d[61]), "+r"(d[62]), "+r"(d[63])           \
+  : "l"(adesc), "l"(bdesc), "r"(scale_d)
+#define B2_I8_REGS                                                                                                          \
+  "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, "    \
+  "%26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, " \
+  "%51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p;\n\t"
+  if constexpr (U8)
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+                 "wgmma.mma_async.sync.aligned.m64n128k32.s32.u8.u8 " B2_I8_REGS "}\n" B2_I8_ARGS);
+  else
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+                 "wgmma.mma_async.sync.aligned.m64n128k32.s32.s8.s8 " B2_I8_REGS "}\n" B2_I8_ARGS);
+#undef B2_I8_REGS
+#undef B2_I8_ARGS
+}
+
 }  // namespace ptx
 }  // namespace b200

@@ -29,6 +29,7 @@
 
 #include <cmath>
 #include <mutex>
+#include <type_traits>
 
 namespace b200 {
 namespace {
@@ -68,19 +69,40 @@ struct cfg {
   static_assert(stages >= 2, "tc_scan_kernel: shared memory budget exceeded");
 };
 
+// Operand types of the scan: bf16 planes (fp32 accumulators), or 8-bit integer rows (s32 accumulators, tc_scan_i8).
+constexpr int kOpBf16 = 0, kOpS8 = 1, kOpU8 = 2;
+
+__device__ __forceinline__ float acc_bits(float x) { return x; }
+__device__ __forceinline__ float acc_bits(uint32_t x) { return __uint_as_float(x); }
+
+// 8-bit scan: the exact integer score s = |x|^2 - 2 q.x (l2) or -q.x of an s32 accumulator q.x and the row's norm n (kI8PadNorm:
+// a padding or hidden row, +inf), as -key with key the order-preserving fp32 image of s (tc_i8_key): the t the epilogue ranks.
+__device__ __forceinline__ uint32_t i8_t_bits(uint32_t acc, int n, int l2)
+{
+  if (n == kI8PadNorm) return __float_as_uint(-INFINITY);
+  const int a = static_cast<int>(acc);
+  const int sc = l2 ? n - 2 * a : -a;
+  return __float_as_uint(-__int_as_float(sc + kI8KeyBias));
+}
+
 // KC > 0: fused top-KC epilogue, two candidate lists per (item, query row) — one per 64-column half of the tiles.
 // KC == 0: "store" epilogue — every score of the tile is written to
 // out_score[out_off + row * out_row_stride + (column within the item's range)] (dense distance block); out_row_stride == 0
 // stands for the item's own width, n_tiles * 128.
-template <int KB, int PASSES, int KC>
+// OP = kOpS8 / kOpU8: one pass over 8-bit rows (a k-block is 128 bytes = 128 components), no half-norm step: the epilogue adds
+// the row norms col_norm[b row] itself (i8_t_bits); scores are order-preserving keys of exact integers.
+template <int KB, int PASSES, int KC, int OP = kOpBf16>
 __global__ void __launch_bounds__(128 + kEpiThreads, 1)
 tc_scan_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant__ CUtensorMap tmA_lo,
                const __grid_constant__ CUtensorMap tmB_hi, const __grid_constant__ CUtensorMap tmB_lo,
                const __grid_constant__ CUtensorMap tmB_x, const tc_item* __restrict__ items, int n_items_host,
                const int* __restrict__ n_items_dev, int kblocks_rt, int* __restrict__ sched_counter, float* __restrict__ out_score, uint32_t* __restrict__ out_pos,
-               int64_t out_row_stride, tc_bound bound)
+               int64_t out_row_stride, tc_bound bound, const int* __restrict__ col_norm, int l2)
 {
+  static_assert(OP == kOpBf16 || PASSES == 1, "8-bit scans are single-pass");
   using C = cfg<KB, PASSES>;
+  constexpr int kBlockK = OP == kOpBf16 ? 64 : 128;  // components of one 128-byte k-block
+  using acc_t = std::conditional_t<OP == kOpBf16, float, uint32_t>;
   constexpr int NA = C::NA, NB = C::NB;
   const int nkb = C::streamed ? kblocks_rt : KB;  // k-blocks of 64 per tile
   const int n_items = n_items_dev ? *n_items_dev : n_items_host;
@@ -170,9 +192,9 @@ tc_scan_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
           ptx::mbar_arrive_expect_tx(a_full, C::a_bytes);
 #pragma unroll
           for (int kb = 0; kb < KB; ++kb) {
-            ptx::tma_load_2d(sA + (0 * KB + kb) * kTileBytes, &tmA_hi, a_full, kb * 64, static_cast<int32_t>(item.a_row0));
+            ptx::tma_load_2d(sA + (0 * KB + kb) * kTileBytes, &tmA_hi, a_full, kb * kBlockK, static_cast<int32_t>(item.a_row0));
             if (NA == 2)
-              ptx::tma_load_2d(sA + (1 * KB + kb) * kTileBytes, &tmA_lo, a_full, kb * 64, static_cast<int32_t>(item.a_row0));
+              ptx::tma_load_2d(sA + (1 * KB + kb) * kTileBytes, &tmA_lo, a_full, kb * kBlockK, static_cast<int32_t>(item.a_row0));
           }
         }
         a_phase ^= 1;
@@ -183,15 +205,15 @@ tc_scan_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
         for (int kb = 0; kb < nkb; ++kb) {
           ptx::mbar_wait(&empty[stage], phase ^ 1);
           if (ptx::elect_one()) {
-            ptx::mbar_arrive_expect_tx(&full[stage], C::x_off + (kb == 0 ? kExtBytes : 0));
+            ptx::mbar_arrive_expect_tx(&full[stage], C::x_off + (OP == kOpBf16 && kb == 0 ? kExtBytes : 0));
             uint8_t* dst = sB + stage * C::stage_bytes;
             if constexpr (C::streamed) {
-              ptx::tma_load_2d(dst, &tmA_hi, &full[stage], kb * 64, static_cast<int32_t>(item.a_row0));
-              if (NA == 2) ptx::tma_load_2d(dst + kTileBytes, &tmA_lo, &full[stage], kb * 64, static_cast<int32_t>(item.a_row0));
+              ptx::tma_load_2d(dst, &tmA_hi, &full[stage], kb * kBlockK, static_cast<int32_t>(item.a_row0));
+              if (NA == 2) ptx::tma_load_2d(dst + kTileBytes, &tmA_lo, &full[stage], kb * kBlockK, static_cast<int32_t>(item.a_row0));
             }
-            ptx::tma_load_2d(dst + C::b_off, &tmB_hi, &full[stage], kb * 64, brow);
-            if (NB == 2) ptx::tma_load_2d(dst + C::b_off + kTileBytes, &tmB_lo, &full[stage], kb * 64, brow);
-            if (kb == 0) ptx::tma_load_2d(dst + C::x_off, &tmB_x, &full[stage], 0, brow);
+            ptx::tma_load_2d(dst + C::b_off, &tmB_hi, &full[stage], kb * kBlockK, brow);
+            if (NB == 2) ptx::tma_load_2d(dst + C::b_off + kTileBytes, &tmB_lo, &full[stage], kb * kBlockK, brow);
+            if (OP == kOpBf16 && kb == 0) ptx::tma_load_2d(dst + C::x_off, &tmB_x, &full[stage], 0, brow);
           }
           if (++stage == C::stages) { stage = 0; phase ^= 1; }
         }
@@ -230,7 +252,7 @@ tc_scan_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
 
     // One tile: run its k-blocks through the tensor cores, then pull this thread's 64 columns into registers.
     auto fetch_tile = [&](uint32_t (&v0)[32], uint32_t (&v1)[32]) {
-      float d[64];
+      acc_t d[64];
 #pragma unroll 1
       for (int kb = 0; kb < nkb; ++kb) {
         ptx::mbar_wait(&full[stage], phase);
@@ -241,18 +263,24 @@ tc_scan_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
           // (16 KB >> 4).  Streamed A: the planes lead the stage, the B planes follow at b_off.
           const uint32_t ah = (C::streamed ? b_lo + wg * 512 : a_lo0 + (0 * KB + kb) * 1024) + k * 2;
           const uint32_t bh = b_lo + (C::b_off >> 4) + k * 2;
-          ptx::wgmma_bf16<128>(d, ptx::desc(ah, ptx::kDescHiSw128), ptx::desc(bh, ptx::kDescHiSw128), (kb | k) != 0 ? 1u : 0u);
-          if (NA == 2) {
-            const uint32_t al = (C::streamed ? b_lo + wg * 512 + 1024 : a_lo0 + (1 * KB + kb) * 1024) + k * 2;
-            ptx::wgmma_bf16<128>(d, ptx::desc(al, ptx::kDescHiSw128), ptx::desc(bh, ptx::kDescHiSw128), 1u);
-          }
-          if (NB == 2) {
-            const uint32_t bl = bh + 1024;
-            ptx::wgmma_bf16<128>(d, ptx::desc(ah, ptx::kDescHiSw128), ptx::desc(bl, ptx::kDescHiSw128), 1u);
+          if constexpr (OP != kOpBf16) {
+            ptx::wgmma_i8_128<OP == kOpU8>(d, ptx::desc(ah, ptx::kDescHiSw128), ptx::desc(bh, ptx::kDescHiSw128), (kb | k) != 0 ? 1u : 0u);
+          } else {
+            ptx::wgmma_bf16<128>(d, ptx::desc(ah, ptx::kDescHiSw128), ptx::desc(bh, ptx::kDescHiSw128), (kb | k) != 0 ? 1u : 0u);
+            if (NA == 2) {
+              const uint32_t al = (C::streamed ? b_lo + wg * 512 + 1024 : a_lo0 + (1 * KB + kb) * 1024) + k * 2;
+              ptx::wgmma_bf16<128>(d, ptx::desc(al, ptx::kDescHiSw128), ptx::desc(bh, ptx::kDescHiSw128), 1u);
+            }
+            if (NB == 2) {
+              const uint32_t bl = bh + 1024;
+              ptx::wgmma_bf16<128>(d, ptx::desc(ah, ptx::kDescHiSw128), ptx::desc(bl, ptx::kDescHiSw128), 1u);
+            }
           }
         }
-        if (kb == 0)  // -= |x|^2/2  (ones rows: all identical, both warpgroups read rows 0..63)
-          ptx::wgmma_bf16<128>(d, ptx::desc(ones_lo, ptx::kDescHiSw32), ptx::desc(b_lo + (C::x_off >> 4), ptx::kDescHiSw32), 1u);
+        if constexpr (OP == kOpBf16) {
+          if (kb == 0)  // -= |x|^2/2  (ones rows: all identical, both warpgroups read rows 0..63)
+            ptx::wgmma_bf16<128>(d, ptx::desc(ones_lo, ptx::kDescHiSw32), ptx::desc(b_lo + (C::x_off >> 4), ptx::kDescHiSw32), 1u);
+        }
         ptx::wgmma_commit();
         ptx::wgmma_wait<0>();
         release(&empty[stage]);  // this warp's share of the MMAs has read the stage
@@ -262,8 +290,8 @@ tc_scan_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
       ptx::named_bar_sync(1 + wg, 128);  // every thread of the warpgroup has read the previous tile's rows
 #pragma unroll
       for (int j = 0; j < 16; ++j) {
-        *reinterpret_cast<float2*>(stg_frag + 8 * j)              = make_float2(d[4 * j], d[4 * j + 1]);
-        *reinterpret_cast<float2*>(stg_frag + 8 * kStgLd + 8 * j) = make_float2(d[4 * j + 2], d[4 * j + 3]);
+        *reinterpret_cast<float2*>(stg_frag + 8 * j)              = make_float2(acc_bits(d[4 * j]), acc_bits(d[4 * j + 1]));
+        *reinterpret_cast<float2*>(stg_frag + 8 * kStgLd + 8 * j) = make_float2(acc_bits(d[4 * j + 2]), acc_bits(d[4 * j + 3]));
       }
       ptx::named_bar_sync(1 + wg, 128);
 #pragma unroll
@@ -273,6 +301,25 @@ tc_scan_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
         v0[4 * c4] = x.x; v0[4 * c4 + 1] = x.y; v0[4 * c4 + 2] = x.z; v0[4 * c4 + 3] = x.w;
         v1[4 * c4] = y.x; v1[4 * c4 + 1] = y.y; v1[4 * c4 + 2] = y.z; v1[4 * c4 + 3] = y.w;
       }
+    };
+    // 8-bit scans: 32 accumulator columns to the epilogue's t (i8_t_bits), nrm their row norms.  Done per 32 columns, just before
+    // they are used: converting all 64 at once makes the fused epilogues spill.
+    auto to_t = [&](uint32_t (&v)[32], const int* nrm) {
+      if constexpr (OP != kOpBf16) {
+#pragma unroll
+        for (int c4 = 0; c4 < 8; ++c4) {
+          const int4 n = __ldg(reinterpret_cast<const int4*>(nrm) + c4);
+          v[4 * c4]     = i8_t_bits(v[4 * c4], n.x, l2);
+          v[4 * c4 + 1] = i8_t_bits(v[4 * c4 + 1], n.y, l2);
+          v[4 * c4 + 2] = i8_t_bits(v[4 * c4 + 2], n.z, l2);
+          v[4 * c4 + 3] = i8_t_bits(v[4 * c4 + 3], n.w, l2);
+        }
+      }
+    };
+    // the norms of this thread's columns of tile t of an item (8-bit scans only)
+    auto tile_norms = [&](const tc_item& item, uint32_t t) -> const int* {
+      if constexpr (OP == kOpBf16) return nullptr;
+      else return col_norm + item.b_row0 + t * 128 + col0;
     };
     auto begin_item = [&]() {
       if constexpr (!C::streamed) ptx::mbar_wait(a_full, a_phase);
@@ -295,6 +342,8 @@ tc_scan_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
         for (uint32_t t = 0; t < item.n_tiles; ++t) {
           uint32_t v0[32], v1[32];
           fetch_tile(v0, v1);
+          to_t(v0, tile_norms(item, t));
+          to_t(v1, tile_norms(item, t) + 32);
           if (live) {
             float4* o4 = reinterpret_cast<float4*>(orow + t * 128);
 #pragma unroll
@@ -397,7 +446,9 @@ tc_scan_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
           uint32_t v0[32], v1[32];
           fetch_tile(v0, v1);
           const uint32_t pos0 = item.b_row0 + t * 128 + col0;
+          to_t(v0, tile_norms(item, t));
           scan32(v0, pos0);
+          to_t(v1, tile_norms(item, t) + 32);
           scan32(v1, pos0 + 32);
         }
         end_item();
@@ -453,6 +504,21 @@ CUtensorMap make_plane_map(const __nv_bfloat16* ptr, int64_t rows, int Kp)
   return m;
 }
 
+// [rows, Kp] 8-bit rows, 128-byte k-blocks (128 components) with the bf16 planes' 128-byte swizzle: the same tile bytes
+CUtensorMap make_byte_map(const void* ptr, int64_t rows, int Kp)
+{
+  CUtensorMap m;
+  cuuint64_t gdim[2]    = {static_cast<cuuint64_t>(Kp), static_cast<cuuint64_t>(rows)};
+  cuuint64_t gstride[1] = {static_cast<cuuint64_t>(Kp)};
+  cuuint32_t box[2]     = {128, 128};
+  cuuint32_t estr[2]    = {1, 1};
+  CUresult r = get_encode_fn()(&m, CU_TENSOR_MAP_DATA_TYPE_UINT8, 2, const_cast<void*>(ptr), gdim, gstride, box, estr,
+                               CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                               CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  B2_EXPECTS(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled (8-bit rows) failed with code %d (rows=%lld Kp=%d)", int(r), (long long)rows, Kp);
+  return m;
+}
+
 // [rows, 16] bf16 half-norm extension plane, one 32-byte row per dataset row
 CUtensorMap make_ext_map(const __nv_bfloat16* ptr, int64_t rows)
 {
@@ -468,12 +534,13 @@ CUtensorMap make_ext_map(const __nv_bfloat16* ptr, int64_t rows)
   return m;
 }
 
-template <int KB, int PASSES, int KC>
+template <int KB, int PASSES, int KC, int OP = kOpBf16>
 void launch(cudaStream_t stream, int sm_count, const CUtensorMap& a_hi, const CUtensorMap& a_lo, const CUtensorMap& b_hi,
             const CUtensorMap& b_lo, const CUtensorMap& b_x, const tc_item* items, int n_items, const int* n_items_dev,
-            float* out_score, uint32_t* out_pos, int64_t out_row_stride, const tc_bound& bound, bool dynamic, int kblocks)
+            float* out_score, uint32_t* out_pos, int64_t out_row_stride, const tc_bound& bound, bool dynamic, int kblocks,
+            const int* col_norm = nullptr, int l2 = 0)
 {
-  auto kern = tc_scan_kernel<KB, PASSES, KC>;
+  auto kern = tc_scan_kernel<KB, PASSES, KC, OP>;
   using C   = cfg<KB, PASSES>;
   static_assert(C::smem <= 227 * 1024, "tc_scan_kernel: shared memory budget exceeded");
   // per launch, not once: the attribute belongs to the current device's context, and one process may drive several GPUs
@@ -488,7 +555,7 @@ void launch(cudaStream_t stream, int sm_count, const CUtensorMap& a_hi, const CU
   timed_section ts("tc_scan", stream);
   count_launch();
   kern<<<grid, C::threads, C::smem, stream>>>(a_hi, a_lo, b_hi, b_lo, b_x, items, n_items, n_items_dev, kblocks, sched.data(), out_score,
-                                               out_pos, out_row_stride, bound);
+                                               out_pos, out_row_stride, bound, col_norm, l2);
   B2_CUDA(cudaGetLastError());
 }
 
@@ -621,6 +688,31 @@ void tc_scan_topk(cudaStream_t stream, int device, const __nv_bfloat16* a_hi, co
   B2_TC_CASE(0, 3, 16) B2_TC_CASE(0, 3, 32) B2_TC_CASE(0, 3, 0)
 #undef B2_TC_CASE
   B2_FAIL("tc_scan_topk: no kernel for Kp=%d passes=%d KC=%d", Kp, passes, KC);
+}
+
+void tc_scan_i8(cudaStream_t stream, int device, bool is_unsigned, const void* a, int64_t a_rows_pad, const void* b,
+                int64_t b_rows_pad, int Kp, const int* b_norm, bool l2, const tc_item* items_dev, int n_items,
+                const int* n_items_dev, int KC, float* out_score, uint32_t* out_pos, int64_t out_row_stride, const tc_bound* bound)
+{
+  if (n_items == 0) return;
+  B2_EXPECTS(Kp >= 128 && Kp % 128 == 0 && Kp <= kTcMaxK, "tc_scan_i8: padded K must be a multiple of 128 up to %d (got %d)", kTcMaxK, Kp);
+  // the fused top-32 epilogue is built for Kp = 128 only: with a second resident k-block or a streamed A it spills
+  B2_EXPECTS(KC == 0 || KC == 16 || (KC == 32 && Kp == 128), "tc_scan_i8: KC must be 0 (store), 16, or 32 with Kp = 128");
+  const int sms      = sm_count_of(device);
+  const tc_bound bnd = bound ? *bound : tc_bound{};
+  CUtensorMap mA     = make_byte_map(a, a_rows_pad, Kp);
+  CUtensorMap mB     = make_byte_map(b, b_rows_pad, Kp);
+  const int kb_case  = Kp <= 256 ? Kp / 128 : 0;  // 0 = streamed A
+#define B2_I8_CASE(KB_, KC_, OP_)                                                                                       \
+  if (kb_case == KB_ && KC == KC_ && (OP_ == kOpU8) == is_unsigned)                                                     \
+    return launch<KB_, 1, KC_, OP_>(stream, sms, mA, mA, mB, mB, mB, items_dev, n_items, n_items_dev, out_score, out_pos,  \
+                                    out_row_stride, bnd, true, Kp / 128, b_norm, l2 ? 1 : 0);
+  B2_I8_CASE(1, 16, kOpS8) B2_I8_CASE(1, 32, kOpS8) B2_I8_CASE(1, 0, kOpS8) B2_I8_CASE(2, 16, kOpS8) B2_I8_CASE(2, 0, kOpS8)
+  B2_I8_CASE(0, 16, kOpS8) B2_I8_CASE(0, 0, kOpS8)
+  B2_I8_CASE(1, 16, kOpU8) B2_I8_CASE(1, 32, kOpU8) B2_I8_CASE(1, 0, kOpU8) B2_I8_CASE(2, 16, kOpU8) B2_I8_CASE(2, 0, kOpU8)
+  B2_I8_CASE(0, 16, kOpU8) B2_I8_CASE(0, 0, kOpU8)
+#undef B2_I8_CASE
+  B2_FAIL("tc_scan_i8: no kernel for Kp=%d KC=%d", Kp, KC);
 }
 
 }  // namespace b200

@@ -90,4 +90,27 @@ void tc_scan_topk(cudaStream_t stream, int device, const __nv_bfloat16* a_hi, co
                   float* out_score, uint32_t* out_pos, int64_t out_row_stride, const tc_bound* bound = nullptr,
                   bool dynamic_schedule = true);
 
+/**
+ * 8-bit rows (DESIGN.md §4 "Row types").  Scores are exact integers, s = |x|^2 - 2 q.x (L2) or -q.x (inner product), handed to
+ * the epilogue and written out as order-preserving fp32 keys: the float whose bits are s + kI8KeyBias (positive and finite
+ * for every d <= 2048), so that the fused top-k, the pruning bound and the radix selects rank them exactly.  A row norm of
+ * kI8PadNorm (padding rows, rows a filter hides) scores +inf.
+ */
+constexpr int kI8KeyBias = 1 << 30;
+constexpr int kI8PadNorm = 0x7fffffff;
+__device__ __forceinline__ float tc_i8_key(int s) { return __int_as_float(s + kI8KeyBias); }
+__device__ __forceinline__ int tc_i8_score(float key) { return __float_as_int(key) - kI8KeyBias; }
+inline int tc_pad_k_i8(int d) { return (d + 127) / 128 * 128; }
+
+/**
+ * tc_scan_topk over 8-bit rows: A [a_rows_pad, Kp] and B [b_rows_pad, Kp] int8 (uint8 when `is_unsigned`), K-major, Kp a
+ * multiple of 128; b_norm [b_rows_pad] the exact |x|^2 of each B row (kI8PadNorm: excluded), `l2` false for inner product.
+ * Same work items, epilogues and outputs as tc_scan_topk with passes = 1 (dynamic schedule), the scores being tc_i8_key's.
+ * KC = 32 needs Kp = 128.
+ */
+void tc_scan_i8(cudaStream_t stream, int device, bool is_unsigned, const void* a, int64_t a_rows_pad, const void* b,
+                int64_t b_rows_pad, int Kp, const int* b_norm, bool l2, const tc_item* items_dev, int n_items,
+                const int* n_items_dev, int KC, float* out_score, uint32_t* out_pos, int64_t out_row_stride,
+                const tc_bound* bound = nullptr);
+
 }  // namespace b200
