@@ -74,9 +74,9 @@ struct ivf_pq_index {
   tc_rows centers_tc;
   list_layout lists;
   // [rows_total, pq_dim], one code per byte.  When the index is served by the code-streaming scan the stream below IS the
-  // index and this flat copy is dropped after (re)building it; ensure_flat_codes() re-materialises it for the paths that
-  // want rows (getters, extend, serialize, the LUT kernel).
-  mutable owned<uint8_t> codes;
+  // index and this flat copy is dropped after (re)building it.  Extend re-materialises it (ensure_flat_codes); the read-only
+  // paths (getters, serialize, the LUT kernel) decode the rows they need into a buffer of their own call (flat_codes).
+  owned<uint8_t> codes;
   owned<int64_t> ids;    // [rows_total], kPadId on padding rows
   // decoded side (the decoded scan)
   int Kp = 0;
@@ -92,13 +92,33 @@ struct ivf_pq_index {
 
 namespace {
 
-void ensure_flat_codes(resources* res, const ivf_pq_index& idx)
+bool has_flat_codes(const ivf_pq_index& idx)
 {
-  const size_t need = static_cast<size_t>(std::max<int64_t>(idx.lists.rows_total, 1)) * idx.pq_dim;
-  if (idx.codes.data() != nullptr && idx.codes.size() >= need) return;
+  return idx.codes.data() != nullptr && idx.codes.size() >= static_cast<size_t>(std::max<int64_t>(idx.lists.rows_total, 1)) * idx.pq_dim;
+}
+
+// Extend only: it rewrites the lists anyway, so the flat codes go back into the index.
+void ensure_flat_codes(resources* res, ivf_pq_index& idx)
+{
+  if (has_flat_codes(idx)) return;
   B2_EXPECTS(idx.cstream.data() != nullptr, "ivf_pq: the index holds neither flat codes nor a code stream");
-  idx.codes.alloc(need);
+  idx.codes.alloc(static_cast<size_t>(std::max<int64_t>(idx.lists.rows_total, 1)) * idx.pq_dim);
   pq_stream_to_flat(res->stream, idx.cstream.data(), idx.lists.rows_total, idx.pq_dim, idx.codes.data());
+}
+
+// Flat codes of rows [row0, row0 + n) for the read-only paths, which must leave the index as they found it: several callers
+// may read one index at once, each on its own stream.  An index that keeps its flat codes is read in place; one served by the
+// code stream has the 128-row tiles covering the rows decoded into `tmp`, stream-ordered on `s` and freed with the call.
+// Returns the address of row row0.
+const uint8_t* flat_codes(cudaStream_t s, const ivf_pq_index& idx, int64_t row0, int64_t n, dbuf<uint8_t>& tmp)
+{
+  if (n == 0) return nullptr;
+  if (has_flat_codes(idx)) return idx.codes.data() + row0 * idx.pq_dim;
+  B2_EXPECTS(idx.cstream.data() != nullptr, "ivf_pq: the index holds neither flat codes nor a code stream");
+  const int64_t t0 = row0 / 128, t1 = (row0 + n + 127) / 128;
+  tmp.alloc(static_cast<size_t>(t1 - t0) * 128 * idx.pq_dim, s);
+  pq_stream_to_flat(s, idx.cstream.data() + t0 * pq_stream_tile_bytes(idx.pq_dim), (t1 - t0) * 128, idx.pq_dim, tmp.data());
+  return tmp.data() + (row0 - t0 * 128) * idx.pq_dim;
 }
 
 // ------------------------------------------------------------------ fp_8bit<5, Signed> (ivf_pq_fp_8bit.cuh:31-100)
@@ -834,8 +854,8 @@ scan_plan plan_scan(const ivf_pq_index& idx, const cuvsIvfPqSearchParams& sp, in
 // one CTA per pair slot: the grid covers every slot, the live count is on the device, and the slots past it (dropped pairs,
 // garbage pair_query) exit at once.  Otherwise the LUT goes to a global scratch with one slice per resident CTA (DESIGN.md §5).
 template <bool Store>
-void launch_lut_scan(cudaStream_t s, const ivf_pq_index& idx, const cuvsIvfPqSearchParams& sp, const float* q_rot, const probe_buckets& pb,
-                     int KC, float* out_score, uint32_t* out_pos, int KCW, const int64_t* seg_off)
+void launch_lut_scan(cudaStream_t s, const ivf_pq_index& idx, const uint8_t* codes, const cuvsIvfPqSearchParams& sp, const float* q_rot,
+                     const probe_buckets& pb, int KC, float* out_score, uint32_t* out_pos, int KCW, const int64_t* seg_off)
 {
   constexpr size_t kMaxSmem = 227 * 1024;
   const size_t lut_b        = sp.lut_dtype == CUDA_R_32F ? 4 : (sp.lut_dtype == CUDA_R_16F ? 2 : 1);
@@ -854,7 +874,7 @@ void launch_lut_scan(cudaStream_t s, const ivf_pq_index& idx, const cuvsIvfPqSea
       timed_section ts("pq_scan", s);
       count_launch();
       kern<<<static_cast<unsigned>(pb.n_pairs), kLutThreads, smem, s>>>(
-        q_rot, idx.centers_rot.data(), idx.pq_centers.data(), per_cl, idx.codes.data(), idx.lists.d_offsets.data(), idx.lists.d_sizes.data(),
+        q_rot, idx.centers_rot.data(), idx.pq_centers.data(), per_cl, codes, idx.lists.d_offsets.data(), idx.lists.d_sizes.data(),
         pb.pair_query.data(), pb.pair_list.data(), pb.n_items.data() + 1, idx.rot_dim, idx.pq_dim, idx.pq_len, idx.pq_bits, ip, cosine,
         KC, out_score, out_pos, KCW, seg_off);
       return;
@@ -880,7 +900,7 @@ void launch_lut_scan(cudaStream_t s, const ivf_pq_index& idx, const cuvsIvfPqSea
     timed_section ts("pq_scan", s);
     count_launch();
     kern<<<static_cast<unsigned>(grid), kLutThreads, work, s>>>(
-      q_rot, idx.centers_rot.data(), idx.pq_centers.data(), per_cl, idx.codes.data(), idx.lists.d_offsets.data(), idx.lists.d_sizes.data(),
+      q_rot, idx.centers_rot.data(), idx.pq_centers.data(), per_cl, codes, idx.lists.d_offsets.data(), idx.lists.d_sizes.data(),
       pb.pair_query.data(), pb.pair_list.data(), pb.n_items.data() + 1, idx.rot_dim, idx.pq_dim, idx.pq_len, idx.pq_bits, ip, cosine,
       KC, out_score, out_pos, KCW, seg_off, scratch.data());
   };
@@ -941,12 +961,14 @@ void ivf_pq_search(resources* res, const ivf_pq_index& idx, const cuvsIvfPqSearc
                 plan.group);
   dbuf<float> add;
   dbuf<int> bkeys;  // per-query pruning bound of the tensor-core scan (tc_bound), reused by the merge
+  dbuf<uint8_t> lut_buf;  // the LUT kernel's flat codes when the index keeps only its code stream
+  const uint8_t* lut_codes = plan.path == scan_path::lut ? flat_codes(s, idx, 0, idx.lists.rows_total, lut_buf) : nullptr;
   float scale = 1.0f;
   // out / out_pos: each pair's KCW candidates; store: the dense segments at seg_off (out_pos unused)
   auto scan = [&](float* out, uint32_t* out_pos, const int64_t* seg_off) {
     if (plan.path == scan_path::lut) {
-      ensure_flat_codes(res, idx);
-      (plan.store ? launch_lut_scan<true> : launch_lut_scan<false>)(s, idx, sp, q_rot.data(), pb, plan.KC, out, out_pos, plan.KCW, seg_off);
+      (plan.store ? launch_lut_scan<true> : launch_lut_scan<false>)(s, idx, lut_codes, sp, q_rot.data(), pb, plan.KC, out, out_pos, plan.KCW,
+                                                                    seg_off);
       return;
     }
     residual_rows a;
@@ -1161,7 +1183,7 @@ cuvsError_t cuvsIvfPqIndexUnpackContiguousListData(cuvsResources_t res, cuvsIvfP
 {
   return guarded([=] {
     auto r    = as_res(res);
-    auto& idx = pq_of(index);
+    const ivf_pq_index& idx = pq_of(index);
     B2_EXPECTS(label < idx.n_lists, "label %u out of range", label);
     const DLTensor& oc = out_codes->dl_tensor;
     B2_EXPECTS(dl_is(oc, kDLUInt, 8) && oc.ndim == 2 && dl_is_device(oc) && dl_is_c_contiguous(oc), "out_codes must be a device uint8 matrix");
@@ -1170,9 +1192,9 @@ cuvsError_t cuvsIvfPqIndexUnpackContiguousListData(cuvsResources_t res, cuvsIvfP
     const int64_t n_take = oc.shape[0];
     B2_EXPECTS(static_cast<int64_t>(offset) + n_take <= idx.lists.h_sizes[label], "offset + n_rows exceeds the list size");
     if (n_take == 0) return;
-    ensure_flat_codes(r, idx);
-    pack_codes_kernel<<<blocks_for(n_take, 128), 128, 0, r->stream>>>(idx.codes.data() + (idx.lists.h_offsets[label] + offset) * idx.pq_dim,
-                                                                      n_take, idx.pq_dim, idx.pq_bits, out_ld, dl_ptr<uint8_t>(oc));
+    dbuf<uint8_t> tmp;
+    const uint8_t* codes = flat_codes(r->stream, idx, idx.lists.h_offsets[label] + offset, n_take, tmp);
+    pack_codes_kernel<<<blocks_for(n_take, 128), 128, 0, r->stream>>>(codes, n_take, idx.pq_dim, idx.pq_bits, out_ld, dl_ptr<uint8_t>(oc));
     B2_CUDA(cudaGetLastError());
   });
 }
@@ -1370,7 +1392,7 @@ cuvsError_t cuvsIvfPqSerialize(cuvsResources_t res, const char* filename, cuvsIv
 {
   return guarded([=] {
     auto r    = as_res(res);
-    auto& idx = pq_of(index);
+    const ivf_pq_index& idx = pq_of(index);
     std::ofstream os(filename, std::ios::out | std::ios::binary);
     B2_EXPECTS(bool(os), "Cannot open file %s", filename);
     npy::write_scalar<int32_t>(os, 4);
@@ -1402,14 +1424,15 @@ cuvsError_t cuvsIvfPqSerialize(cuvsResources_t res, const char* filename, cuvsIv
     std::vector<uint8_t> codes;
     std::vector<int64_t> ids;
     const int C = 128 / idx.pq_bits;
-    ensure_flat_codes(r, idx);
+    dbuf<uint8_t> tmp;
     for (uint32_t l = 0; l < idx.n_lists; ++l) {
       const int64_t sz = idx.lists.h_sizes[l];
       npy::write_scalar<uint32_t>(os, static_cast<uint32_t>(sz));
       if (!sz) continue;
       codes.resize(static_cast<size_t>(sz) * idx.pq_dim);
       ids.resize(static_cast<size_t>(sz));
-      B2_CUDA(cudaMemcpyAsync(codes.data(), idx.codes.data() + idx.lists.h_offsets[l] * idx.pq_dim, codes.size(), cudaMemcpyDeviceToHost, r->stream));
+      const uint8_t* d_codes = flat_codes(r->stream, idx, idx.lists.h_offsets[l], sz, tmp);
+      B2_CUDA(cudaMemcpyAsync(codes.data(), d_codes, codes.size(), cudaMemcpyDeviceToHost, r->stream));
       B2_CUDA(cudaMemcpyAsync(ids.data(), idx.ids.data() + idx.lists.h_offsets[l], ids.size() * sizeof(int64_t), cudaMemcpyDeviceToHost, r->stream));
       B2_CUDA(cudaStreamSynchronize(r->stream));
       const std::vector<uint8_t> packed = pack_interleaved(codes.data(), sz, idx.pq_dim, idx.pq_bits);
