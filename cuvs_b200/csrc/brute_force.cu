@@ -366,8 +366,6 @@ static void bf_search(resources* res, const bf_index& idx, const DLTensor& qt, c
   auto stream      = res->stream;
   const int64_t nq = qt.shape[0];
   const int k      = static_cast<int>(nt.shape[1]);
-  B2_EXPECTS(qt.shape[1] == idx.d, "queries dim (%lld) != index dim (%d)", (long long)qt.shape[1], idx.d);
-  B2_EXPECTS(nt.shape[0] == nq && dt.shape[0] == nq && dt.shape[1] == k, "neighbors/distances shape mismatch");
   B2_EXPECTS(k >= 1, "k must be >= 1");
   int64_t* out_idx = dl_ptr<int64_t>(nt);
   float* out_dist  = dl_ptr<float>(dt);
@@ -384,15 +382,8 @@ static void bf_search(resources* res, const bf_index& idx, const DLTensor& qt, c
     q = qcopy.data();
   }
 
-  filter_view filt;
-  if (prefilter.type != NO_FILTER) {
-    B2_EXPECTS(prefilter.type == BITSET || prefilter.type == BITMAP, "Unsupported prefilter type");
-    auto ft = reinterpret_cast<DLManagedTensor*>(prefilter.addr);
-    B2_EXPECTS(ft != nullptr && dl_is_device(ft->dl_tensor), "prefilter should have device compatible memory");
-    filt.bits      = dl_ptr<uint32_t>(ft->dl_tensor);
-    filt.kind      = prefilter.type == BITSET ? 1 : 2;
-    filt.n_samples = idx.n;
-  }
+  filter_view filt = read_prefilter(prefilter, true, "Unsupported prefilter type");
+  if (filt.kind) filt.n_samples = idx.n;  // the bitmap's row length
 
   const bool select_min = metric_is_min_close(idx.metric);
   // k <= 24: fused lists of 16 / 32, merged to the list length.  24 < k <= 64 (the reference's fused range,
@@ -456,7 +447,7 @@ cuvsError_t cuvsBruteForceIndexDestroy(cuvsBruteForceIndex_t index)
 {
   return guarded([=] {
     if (!index) return;
-    delete reinterpret_cast<bf_index*>(index->addr);
+    drop_index<bf_index>(index);
     delete index;
   });
 }
@@ -469,18 +460,16 @@ cuvsError_t cuvsBruteForceBuild(cuvsResources_t res, DLManagedTensor* dataset_te
     B2_EXPECTS(dataset_tensor != nullptr && index != nullptr, "null argument");
     const DLTensor& ds = dataset_tensor->dl_tensor;
     if (dl_is(ds, kDLFloat, 32)) {
-      if (index->addr) { delete reinterpret_cast<bf_index*>(index->addr); index->addr = 0; }
-      index->addr  = reinterpret_cast<uintptr_t>(bf_build(r, ds, metric, metric_arg));
-      index->dtype = ds.dtype;
+      drop_index<bf_index>(index);
+      set_index(index, bf_build(r, ds, metric, metric_arg), ds.dtype);
     } else if (dl_is_dataset_dtype(ds)) {
       // float16 / int8 / uint8 (c/src/neighbors/brute_force.cpp:60-110): widened once, the index owns the fp32 copy
       f32_matrix w;
       widen_to_f32(r, ds, w);
-      if (index->addr) { delete reinterpret_cast<bf_index*>(index->addr); index->addr = 0; }
+      drop_index<bf_index>(index);
       bf_index* b = bf_build(r, w.t, metric, metric_arg);
       if (b->data == w.own.data()) b->data_own = std::move(w.own);
-      index->addr  = reinterpret_cast<uintptr_t>(b);
-      index->dtype = ds.dtype;
+      set_index(index, b, ds.dtype);
     } else {
       B2_FAIL("Unsupported dataset DLtensor dtype: %d and bits: %d", ds.dtype.code, ds.dtype.bits);
     }
@@ -492,25 +481,19 @@ cuvsError_t cuvsBruteForceSearch(cuvsResources_t res, cuvsBruteForceIndex_t inde
 {
   return guarded([=] {
     auto r = as_res(res);
-    B2_EXPECTS(index && index->addr && queries_tensor && neighbors_tensor && distances_tensor, "null argument");
+    B2_EXPECTS(queries_tensor && neighbors_tensor && distances_tensor, "null argument");
+    auto& idx                 = index_of<bf_index>(index);
     const DLTensor& queries   = queries_tensor->dl_tensor;
     const DLTensor& neighbors = neighbors_tensor->dl_tensor;
     const DLTensor& distances = distances_tensor->dl_tensor;
-    // same checks / messages as c/src/neighbors/brute_force.cpp:193-206
-    B2_EXPECTS(dl_is_device(queries), "queries should have device compatible memory");
-    B2_EXPECTS(dl_is_device(neighbors), "neighbors should have device compatible memory");
-    B2_EXPECTS(dl_is_device(distances), "distances should have device compatible memory");
-    B2_EXPECTS(dl_is(neighbors, kDLInt, 64), "neighbors should be of type int64_t");
-    B2_EXPECTS(dl_is(distances, kDLFloat, 32), "distances should be of type float32");
+    check_search_tensors(queries, neighbors, distances, idx.d, false);
     B2_EXPECTS(queries.dtype.code == index->dtype.code, "type mismatch between index and queries");
-    B2_EXPECTS(queries.ndim == 2 && neighbors.ndim == 2 && distances.ndim == 2, "queries/neighbors/distances must be 2-D");
-    B2_EXPECTS(dl_is_c_contiguous(neighbors) && dl_is_c_contiguous(distances), "outputs must be row-major contiguous");
     if (dl_is(queries, kDLFloat, 32)) {
-      bf_search(r, *reinterpret_cast<bf_index*>(index->addr), queries, neighbors, distances, prefilter);
+      bf_search(r, idx, queries, neighbors, distances, prefilter);
     } else if (dl_is_dataset_dtype(queries) && queries.dtype.bits == index->dtype.bits) {
-      f32_matrix w;
+      f32_rows w;
       widen_to_f32(r, queries, w);
-      bf_search(r, *reinterpret_cast<bf_index*>(index->addr), w.t, neighbors, distances, prefilter);
+      bf_search(r, idx, w.t, neighbors, distances, prefilter);
     } else {
       B2_FAIL("Unsupported queries DLtensor dtype: %d and bits: %d", queries.dtype.code, queries.dtype.bits);
     }
@@ -522,8 +505,8 @@ cuvsError_t cuvsB200BruteForceCandidates(cuvsResources_t res, cuvsBruteForceInde
 {
   return guarded([=] {
     auto r = as_res(res);
-    B2_EXPECTS(index && index->addr && queries && cand_pos && cand_score, "null argument");
-    auto& idx           = *reinterpret_cast<bf_index*>(index->addr);
+    B2_EXPECTS(queries && cand_pos && cand_score, "null argument");
+    auto& idx           = index_of<bf_index>(index);
     const DLTensor& q   = queries->dl_tensor;
     const DLTensor& cp  = cand_pos->dl_tensor;
     const DLTensor& cs  = cand_score->dl_tensor;
@@ -547,8 +530,8 @@ cuvsError_t cuvsBruteForceSerialize(cuvsResources_t res, const char* filename, c
 {
   return guarded([=] {
     auto r = as_res(res);
-    B2_EXPECTS(index && index->addr && filename, "null argument");
-    auto& idx = *reinterpret_cast<bf_index*>(index->addr);
+    B2_EXPECTS(filename, "null argument");
+    auto& idx = index_of<bf_index>(index);
     std::vector<float> host(static_cast<size_t>(idx.n) * idx.d);
     B2_CUDA(cudaMemcpyAsync(host.data(), idx.data, host.size() * sizeof(float), cudaMemcpyDeviceToHost, r->stream));
     B2_CUDA(cudaStreamSynchronize(r->stream));
@@ -588,16 +571,9 @@ cuvsError_t cuvsBruteForceDeserialize(cuvsResources_t res, const char* filename,
     std::vector<float> host(static_cast<size_t>(n) * d);
     is.read(reinterpret_cast<char*>(host.data()), static_cast<std::streamsize>(host.size() * sizeof(float)));
     B2_EXPECTS(bool(is), "Truncated index file %s", filename);
-    int64_t shape[2] = {n, d};
-    DLTensor t{};
-    t.data   = host.data();
-    t.device = DLDevice{kDLCPU, 0};
-    t.ndim   = 2;
-    t.dtype  = DLDataType{kDLFloat, 32, 1};
-    t.shape  = shape;
-    if (index->addr) { delete reinterpret_cast<bf_index*>(index->addr); index->addr = 0; }
-    index->addr  = reinterpret_cast<uintptr_t>(bf_build(r, t, static_cast<cuvsDistanceType>(m), marg));
-    index->dtype = t.dtype;
+    const dl_view rows(host.data(), DLDevice{kDLCPU, 0}, DLDataType{kDLFloat, 32, 1}, n, d);
+    drop_index<bf_index>(index);
+    set_index(index, bf_build(r, rows.t(), static_cast<cuvsDistanceType>(m), marg), rows.t().dtype);
   });
 }
 

@@ -34,7 +34,11 @@ void widen_async(cudaStream_t s, const void* in, DLDataType dt, int64_t count, f
   B2_CUDA(cudaGetLastError());
 }
 
-void widen_to_f32(resources* res, const DLTensor& src, f32_matrix& out)
+static void alloc_on(owned<float>& b, size_t count, cudaStream_t) { b.alloc(count); }
+static void alloc_on(dbuf<float>& b, size_t count, cudaStream_t s) { b.alloc(count, s); }
+
+template <typename Buf>
+static void widen_into(resources* res, const DLTensor& src, f32_widened<Buf>& out)
 {
   B2_EXPECTS(src.ndim == 2 && dl_is_c_contiguous(src), "matrix must be a row-major 2-D tensor");
   B2_EXPECTS(dl_is_dataset_dtype(src), "Unsupported DLtensor dtype: %d and bits: %d", src.dtype.code, src.dtype.bits);
@@ -46,9 +50,8 @@ void widen_to_f32(resources* res, const DLTensor& src, f32_matrix& out)
   if (dl_is(src, kDLFloat, 32)) return;
   const int64_t count = src.shape[0] * src.shape[1];
   const size_t esize  = src.dtype.bits / 8;
-  out.own.alloc(static_cast<size_t>(std::max<int64_t>(count, 1)));
-  out.widened = true;
-  auto s      = res->stream;
+  auto s              = res->stream;
+  alloc_on(out.own, static_cast<size_t>(std::max<int64_t>(count, 1)), s);
   const void* in = dl_ptr<char>(src);
   dbuf<uint8_t> stage;
   const bool dev = dl_is_device(src) && src.device.device_type != kDLCUDAHost;
@@ -62,6 +65,38 @@ void widen_to_f32(resources* res, const DLTensor& src, f32_matrix& out)
   out.t.byte_offset = 0;
   out.t.dtype       = DLDataType{kDLFloat, 32, 1};
   out.t.device      = DLDevice{kDLCUDA, res->device};
+}
+void widen_to_f32(resources* res, const DLTensor& src, f32_matrix& out) { widen_into(res, src, out); }
+void widen_to_f32(resources* res, const DLTensor& src, f32_rows& out) { widen_into(res, src, out); }
+
+void check_search_tensors(const DLTensor& queries, const DLTensor& neighbors, const DLTensor& distances, int64_t dim,
+                          bool uint32_neighbors)
+{
+  B2_EXPECTS(dl_is_device(queries), "queries should have device compatible memory");
+  B2_EXPECTS(dl_is_device(neighbors), "neighbors should have device compatible memory");
+  B2_EXPECTS(dl_is_device(distances), "distances should have device compatible memory");
+  if (uint32_neighbors)
+    B2_EXPECTS(dl_is(neighbors, kDLUInt, 32) || dl_is(neighbors, kDLInt, 64), "neighbors should be of type uint32_t or int64_t");
+  else
+    B2_EXPECTS(dl_is(neighbors, kDLInt, 64), "neighbors should be of type int64_t");
+  B2_EXPECTS(dl_is(distances, kDLFloat, 32), "distances should be of type float32");
+  B2_EXPECTS(queries.ndim == 2 && neighbors.ndim == 2 && distances.ndim == 2, "queries/neighbors/distances must be 2-D");
+  B2_EXPECTS(dl_is_c_contiguous(neighbors) && dl_is_c_contiguous(distances), "neighbors/distances must be row-major contiguous");
+  B2_EXPECTS(neighbors.shape[0] == queries.shape[0] && distances.shape[0] == neighbors.shape[0] && distances.shape[1] == neighbors.shape[1],
+             "neighbors/distances shape mismatch");
+  B2_EXPECTS(queries.shape[1] == dim, "queries dim (%lld) != index dim (%lld)", (long long)queries.shape[1], (long long)dim);
+}
+
+filter_view read_prefilter(cuvsFilter filter, bool bitmap_ok, const char* unsupported)
+{
+  if (filter.type == NO_FILTER) return filter_view{};
+  B2_EXPECTS(filter.type == BITSET || (bitmap_ok && filter.type == BITMAP), "%s", unsupported);
+  auto ft = reinterpret_cast<const DLManagedTensor*>(filter.addr);
+  B2_EXPECTS(ft != nullptr && dl_is_device(ft->dl_tensor), "prefilter should have device compatible memory");
+  const DLTensor& t = ft->dl_tensor;
+  B2_EXPECTS(dl_is(t, kDLUInt, 32) && t.ndim == 1 && dl_is_c_contiguous(t), "prefilter must be a contiguous 1-D uint32 tensor (got dtype code %d, bits %d, ndim %d)",
+             int(t.dtype.code), int(t.dtype.bits), t.ndim);
+  return filter_view{dl_ptr<uint32_t>(t), filter.type == BITSET ? 1 : 2, t.shape[0] * 32};
 }
 
 

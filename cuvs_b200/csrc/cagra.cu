@@ -1458,83 +1458,55 @@ __global__ void select_pruned_kernel(const uint32_t* __restrict__ knn, const uin
 
 }  // namespace
 
-// exact kNN graph through the library's own brute-force search (C boundary re-used internally)
+// kNN graph of the rows (kk neighbours, self included) by a chunked self-search through the library's own C entry points:
+// exact brute force, or (large inputs) an IVF-Flat index of ~sqrt(n) lists, whose search takes k <= 64
 static void build_knn_graph(cuvsResources_t res_h, resources* res, const float* data, int64_t n, int dim, cuvsDistanceType metric,
-                            int kk, int64_t* knn_out)
+                            int kk, bool exact, int64_t* knn_out)
 {
-  cuvsBruteForceIndex_t bf = nullptr;
-  B2_EXPECTS(cuvsBruteForceIndexCreate(&bf) == CUVS_SUCCESS, "brute force index create failed");
-  int64_t shape[2] = {n, dim};
-  DLManagedTensor ds{};
-  ds.dl_tensor.data = const_cast<float*>(data); ds.dl_tensor.device = DLDevice{kDLCUDA, res->device}; ds.dl_tensor.ndim = 2;
-  ds.dl_tensor.dtype = DLDataType{kDLFloat, 32, 1}; ds.dl_tensor.shape = shape;
-  cuvsDistanceType m = metric == InnerProduct || metric == CosineExpanded ? metric : L2Expanded;
-  if (cuvsBruteForceBuild(res_h, &ds, m, 2.0f, bf) != CUVS_SUCCESS) {
-    std::string e = cuvsGetLastErrorText() ? cuvsGetLastErrorText() : "?";
-    cuvsBruteForceIndexDestroy(bf);
-    B2_FAIL("cagra build: kNN stage failed: %s", e.c_str());
-  }
-  const int64_t chunk = 16384;
-  dbuf<float> dist(static_cast<size_t>(chunk) * kk, res->stream);
-  for (int64_t r0 = 0; r0 < n; r0 += chunk) {
-    int64_t rows = std::min(chunk, n - r0);
-    int64_t qs[2] = {rows, dim}, os[2] = {rows, kk};
-    DLManagedTensor q = ds, nb{}, dd{};
-    q.dl_tensor.data = const_cast<float*>(data) + r0 * dim; q.dl_tensor.shape = qs;
-    nb.dl_tensor.data = knn_out + r0 * kk; nb.dl_tensor.device = ds.dl_tensor.device; nb.dl_tensor.ndim = 2;
-    nb.dl_tensor.dtype = DLDataType{kDLInt, 64, 1}; nb.dl_tensor.shape = os;
-    dd = nb; dd.dl_tensor.data = dist.data(); dd.dl_tensor.dtype = DLDataType{kDLFloat, 32, 1};
-    if (cuvsBruteForceSearch(res_h, bf, &q, &nb, &dd, cuvsFilter{0, NO_FILTER}) != CUVS_SUCCESS) {
-      std::string e = cuvsGetLastErrorText() ? cuvsGetLastErrorText() : "?";
-      cuvsBruteForceIndexDestroy(bf);
-      B2_FAIL("cagra build: kNN stage failed: %s", e.c_str());
-    }
-  }
-  B2_CUDA(cudaStreamSynchronize(res->stream));
-  cuvsBruteForceIndexDestroy(bf);
-}
-
-// approximate kNN graph for large inputs: IVF-Flat self-search (k <= 64) in query chunks
-static void build_knn_graph_ivf(cuvsResources_t res_h, resources* res, const float* data, int64_t n, int dim, cuvsDistanceType metric,
-                                int kk, int64_t* knn_out)
-{
-  cuvsIvfFlatIndexParams_t ip = nullptr;
+  const cuvsDistanceType m  = metric == InnerProduct || metric == CosineExpanded ? metric : L2Expanded;
+  const DLDevice dev{kDLCUDA, res->device};
+  cuvsBruteForceIndex_t bf     = nullptr;
+  cuvsIvfFlatIndexParams_t ip  = nullptr;
   cuvsIvfFlatSearchParams_t sp = nullptr;
-  cuvsIvfFlatIndex_t ix = nullptr;
-  auto fail = [&](const char* what) {
-    std::string e = cuvsGetLastErrorText() ? cuvsGetLastErrorText() : "?";
+  cuvsIvfFlatIndex_t ix        = nullptr;
+  auto release = [&] {
+    if (bf) cuvsBruteForceIndexDestroy(bf);
     if (ix) cuvsIvfFlatIndexDestroy(ix);
     if (ip) cuvsIvfFlatIndexParamsDestroy(ip);
     if (sp) cuvsIvfFlatSearchParamsDestroy(sp);
-    B2_FAIL("cagra build: %s failed: %s", what, e.c_str());
   };
-  if (cuvsIvfFlatIndexParamsCreate(&ip) != CUVS_SUCCESS || cuvsIvfFlatSearchParamsCreate(&sp) != CUVS_SUCCESS || cuvsIvfFlatIndexCreate(&ix) != CUVS_SUCCESS)
-    fail("parameter setup");
-  uint32_t n_lists = 16;
-  while (static_cast<int64_t>(n_lists) * n_lists < n) n_lists *= 2;  // ~sqrt(n), power of two
-  ip->n_lists = n_lists; ip->metric = metric == InnerProduct || metric == CosineExpanded ? metric : L2Expanded; ip->kmeans_n_iters = 10;
-  sp->n_probes = std::max<uint32_t>(16, n_lists / 32);
-  int64_t shape[2] = {n, dim};
-  DLManagedTensor ds{};
-  ds.dl_tensor.data = const_cast<float*>(data); ds.dl_tensor.device = DLDevice{kDLCUDA, res->device}; ds.dl_tensor.ndim = 2;
-  ds.dl_tensor.dtype = DLDataType{kDLFloat, 32, 1}; ds.dl_tensor.shape = shape;
-  if (cuvsIvfFlatBuild(res_h, ip, &ds, ix) != CUVS_SUCCESS) fail("kNN stage (ivf_flat build)");
-  const int64_t chunk = 65536;
+  auto check = [&](cuvsError_t e, const char* what) {
+    if (e == CUVS_SUCCESS) return;
+    std::string text = cuvsGetLastErrorText() ? cuvsGetLastErrorText() : "?";
+    release();
+    B2_FAIL("cagra build: %s failed: %s", what, text.c_str());
+  };
+  dl_view ds(data, dev, DLDataType{kDLFloat, 32, 1}, n, dim);
+  if (exact) {
+    check(cuvsBruteForceIndexCreate(&bf), "kNN stage (brute force create)");
+    check(cuvsBruteForceBuild(res_h, &ds.m, m, 2.0f, bf), "kNN stage (brute force build)");
+  } else {
+    check(cuvsIvfFlatIndexParamsCreate(&ip), "parameter setup");
+    check(cuvsIvfFlatSearchParamsCreate(&sp), "parameter setup");
+    check(cuvsIvfFlatIndexCreate(&ix), "parameter setup");
+    uint32_t n_lists = 16;
+    while (static_cast<int64_t>(n_lists) * n_lists < n) n_lists *= 2;  // ~sqrt(n), power of two
+    ip->n_lists = n_lists; ip->metric = m; ip->kmeans_n_iters = 10;
+    sp->n_probes = std::max<uint32_t>(16, n_lists / 32);
+    check(cuvsIvfFlatBuild(res_h, ip, &ds.m, ix), "kNN stage (ivf_flat build)");
+  }
+  const int64_t chunk = exact ? 16384 : 65536;
   dbuf<float> dist(static_cast<size_t>(chunk) * kk, res->stream);
   for (int64_t r0 = 0; r0 < n; r0 += chunk) {
-    int64_t rows = std::min(chunk, n - r0);
-    int64_t qs[2] = {rows, dim}, os[2] = {rows, kk};
-    DLManagedTensor q = ds, nb{}, dd{};
-    q.dl_tensor.data = const_cast<float*>(data) + r0 * dim; q.dl_tensor.shape = qs;
-    nb.dl_tensor.data = knn_out + r0 * kk; nb.dl_tensor.device = ds.dl_tensor.device; nb.dl_tensor.ndim = 2;
-    nb.dl_tensor.dtype = DLDataType{kDLInt, 64, 1}; nb.dl_tensor.shape = os;
-    dd = nb; dd.dl_tensor.data = dist.data(); dd.dl_tensor.dtype = DLDataType{kDLFloat, 32, 1};
-    if (cuvsIvfFlatSearch(res_h, sp, ix, &q, &nb, &dd, cuvsFilter{0, NO_FILTER}) != CUVS_SUCCESS) fail("kNN stage (ivf_flat search)");
+    const int64_t rows = std::min(chunk, n - r0);
+    dl_view q(data + r0 * dim, dev, DLDataType{kDLFloat, 32, 1}, rows, dim);
+    dl_view nb(knn_out + r0 * kk, dev, DLDataType{kDLInt, 64, 1}, rows, kk);
+    dl_view dd(dist.data(), dev, DLDataType{kDLFloat, 32, 1}, rows, kk);
+    if (exact) check(cuvsBruteForceSearch(res_h, bf, &q.m, &nb.m, &dd.m, cuvsFilter{0, NO_FILTER}), "kNN stage (brute force search)");
+    else check(cuvsIvfFlatSearch(res_h, sp, ix, &q.m, &nb.m, &dd.m, cuvsFilter{0, NO_FILTER}), "kNN stage (ivf_flat search)");
   }
   B2_CUDA(cudaStreamSynchronize(res->stream));
-  cuvsIvfFlatIndexDestroy(ix);
-  cuvsIvfFlatIndexParamsDestroy(ip);
-  cuvsIvfFlatSearchParamsDestroy(sp);
+  release();
 }
 
 }  // namespace b200
@@ -1593,19 +1565,6 @@ void b200::set_half_rows(resources* r, cagra_index& idx)
   count_launch();
   to_half_rows_kernel<<<blocks_for(idx.n * idx.ld16, 256), 256, 0, r->stream>>>(idx.rows_f32(), idx.n, idx.dim, idx.ld, idx.ld16, idx.data16.data());
   B2_CUDA(cudaGetLastError());
-}
-
-// what an index file says about the element type: the 4-byte tag in front (cagra_serialize.cuh:59-61) and the strided
-// dataset record's cudaDataType (dataset_serialize.hpp:83-99).  float16 is numpy kind 'e' (c/src/neighbors/cagra.cpp:889).
-struct file_dtype {
-  const char* tag;    // written; the reader looks at kind and size only
-  const char* descr;  // NPY descr of the data record
-  cudaDataType cuda;
-};
-static file_dtype file_dtype_of(DLDataType t)
-{
-  if (t.code == kDLFloat) return t.bits == 32 ? file_dtype{"<f4", "<f4", CUDA_R_32F} : file_dtype{"<e2", "<f2", CUDA_R_16F};
-  return t.code == kDLInt ? file_dtype{"|i1", "|i1", CUDA_R_8I} : file_dtype{"|u1", "|u1", CUDA_R_8U};
 }
 
 // BitwiseHamming counts the differing bits of the rows' bytes, so it takes int8 and uint8 rows only
@@ -1688,17 +1647,17 @@ cuvsError_t cuvsCagraIndexDestroy(cuvsCagraIndex_t index)
 {
   return guarded([=] {
     if (!index) return;
-    delete reinterpret_cast<cagra_index*>(index->addr);
+    drop_index<cagra_index>(index);
     delete index;
   });
 }
-cuvsError_t cuvsCagraIndexGetDims(cuvsCagraIndex_t index, int64_t* dim) { return guarded([=] { *dim = cagra_of(index).dim; }); }
-cuvsError_t cuvsCagraIndexGetSize(cuvsCagraIndex_t index, int64_t* size) { return guarded([=] { *size = cagra_of(index).n; }); }
-cuvsError_t cuvsCagraIndexGetGraphDegree(cuvsCagraIndex_t index, int64_t* d) { return guarded([=] { *d = cagra_of(index).degree; }); }
+cuvsError_t cuvsCagraIndexGetDims(cuvsCagraIndex_t index, int64_t* dim) { return guarded([=] { *dim = index_of<cagra_index>(index).dim; }); }
+cuvsError_t cuvsCagraIndexGetSize(cuvsCagraIndex_t index, int64_t* size) { return guarded([=] { *size = index_of<cagra_index>(index).n; }); }
+cuvsError_t cuvsCagraIndexGetGraphDegree(cuvsCagraIndex_t index, int64_t* d) { return guarded([=] { *d = index_of<cagra_index>(index).degree; }); }
 cuvsError_t cuvsCagraIndexGetDataset(cuvsCagraIndex_t index, DLManagedTensor* dataset)
 {
   return guarded([=] {
-    auto& idx        = cagra_of(index);
+    auto& idx        = index_of<cagra_index>(index);
     int64_t shape[2] = {idx.n, idx.dim};
     dl_fill_view(dataset, const_cast<void*>(idx.data), idx.device, idx.dtype, 2, shape);
     if (idx.ld != idx.dim) {
@@ -1715,7 +1674,7 @@ cuvsError_t cuvsCagraIndexGetDataset(cuvsCagraIndex_t index, DLManagedTensor* da
 cuvsError_t cuvsCagraIndexGetGraph(cuvsCagraIndex_t index, DLManagedTensor* graph)
 {
   return guarded([=] {
-    auto& idx        = cagra_of(index);
+    auto& idx        = index_of<cagra_index>(index);
     int64_t shape[2] = {idx.n, idx.degree};
     dl_fill_view(graph, const_cast<uint32_t*>(idx.graph), idx.device, DLDataType{kDLUInt, 32, 1}, 2, shape);
   });
@@ -1745,9 +1704,8 @@ cuvsError_t cuvsCagraIndexFromArgs(cuvsResources_t res, cuvsDistanceType metric,
       idx->graph = idx->graph_own.data();
     }
     B2_CUDA(cudaStreamSynchronize(r->stream));
-    if (index->addr) delete reinterpret_cast<cagra_index*>(index->addr);
-    index->dtype = idx->dtype;
-    index->addr  = reinterpret_cast<uintptr_t>(idx.release());
+    const DLDataType dtype = idx->dtype;
+    set_index(index, idx.release(), dtype);
   });
 }
 
@@ -1803,8 +1761,7 @@ cuvsError_t cuvsCagraBuild(cuvsResources_t res, cuvsCagraIndexParams_t params, D
         data = compact.data();
       }
       dbuf<int64_t> knn(static_cast<size_t>(n) * kk, r->stream);
-      if (exact) build_knn_graph(res, r, data, n, idx->dim, idx->metric, kk, knn.data());
-      else build_knn_graph_ivf(res, r, data, n, idx->dim, idx->metric, kk, knn.data());
+      build_knn_graph(res, r, data, n, idx->dim, idx->metric, kk, exact, knn.data());
       // ---- self-free neighbour rows
       nbr.alloc(static_cast<size_t>(n) * di, r->stream);
       count_launch();
@@ -1827,9 +1784,8 @@ cuvsError_t cuvsCagraBuild(cuvsResources_t res, cuvsCagraIndexParams_t params, D
     B2_CUDA(cudaStreamSynchronize(r->stream));
     idx->graph  = idx->graph_own.data();
     idx->degree = degree;
-    if (index->addr) delete reinterpret_cast<cagra_index*>(index->addr);
-    index->dtype = idx->dtype;
-    index->addr  = reinterpret_cast<uintptr_t>(idx.release());
+    const DLDataType dtype = idx->dtype;
+    set_index(index, idx.release(), dtype);
   });
 }
 
@@ -1839,36 +1795,21 @@ cuvsError_t cuvsCagraSearch(cuvsResources_t res, cuvsCagraSearchParams_t params,
   return guarded([=] {
     auto r = as_res(res);
     B2_EXPECTS(params && queries_t && neighbors_t && distances_t, "null argument");
-    auto& idx = cagra_of(index);
+    auto& idx = index_of<cagra_index>(index);
     const DLTensor& queries   = queries_t->dl_tensor;
     const DLTensor& neighbors = neighbors_t->dl_tensor;
     const DLTensor& distances = distances_t->dl_tensor;
     // checks as in c/src/neighbors/cagra.cpp:646-690
-    B2_EXPECTS(dl_is_device(queries), "queries should have device compatible memory");
-    B2_EXPECTS(dl_is_device(neighbors), "neighbors should have device compatible memory");
-    B2_EXPECTS(dl_is_device(distances), "distances should have device compatible memory");
-    B2_EXPECTS(dl_is(neighbors, kDLUInt, 32) || dl_is(neighbors, kDLInt, 64), "neighbors should be of type uint32_t or int64_t");
-    B2_EXPECTS(dl_is(distances, kDLFloat, 32), "distances should be of type float32");
+    check_search_tensors(queries, neighbors, distances, idx.dim, true);
     B2_EXPECTS(queries.dtype.code == index->dtype.code && queries.dtype.bits == index->dtype.bits, "type mismatch between index and queries");
-    B2_EXPECTS(queries.ndim == 2 && neighbors.ndim == 2 && distances.ndim == 2, "queries/neighbors/distances must be 2-D");
-    B2_EXPECTS(dl_is_c_contiguous(queries) && dl_is_c_contiguous(neighbors) && dl_is_c_contiguous(distances), "tensors must be row-major contiguous");
-    B2_EXPECTS(queries.shape[1] == idx.dim, "queries dim (%lld) != index dim (%d)", (long long)queries.shape[1], idx.dim);
-    B2_EXPECTS(neighbors.shape[0] == queries.shape[0] && distances.shape[0] == queries.shape[0] && distances.shape[1] == neighbors.shape[1], "neighbors/distances shape mismatch");
-    const uint32_t* keep = nullptr;
-    int64_t n_bits       = 0;
-    if (filter.type != NO_FILTER) {
-      B2_EXPECTS(filter.type == BITSET, "cagra search: only bitset pre-filters are supported (c/src/neighbors/cagra.cpp)");
-      auto ft = reinterpret_cast<DLManagedTensor*>(filter.addr);
-      B2_EXPECTS(ft != nullptr && dl_is_device(ft->dl_tensor), "prefilter should have device compatible memory");
-      keep   = dl_ptr<uint32_t>(ft->dl_tensor);
-      n_bits = ft->dl_tensor.shape[0] * 32;
-    }
+    B2_EXPECTS(dl_is_c_contiguous(queries), "queries must be row-major contiguous");
+    const filter_view filt = read_prefilter(filter, false, "cagra search: only bitset pre-filters are supported (c/src/neighbors/cagra.cpp)");
     const bool u32 = dl_is(neighbors, kDLUInt, 32);
-    f32_matrix wq;
+    f32_rows wq;
     widen_to_f32(r, queries, wq);
     cagra_search(r, idx, *params, dl_ptr<float>(wq.t), queries.shape[0], static_cast<int>(neighbors.shape[1]),
                  u32 ? dl_ptr<uint32_t>(neighbors) : nullptr, u32 ? nullptr : dl_ptr<int64_t>(neighbors), dl_ptr<float>(distances),
-                 keep, n_bits);
+                 filt.bits, filt.n_samples);
   });
 }
 
@@ -1882,12 +1823,11 @@ cuvsError_t cuvsCagraSerialize(cuvsResources_t res, const char* filename, cuvsCa
 {
   return guarded([=] {
     auto r    = as_res(res);
-    auto& idx = cagra_of(index);
+    auto& idx = index_of<cagra_index>(index);
     std::ofstream os(filename, std::ios::out | std::ios::binary);
     B2_EXPECTS(bool(os), "Cannot open file %s", filename);
-    const file_dtype ft = file_dtype_of(idx.dtype);
-    const char tag[4]   = {ft.tag[0], ft.tag[1], ft.tag[2], 0};
-    os.write(tag, 4);
+    const npy::file_dtype& ft = npy::file_dtype_for(idx.dtype);
+    os.write(ft.tag, 4);  // three characters and the terminating zero
     npy::write_scalar<int32_t>(os, 5);
     npy::write_scalar<uint32_t>(os, static_cast<uint32_t>(idx.n));
     npy::write_scalar<uint32_t>(os, static_cast<uint32_t>(idx.dim));
@@ -1925,13 +1865,9 @@ cuvsError_t cuvsCagraDeserialize(cuvsResources_t res, const char* filename, cuvs
     B2_EXPECTS(bool(is), "Cannot open file %s", filename);
     char tag[4]{};
     B2_EXPECTS(bool(is.read(tag, 4)), "cagra::deserialize: failed to read dtype prefix");
-    // c/src/neighbors/cagra.cpp:881-899: kind and item size name the element type; 1-byte types carry no byte order
-    DLDataType dtype{};
-    if (tag[1] == 'f' && tag[2] == '4') dtype = DLDataType{kDLFloat, 32, 1};
-    else if ((tag[1] == 'e' || tag[1] == 'f') && tag[2] == '2') dtype = DLDataType{kDLFloat, 16, 1};
-    else if (tag[1] == 'i' && tag[2] == '1') dtype = DLDataType{kDLInt, 8, 1};
-    else if (tag[1] == 'u' && tag[2] == '1') dtype = DLDataType{kDLUInt, 8, 1};
-    B2_EXPECTS(dtype.bits != 0 && (tag[0] == '<' || tag[0] == '|' || tag[0] == '='), "cagra::deserialize: unsupported dtype prefix in the index file");
+    const npy::file_dtype* ft = npy::file_dtype_named(std::string(tag, 3));
+    B2_EXPECTS(ft != nullptr, "cagra::deserialize: unsupported dtype prefix in the index file");
+    const DLDataType dtype = ft->dl;
     const int ver = npy::read_scalar<int32_t>(is, filename);
     B2_EXPECTS(ver == 5, "serialization version mismatch, expected %d, got %d ", 5, ver);
     auto idx    = std::make_unique<cagra_index>();
@@ -1955,7 +1891,7 @@ cuvsError_t cuvsCagraDeserialize(cuvsResources_t res, const char* filename, cuvs
     B2_EXPECTS(dt == static_cast<uint32_t>(CUDA_R_32F) || dt == static_cast<uint32_t>(CUDA_R_16F) || dt == static_cast<uint32_t>(CUDA_R_8I) ||
                  dt == static_cast<uint32_t>(CUDA_R_8U),
                "Failed to deserialize dataset: unsupported strided dataset element type %u.", dt);
-    B2_EXPECTS(dt == static_cast<uint32_t>(file_dtype_of(dtype).cuda),
+    B2_EXPECTS(dt == static_cast<uint32_t>(ft->cuda),
                "cagra::deserialize: the dataset's element type %u contradicts the file's dtype prefix '%c%c'", dt, tag[1], tag[2]);
     const int64_t rows = npy::read_scalar<int64_t>(is, filename);
     const uint32_t dim = npy::read_scalar<uint32_t>(is, filename);
@@ -1973,9 +1909,7 @@ cuvsError_t cuvsCagraDeserialize(cuvsResources_t res, const char* filename, cuvs
     idx->data  = idx->data_own.data();
     set_inv_norms(r, *idx);  // the file has no norm record (cagra_serialize.cuh): recomputed from the loaded rows
     B2_CUDA(cudaStreamSynchronize(r->stream));
-    if (index->addr) delete reinterpret_cast<cagra_index*>(index->addr);
-    index->addr  = reinterpret_cast<uintptr_t>(idx.release());
-    index->dtype = dtype;
+    set_index(index, idx.release(), dtype);
   });
 }
 
@@ -1995,7 +1929,7 @@ cuvsError_t cuvsB200CagraSetWalkPrecision(cuvsResources_t res, cuvsCagraIndex_t 
 {
   return guarded([=] {
     auto r    = as_res(res);
-    auto& idx = cagra_of(index);
+    auto& idx = index_of<cagra_index>(index);
     B2_EXPECTS(bits == 16 || bits == 32, "walk precision must be 16 or 32 bits");
     B2_EXPECTS(bits == 32 || idx.elem_size() != 1, "walk precision 16 is refused: the index's rows are 8-bit, already narrower than fp16");
     if (!idx.is_f32()) return;

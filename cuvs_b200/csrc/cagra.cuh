@@ -32,12 +32,6 @@ struct cagra_index {
   owned<float> inv_norm;
 };
 
-inline cagra_index& cagra_of(cuvsCagraIndex_t index)
-{
-  B2_EXPECTS(index != nullptr && index->addr != 0, "index is not built");
-  return *reinterpret_cast<cagra_index*>(index->addr);
-}
-
 /** The graph walk over `nq` fp32 queries (device), the algorithm chosen by `sp.algo` (AUTO as cuvsCagraSearch). */
 void cagra_search(resources* res, const cagra_index& idx, const cuvsCagraSearchParams& sp, const float* queries, int64_t nq, int k,
                   uint32_t* out32, int64_t* out64, float* out_dist, const uint32_t* keep_bits = nullptr, int64_t n_bits = 0);

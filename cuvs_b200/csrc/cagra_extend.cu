@@ -282,11 +282,9 @@ static void extend_chunk(resources* r, cagra_index& g, int64_t n0, int64_t nc, u
     dbuf<unsigned char> rows(static_cast<size_t>(nc) * g.dim * es, s);
     B2_CUDA(cudaMemcpy2DAsync(rows.data(), es * g.dim, static_cast<const unsigned char*>(g.data) + static_cast<size_t>(n0) * g.ld * es, es * g.ld,
                               es * g.dim, nc, cudaMemcpyDeviceToDevice, s));
-    int64_t shape[2] = {nc, g.dim};
-    DLTensor q{};
-    q.data = rows.data(); q.device = DLDevice{kDLCUDA, r->device}; q.ndim = 2; q.dtype = g.dtype; q.shape = shape;
-    f32_matrix wq;
-    widen_to_f32(r, q, wq);
+    const dl_view q(rows.data(), DLDevice{kDLCUDA, r->device}, g.dtype, nc, g.dim);
+    f32_rows wq;
+    widen_to_f32(r, q.t(), wq);
     search_params_guard sp;
     B2_EXPECTS(cuvsCagraSearchParamsCreate(&sp.p) == CUVS_SUCCESS, "cagra extend: search parameters");
     sp.p->itopk_size   = std::max<size_t>(2 * static_cast<size_t>(B), 256);
@@ -348,7 +346,7 @@ static void extend_chunk(resources* r, cagra_index& g, int64_t n0, int64_t nc, u
 
 static void cagra_extend(resources* r, const cuvsCagraExtendParams& ep, const DLTensor& add, cuvsCagraIndex_t index)
 {
-  auto& idx = cagra_of(index);
+  auto& idx = index_of<cagra_index>(index);
   B2_EXPECTS(dl_is_dataset_dtype(add), "Unsupported dataset DLtensor dtype: %d and bits: %d", add.dtype.code, add.dtype.bits);
   B2_EXPECTS(add.dtype.code == idx.dtype.code && add.dtype.bits == idx.dtype.bits, "type mismatch between index and additional dataset");
   B2_EXPECTS(add.ndim == 2 && dl_is_c_contiguous(add), "additional dataset must be a row-major 2-D tensor");
@@ -400,8 +398,7 @@ static void cagra_extend(resources* r, const cuvsCagraExtendParams& ep, const DL
               static_cast<uint32_t>(e[1]), d);
   }
   B2_CUDA(cudaStreamSynchronize(s));
-  delete reinterpret_cast<cagra_index*>(index->addr);
-  index->addr = reinterpret_cast<uintptr_t>(g.release());
+  set_index(index, g.release(), index->dtype);
 }
 
 }  // namespace b200

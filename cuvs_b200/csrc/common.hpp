@@ -18,6 +18,7 @@
 
 #include <cuvs/core/c_api.h>
 #include <cuvs/distance/distance.h>
+#include <cuvs/neighbors/common.h>
 
 namespace b200 {
 
@@ -190,16 +191,34 @@ inline T* dl_ptr(const DLTensor& t)
 {
   return reinterpret_cast<T*>(t.data);
 }
-inline const DLTensor& dl_req(DLManagedTensor* m, const char* name)
-{
-  B2_EXPECTS(m != nullptr && m->dl_tensor.data != nullptr || (m != nullptr && m->dl_tensor.ndim > 0 &&
-             m->dl_tensor.shape != nullptr), "%s tensor is null", name);
-  return m->dl_tensor;
-}
-inline void dl_expect_matrix(const DLTensor& t, const char* name)
-{
-  B2_EXPECTS(t.ndim == 2, "%s must be a 2-D tensor (got ndim=%d)", name, t.ndim);
-}
+
+/** A non-owning row-major view of `rows` x `cols` (or, 1-D, `rows`) elements at `data`: how the library hands its own
+ *  buffers to its C entry points. */
+struct dl_view {
+  DLManagedTensor m{};
+  int64_t shape[2];
+  dl_view(const void* data, DLDevice dev, DLDataType dt, int64_t rows, int64_t cols) : dl_view(data, dev, dt, 2, rows, cols) {}
+  dl_view(const void* data, DLDevice dev, DLDataType dt, int64_t rows) : dl_view(data, dev, dt, 1, rows, 1) {}
+  dl_view(const dl_view&) = delete;  // the tensor's shape points into this object
+  const DLTensor& t() const { return m.dl_tensor; }
+
+ private:
+  dl_view(const void* data, DLDevice dev, DLDataType dt, int ndim, int64_t rows, int64_t cols) : shape{rows, cols}
+  {
+    m.dl_tensor.data   = const_cast<void*>(data);
+    m.dl_tensor.device = dev;
+    m.dl_tensor.ndim   = ndim;
+    m.dl_tensor.dtype  = dt;
+    m.dl_tensor.shape  = shape;
+  }
+};
+
+/** The queries / neighbors / distances checks every search entry point shares (the reference's from_dlpack of
+ *  device_matrix_views, c/src/neighbors/*.cpp): all three device-accessible and 2-D, neighbors int64 (or, where
+ *  `uint32_neighbors` is set, uint32), distances float32, both row-major and of one shape with a row per query, and queries
+ *  `dim` wide.  The queries' element type and layout are each index's own policy and are checked by its caller. */
+void check_search_tensors(const DLTensor& queries, const DLTensor& neighbors, const DLTensor& distances, int64_t dim,
+                          bool uint32_neighbors);
 
 /** Rows [r0, r0 + rows) of a C-contiguous 2-D tensor as a non-owning view (query batching inside the searches). */
 struct dl_row_slice {
@@ -221,29 +240,67 @@ struct dl_row_slice {
 /**
  * fp32 view of a dataset / query matrix given as float32, float16, int8 or uint8 — the element types the reference's C ABI
  * dispatches on (c/src/neighbors/ivf_pq.cpp:80-103, ivf_flat.cpp, brute_force.cpp:60-110, cagra.cpp:245-264).  float32
- * passes through untouched; the narrower types are widened into an owned device buffer (host sources are staged), values
+ * passes through untouched; the narrower types are widened into `Buf` on the device (host sources are staged), values
  * unchanged — the reference maps int8 / uint8 through utils::mapping<float> and scales the distances back
  * (ivf_pq_search.cuh:1043), which is the same arithmetic in different units.  The kernels then run on fp32, except the CAGRA
  * walk, which keeps and reads dataset rows in the type they were given in (only its query batch comes through here).
+ *
+ * Builds widen into `owned` memory (f32_matrix), which the index may keep.  Queries and extend chunks widen into a
+ * stream-ordered `dbuf` (f32_rows): a search must not cudaFree, which waits for every stream on the device.
  */
-struct f32_matrix {
+template <typename Buf>
+struct f32_widened {
   DLTensor t{};
   int64_t shape[2] = {0, 0};
-  owned<float> own;      // non-empty when the source was widened
-  bool widened = false;
-  f32_matrix() = default;
-  f32_matrix(const f32_matrix&) = delete;
+  Buf own;  // non-empty when the source was widened
+  f32_widened() = default;
+  f32_widened(const f32_widened&) = delete;
 };
+using f32_matrix = f32_widened<owned<float>>;
+using f32_rows   = f32_widened<dbuf<float>>;
 inline bool dl_is_dataset_dtype(const DLTensor& t)
 {
   return dl_is(t, kDLFloat, 32) || dl_is(t, kDLFloat, 16) || dl_is(t, kDLInt, 8) || dl_is(t, kDLUInt, 8);
 }
 void widen_to_f32(struct resources* res, const DLTensor& src, f32_matrix& out);
+void widen_to_f32(struct resources* res, const DLTensor& src, f32_rows& out);
 /** out[i] = float(in[i]) for `count` device elements of type `dt` (float16, int8 or uint8), stream-ordered. */
 void widen_async(cudaStream_t s, const void* in, DLDataType dt, int64_t count, float* out);
 
 /** Fill a caller-provided DLManagedTensor as a non-owning row-major view (used by index getters). */
 void dl_fill_view(DLManagedTensor* out, void* data, int device, DLDataType dt, int ndim, const int64_t* shape);
+
+struct filter_view {
+  const uint32_t* bits = nullptr;  // 1 = keep
+  int kind             = 0;        // 0 none, 1 bitset (per sample), 2 bitmap (per query x sample)
+  int64_t n_samples    = 0;
+};
+
+/** A search's pre-filter: none, a bitset or, where `bitmap_ok`, a bitmap, each a device-accessible 1-D uint32 tensor as the
+ *  reference's from_dlpack<device_vector_view<uint32_t>> requires.  n_samples is the tensor's bit count.  Any other filter
+ *  type fails with `unsupported`. */
+filter_view read_prefilter(cuvsFilter filter, bool bitmap_ok, const char* unsupported);
+
+/** The index object behind a C index handle (a struct of `uintptr_t addr` and `DLDataType dtype`). */
+template <typename T, typename Handle>
+T& index_of(Handle* handle)
+{
+  B2_EXPECTS(handle != nullptr && handle->addr != 0, "index is not built");
+  return *reinterpret_cast<T*>(handle->addr);
+}
+/** Deletes the handle's index object, if any, and stores `idx` (null: none) with the element type `dtype`. */
+template <typename T, typename Handle>
+void set_index(Handle* handle, T* idx, DLDataType dtype)
+{
+  delete reinterpret_cast<T*>(handle->addr);
+  handle->addr  = reinterpret_cast<uintptr_t>(idx);
+  handle->dtype = dtype;
+}
+template <typename T, typename Handle>
+void drop_index(Handle* handle)
+{
+  set_index<T>(handle, nullptr, handle->dtype);
+}
 
 inline bool metric_is_min_close(cuvsDistanceType m) { return m != InnerProduct; }
 inline bool is_l2(cuvsDistanceType m) { return m == L2Expanded || m == L2SqrtExpanded || m == L2Unexpanded || m == L2SqrtUnexpanded; }

@@ -11,6 +11,8 @@
 
 #include <cuvs/distance/distance.h>
 
+#include "common.hpp"  // filter_view
+
 namespace b200 {
 
 /** out[i] = sum_k x[i,k]^2 (ascending k, fmaf). */
@@ -22,12 +24,6 @@ void rsqrt_rows(cudaStream_t stream, const float* xn, int64_t n, float* out);
 
 /** x[i, :d] *= 1 / |x_i| in place (row_norms + rsqrt_rows, then one fp32 multiply per element); zero rows stay zero. */
 void normalize_rows(cudaStream_t stream, float* x, int64_t n, int d, int64_t ld);
-
-struct filter_view {
-  const uint32_t* bits = nullptr;  // 1 = keep
-  int kind             = 0;        // 0 none, 1 bitset (per sample), 2 bitmap (per query x sample)
-  int64_t n_samples    = 0;
-};
 
 /**
  * Dense distance tile: out[i, j] = dist(q_i, x_j) for i < nq, j < n, in the metric's *selection*

@@ -822,8 +822,6 @@ void ivf_flat_search(resources* res, const ivf_flat_index& idx, uint32_t n_probe
   auto s           = res->stream;
   const int64_t nq = qt.shape[0];
   const int k      = static_cast<int>(nt.shape[1]);
-  B2_EXPECTS(qt.shape[1] == idx.dim, "queries dim (%lld) != index dim (%d)", (long long)qt.shape[1], idx.dim);
-  B2_EXPECTS(nt.shape[0] == nq && dt.shape[0] == nq && dt.shape[1] == k, "neighbors/distances shape mismatch");
   B2_EXPECTS(k >= 1 && k <= kSelectMaxK, "ivf_flat search: k must be in [1, %d] (got %d)", kSelectMaxK, k);
   B2_EXPECTS(n_probes >= 1, "n_probes must be >= 1");
   if (nq == 0) return;
@@ -1037,26 +1035,20 @@ cuvsError_t cuvsIvfFlatIndexDestroy(cuvsIvfFlatIndex_t index)
 {
   return guarded([=] {
     if (!index) return;
-    delete reinterpret_cast<ivf_flat_index*>(index->addr);
+    drop_index<ivf_flat_index>(index);
     delete index;
   });
 }
 
-static ivf_flat_index& flat_of(cuvsIvfFlatIndex_t index)
-{
-  B2_EXPECTS(index != nullptr && index->addr != 0, "index is not built");
-  return *reinterpret_cast<ivf_flat_index*>(index->addr);
-}
-
 cuvsError_t cuvsIvfFlatIndexGetNLists(cuvsIvfFlatIndex_t index, int64_t* n_lists)
 {
-  return guarded([=] { *n_lists = flat_of(index).n_lists; });
+  return guarded([=] { *n_lists = index_of<ivf_flat_index>(index).n_lists; });
 }
-cuvsError_t cuvsIvfFlatIndexGetDim(cuvsIvfFlatIndex_t index, int64_t* dim) { return guarded([=] { *dim = flat_of(index).dim; }); }
+cuvsError_t cuvsIvfFlatIndexGetDim(cuvsIvfFlatIndex_t index, int64_t* dim) { return guarded([=] { *dim = index_of<ivf_flat_index>(index).dim; }); }
 cuvsError_t cuvsIvfFlatIndexGetCenters(cuvsIvfFlatIndex_t index, DLManagedTensor* centers)
 {
   return guarded([=] {
-    auto& idx        = flat_of(index);
+    auto& idx        = index_of<ivf_flat_index>(index);
     int64_t shape[2] = {idx.n_lists, idx.dim};
     dl_fill_view(centers, idx.centers.data(), idx.device, DLDataType{kDLFloat, 32, 1}, 2, shape);
   });
@@ -1065,7 +1057,7 @@ cuvsError_t cuvsIvfFlatIndexGetCenters(cuvsIvfFlatIndex_t index, DLManagedTensor
 cuvsError_t cuvsB200IvfFlatGetListSizes(cuvsIvfFlatIndex_t index, DLManagedTensor* list_sizes)
 {
   return guarded([=] {
-    auto& idx        = flat_of(index);
+    auto& idx        = index_of<ivf_flat_index>(index);
     int64_t shape[1] = {idx.n_lists};
     dl_fill_view(list_sizes, idx.lists.d_sizes.data(), idx.device, DLDataType{kDLUInt, 32, 1}, 1, shape);
   });
@@ -1073,7 +1065,7 @@ cuvsError_t cuvsB200IvfFlatGetListSizes(cuvsIvfFlatIndex_t index, DLManagedTenso
 cuvsError_t cuvsB200IvfFlatGetListIndices(cuvsIvfFlatIndex_t index, uint32_t label, DLManagedTensor* ids)
 {
   return guarded([=] {
-    auto& idx = flat_of(index);
+    auto& idx = index_of<ivf_flat_index>(index);
     B2_EXPECTS(label < idx.n_lists, "label %u out of range", label);
     int64_t shape[1] = {idx.lists.h_sizes[label]};
     dl_fill_view(ids, idx.ids.data() + idx.lists.h_offsets[label], idx.device, DLDataType{kDLInt, 64, 1}, 1, shape);
@@ -1083,7 +1075,7 @@ cuvsError_t cuvsB200IvfFlatSetCenters(cuvsResources_t res, cuvsIvfFlatIndex_t in
 {
   return guarded([=] {
     auto r    = as_res(res);
-    auto& idx = flat_of(index);
+    auto& idx = index_of<ivf_flat_index>(index);
     B2_EXPECTS(centers != nullptr, "centers is null");
     const DLTensor& c = centers->dl_tensor;
     B2_EXPECTS(dl_is(c, kDLFloat, 32) && c.ndim == 2 && c.shape[0] == idx.n_lists && c.shape[1] == idx.dim && dl_is_c_contiguous(c),
@@ -1093,14 +1085,14 @@ cuvsError_t cuvsB200IvfFlatSetCenters(cuvsResources_t res, cuvsIvfFlatIndex_t in
     refresh_centers_tc(r, idx);
   });
 }
-cuvsError_t cuvsB200IvfFlatGetSize(cuvsIvfFlatIndex_t index, int64_t* size) { return guarded([=] { *size = flat_of(index).lists.size; }); }
+cuvsError_t cuvsB200IvfFlatGetSize(cuvsIvfFlatIndex_t index, int64_t* size) { return guarded([=] { *size = index_of<ivf_flat_index>(index).lists.size; }); }
 
 cuvsError_t cuvsB200IvfFlatCandidates(cuvsResources_t res, cuvsIvfFlatIndex_t index, uint32_t n_probes, int k, DLManagedTensor* queries,
                                       DLManagedTensor* cand_ids, DLManagedTensor* cand_dist, DLManagedTensor* bound)
 {
   return guarded([=] {
     auto r    = as_res(res);
-    auto& idx = flat_of(index);
+    auto& idx = index_of<ivf_flat_index>(index);
     B2_EXPECTS(queries && cand_ids && cand_dist && bound, "null argument");
     const DLTensor& q  = queries->dl_tensor;
     const DLTensor& ci = cand_ids->dl_tensor;
@@ -1118,12 +1110,9 @@ cuvsError_t cuvsB200IvfFlatCandidates(cuvsResources_t res, cuvsIvfFlatIndex_t in
     B2_EXPECTS(static_cast<int64_t>(std::min(n_probes, idx.n_lists)) * 2 * (k + k / 2 <= 16 ? 16 : 32) >= kc2, "n_probes too small for kc2");
     dbuf<int64_t> ni(static_cast<size_t>(nq) * k, r->stream);
     dbuf<float> nd(static_cast<size_t>(nq) * k, r->stream);
-    int64_t shape[2] = {nq, k};
-    DLTensor nt{}, dt{};
-    nt.data = ni.data(); nt.device = q.device; nt.ndim = 2; nt.dtype = DLDataType{kDLInt, 64, 1}; nt.shape = shape;
-    dt.data = nd.data(); dt.device = q.device; dt.ndim = 2; dt.dtype = DLDataType{kDLFloat, 32, 1}; dt.shape = shape;
+    const dl_view nt(ni.data(), q.device, DLDataType{kDLInt, 64, 1}, nq, k), dt(nd.data(), q.device, DLDataType{kDLFloat, 32, 1}, nq, k);
     flat_candidates c{dl_ptr<int64_t>(ci), dl_ptr<float>(cd), dl_ptr<float>(b)};
-    ivf_flat_search(r, idx, n_probes, q, nt, dt, nullptr, 0, &c);
+    ivf_flat_search(r, idx, n_probes, q, nt.t(), dt.t(), nullptr, 0, &c);
   });
 }
 
@@ -1134,17 +1123,16 @@ cuvsError_t cuvsIvfFlatBuild(cuvsResources_t res, cuvsIvfFlatIndexParams_t param
     B2_EXPECTS(params && dataset && index, "null argument");
     const DLTensor& ds = dataset->dl_tensor;
     B2_EXPECTS(dl_is_dataset_dtype(ds), "Unsupported dataset DLtensor dtype: %d and bits: %d", ds.dtype.code, ds.dtype.bits);
-    if (index->addr) { delete reinterpret_cast<ivf_flat_index*>(index->addr); index->addr = 0; }
+    drop_index<ivf_flat_index>(index);
     // int8 / uint8 datasets in L2 or inner product keep their type; float16 ones, and 8-bit ones for cosine, are widened to fp32
     // rows (c/src/neighbors/ivf_flat.cpp dtype switch)
     if (row_type_for(ds.dtype, params->metric) != kRowF32) {
-      index->addr = reinterpret_cast<uintptr_t>(ivf_flat_build(r, *params, ds));
+      set_index(index, ivf_flat_build(r, *params, ds), ds.dtype);
     } else {
       f32_matrix w;
       widen_to_f32(r, ds, w);
-      index->addr = reinterpret_cast<uintptr_t>(ivf_flat_build(r, *params, w.t));
+      set_index(index, ivf_flat_build(r, *params, w.t), ds.dtype);
     }
-    index->dtype = ds.dtype;
   });
 }
 
@@ -1154,38 +1142,17 @@ cuvsError_t cuvsIvfFlatSearch(cuvsResources_t res, cuvsIvfFlatSearchParams_t par
   return guarded([=] {
     auto r = as_res(res);
     B2_EXPECTS(params && queries_t && neighbors_t && distances_t, "null argument");
-    auto& idx = flat_of(index);
+    auto& idx = index_of<ivf_flat_index>(index);
     const DLTensor& queries   = queries_t->dl_tensor;
     const DLTensor& neighbors = neighbors_t->dl_tensor;
     const DLTensor& distances = distances_t->dl_tensor;
-    B2_EXPECTS(dl_is_device(queries), "queries should have device compatible memory");
-    B2_EXPECTS(dl_is_device(neighbors), "neighbors should have device compatible memory");
-    B2_EXPECTS(dl_is_device(distances), "distances should have device compatible memory");
-    B2_EXPECTS(dl_is(neighbors, kDLInt, 64), "neighbors should be of type int64_t");
-    B2_EXPECTS(dl_is(distances, kDLFloat, 32), "distances should be of type float32");
+    check_search_tensors(queries, neighbors, distances, idx.dim, false);
     B2_EXPECTS(queries.dtype.code == index->dtype.code && queries.dtype.bits == index->dtype.bits, "type mismatch between index and queries");
-    B2_EXPECTS(queries.ndim == 2 && neighbors.ndim == 2 && distances.ndim == 2, "queries/neighbors/distances must be 2-D");
-    B2_EXPECTS(dl_is_c_contiguous(queries) && dl_is_c_contiguous(neighbors) && dl_is_c_contiguous(distances), "tensors must be row-major contiguous");
-    const uint32_t* keep = nullptr;
-    int64_t n_bits       = 0;
-    if (filter.type != NO_FILTER) {
-      B2_EXPECTS(filter.type == BITSET, "ivf_flat search: only bitset pre-filters are supported (as in the reference)");
-      auto ft = reinterpret_cast<DLManagedTensor*>(filter.addr);
-      B2_EXPECTS(ft != nullptr && dl_is_device(ft->dl_tensor), "prefilter should have device compatible memory");
-      keep   = dl_ptr<uint32_t>(ft->dl_tensor);
-      n_bits = ft->dl_tensor.shape[0] * 32;
-    }
-    // narrower queries are widened into stream-ordered memory: no device-wide synchronisation per search
-    B2_EXPECTS(dl_is_dataset_dtype(queries), "Unsupported queries DLtensor dtype: %d and bits: %d", queries.dtype.code, queries.dtype.bits);
-    DLTensor qv = queries;
-    dbuf<float> qw;
-    if (!dl_is(queries, kDLFloat, 32)) {
-      qw.alloc(static_cast<size_t>(std::max<int64_t>(queries.shape[0] * queries.shape[1], 1)), r->stream);
-      widen_async(r->stream, dl_ptr<void>(queries), queries.dtype, queries.shape[0] * queries.shape[1], qw.data());
-      qv.data  = qw.data();
-      qv.dtype = DLDataType{kDLFloat, 32, 1};
-    }
-    ivf_flat_search(r, idx, params->n_probes, qv, neighbors, distances, keep, n_bits);
+    B2_EXPECTS(dl_is_c_contiguous(queries), "queries must be row-major contiguous");
+    const filter_view filt = read_prefilter(filter, false, "ivf_flat search: only bitset pre-filters are supported (as in the reference)");
+    f32_rows qv;
+    widen_to_f32(r, queries, qv);
+    ivf_flat_search(r, idx, params->n_probes, qv.t, neighbors, distances, filt.bits, filt.n_samples);
   });
 }
 
@@ -1193,11 +1160,11 @@ cuvsError_t cuvsIvfFlatExtend(cuvsResources_t res, DLManagedTensor* new_vectors,
 {
   return guarded([=] {
     auto r    = as_res(res);
-    auto& idx = flat_of(index);
+    auto& idx = index_of<ivf_flat_index>(index);
     B2_EXPECTS(new_vectors != nullptr, "new_vectors is null");
     B2_EXPECTS(dl_is_dataset_dtype(new_vectors->dl_tensor), "Unsupported new_vectors DLtensor dtype: %d and bits: %d",
                new_vectors->dl_tensor.dtype.code, new_vectors->dl_tensor.dtype.bits);
-    f32_matrix wv;
+    f32_rows wv;
     if (idx.row_type != kRowF32) {  // 8-bit lists take rows of their own type
       const DLTensor& nv = new_vectors->dl_tensor;
       B2_EXPECTS(nv.dtype.code == index->dtype.code && nv.dtype.bits == 8, "type mismatch between index and new_vectors");
@@ -1225,27 +1192,6 @@ cuvsError_t cuvsIvfFlatExtend(cuvsResources_t res, DLManagedTensor* new_vectors,
 //   indices i8 [capacity] (-1 = kInvalidRecord on the padding rows).
 namespace {
 
-// an index file's element type: its tag, the descr of its data records and the element size
-struct flat_file_type {
-  const char* tag;
-  const char* descr;
-  int size;
-};
-flat_file_type flat_file_type_of(DLDataType t)
-{
-  if (t.code == kDLFloat) return t.bits == 32 ? flat_file_type{"<f4", "<f4", 4} : flat_file_type{"<e2", "<f2", 2};
-  return t.code == kDLInt ? flat_file_type{"|i1", "|i1", 1} : flat_file_type{"|u1", "|u1", 1};
-}
-// the type a tag or a data record names by its kind and size (float16 is kind 'e' to the reference and 'f' to NumPy); bits 0:
-// none of the four
-DLDataType flat_dtype_of(char kind, int size)
-{
-  if (kind == 'f' && size == 4) return DLDataType{kDLFloat, 32, 1};
-  if ((kind == 'e' || kind == 'f') && size == 2) return DLDataType{kDLFloat, 16, 1};
-  if (kind == 'i' && size == 1) return DLDataType{kDLInt, 8, 1};
-  if (kind == 'u' && size == 1) return DLDataType{kDLUInt, 8, 1};
-  return DLDataType{kDLFloat, 0, 1};
-}
 inline int flat_veclen(int dim, int size) { return dim % (16 / size) == 0 ? 16 / size : 1; }
 inline int64_t interleaved_at(int64_t r, int k, int dim, int vl) { return (r / 32) * 32 * dim + (k / vl) * 32 * vl + (r % 32) * vl + k % vl; }
 
@@ -1269,10 +1215,10 @@ cuvsError_t cuvsIvfFlatSerialize(cuvsResources_t res, const char* filename, cuvs
 {
   return guarded([=] {
     auto r    = as_res(res);
-    auto& idx = flat_of(index);
+    auto& idx = index_of<ivf_flat_index>(index);
     std::ofstream os(filename, std::ios::out | std::ios::binary);
     B2_EXPECTS(bool(os), "Cannot open file %s", filename);
-    const flat_file_type ft = flat_file_type_of(index->dtype);
+    const npy::file_dtype& ft = npy::file_dtype_for(index->dtype);
     os.write(ft.tag, 4);  // three characters and the terminating zero
     npy::write_scalar<int32_t>(os, 4);
     npy::write_scalar<int64_t>(os, idx.lists.size);
@@ -1342,9 +1288,9 @@ cuvsError_t cuvsIvfFlatDeserialize(cuvsResources_t res, const char* filename, cu
     B2_EXPECTS(bool(is), "Cannot open file %s", filename);
     char tag[4]{};
     B2_EXPECTS(bool(is.read(tag, 4)), "ivf_flat::deserialize: failed to read dtype prefix");
-    const DLDataType dtype = flat_dtype_of(tag[1], tag[2] - '0');
-    B2_EXPECTS(dtype.bits != 0 && (tag[0] == '<' || tag[0] == '|' || tag[0] == '='),
-               "ivf_flat::deserialize: unsupported dtype prefix '%.3s' in the index file", tag);
+    const npy::file_dtype* ft = npy::file_dtype_named(std::string(tag, 3));
+    B2_EXPECTS(ft != nullptr, "ivf_flat::deserialize: unsupported dtype prefix '%.3s' in the index file", tag);
+    const DLDataType dtype = ft->dl;
     const int ver = npy::read_scalar<int32_t>(is, filename);
     B2_EXPECTS(ver == 4, "serialization version mismatch, expected %d, got %d ", 4, ver);
     const int64_t n_rows = npy::read_scalar<int64_t>(is, filename);
@@ -1386,8 +1332,7 @@ cuvsError_t cuvsIvfFlatDeserialize(cuvsResources_t res, const char* filename, cu
       B2_EXPECTS(cap >= sz, "ivf_flat::deserialize: list %u stores %lld rows, list_sizes says %lld", l, (long long)cap, (long long)sz);
       if (!cap) continue;
       const npy::header h = npy::read_header(is, filename);
-      const DLDataType rt = flat_dtype_of(h.descr.size() >= 3 ? h.descr[1] : '?', h.item_size());
-      B2_EXPECTS(rt.code == dtype.code && rt.bits == dtype.bits && !h.fortran && h.count() == cap * dim,
+      B2_EXPECTS(npy::file_dtype_named(h.descr) == ft && !h.fortran && h.count() == cap * dim,
                  "ivf_flat::deserialize: list %u holds %lld elements of '%s', the file's type '%.3s' needs %lld", l, (long long)h.count(),
                  h.descr.c_str(), tag, (long long)(cap * dim));
       inter.resize(static_cast<size_t>(cap) * dim * es);
@@ -1412,9 +1357,7 @@ cuvsError_t cuvsIvfFlatDeserialize(cuvsResources_t res, const char* filename, cu
       B2_CUDA(cudaStreamSynchronize(r->stream));
     }
     refresh_rows(r, *idx);
-    if (index->addr) delete reinterpret_cast<ivf_flat_index*>(index->addr);
-    index->addr  = reinterpret_cast<uintptr_t>(idx.release());
-    index->dtype = dtype;
+    set_index(index, idx.release(), dtype);
   });
 }
 

@@ -919,8 +919,6 @@ void ivf_pq_search(resources* res, const ivf_pq_index& idx, const cuvsIvfPqSearc
   auto s           = res->stream;
   const int64_t nq = qt.shape[0];
   const int k      = static_cast<int>(nt.shape[1]);
-  B2_EXPECTS(qt.shape[1] == idx.dim, "queries dim (%lld) != index dim (%d)", (long long)qt.shape[1], idx.dim);
-  B2_EXPECTS(nt.shape[0] == nq && dt.shape[0] == nq && dt.shape[1] == k, "neighbors/distances shape mismatch");
   B2_EXPECTS(k >= 1 && k <= kSelectMaxK, "ivf_pq search: k must be in [1, %d] (got %d)", kSelectMaxK, k);
   B2_EXPECTS(sp.n_probes >= 1, "n_probes must be >= 1");
   B2_EXPECTS(sp.lut_dtype == CUDA_R_32F || sp.lut_dtype == CUDA_R_16F || sp.lut_dtype == CUDA_R_8U, "unsupported lut_dtype");
@@ -1040,12 +1038,6 @@ void ivf_pq_search(resources* res, const ivf_pq_index& idx, const cuvsIvfPqSearc
 
 using namespace b200;
 
-static ivf_pq_index& pq_of(cuvsIvfPqIndex_t index)
-{
-  B2_EXPECTS(index != nullptr && index->addr != 0, "index is not built");
-  return *reinterpret_cast<ivf_pq_index*>(index->addr);
-}
-
 extern "C" {
 
 cuvsError_t cuvsIvfPqIndexParamsCreate(cuvsIvfPqIndexParams_t* params)
@@ -1079,7 +1071,7 @@ cuvsError_t cuvsIvfPqIndexDestroy(cuvsIvfPqIndex_t index)
 {
   return guarded([=] {
     if (!index) return;
-    delete reinterpret_cast<ivf_pq_index*>(index->addr);
+    drop_index<ivf_pq_index>(index);
     delete index;
   });
 }
@@ -1096,7 +1088,7 @@ int64_t cuvsB200IvfPqPrimedBounds(float* out, int64_t cap)
 cuvsError_t cuvsB200IvfPqIndexInfo(cuvsIvfPqIndex_t index, int* path, int64_t* device_bytes)
 {
   return guarded([=] {
-    const ivf_pq_index& idx = pq_of(index);
+    const ivf_pq_index& idx = index_of<ivf_pq_index>(index);
     if (path) *path = (idx.cstream.data() ? 2 : 0) | (idx.yhat.data() ? 1 : 0);
     if (device_bytes)
       *device_bytes = static_cast<int64_t>(idx.codes.size() + idx.ids.size() * 8 + idx.cstream.size() + idx.cb_words.size() * 4 +
@@ -1106,17 +1098,17 @@ cuvsError_t cuvsB200IvfPqIndexInfo(cuvsIvfPqIndex_t index, int* path, int64_t* d
   });
 }
 
-cuvsError_t cuvsIvfPqIndexGetNLists(cuvsIvfPqIndex_t index, int64_t* v) { return guarded([=] { *v = pq_of(index).n_lists; }); }
-cuvsError_t cuvsIvfPqIndexGetDim(cuvsIvfPqIndex_t index, int64_t* v) { return guarded([=] { *v = pq_of(index).dim; }); }
-cuvsError_t cuvsIvfPqIndexGetSize(cuvsIvfPqIndex_t index, int64_t* v) { return guarded([=] { *v = pq_of(index).lists.size; }); }
-cuvsError_t cuvsIvfPqIndexGetPqDim(cuvsIvfPqIndex_t index, int64_t* v) { return guarded([=] { *v = pq_of(index).pq_dim; }); }
-cuvsError_t cuvsIvfPqIndexGetPqBits(cuvsIvfPqIndex_t index, int64_t* v) { return guarded([=] { *v = pq_of(index).pq_bits; }); }
-cuvsError_t cuvsIvfPqIndexGetPqLen(cuvsIvfPqIndex_t index, int64_t* v) { return guarded([=] { *v = pq_of(index).pq_len; }); }
+cuvsError_t cuvsIvfPqIndexGetNLists(cuvsIvfPqIndex_t index, int64_t* v) { return guarded([=] { *v = index_of<ivf_pq_index>(index).n_lists; }); }
+cuvsError_t cuvsIvfPqIndexGetDim(cuvsIvfPqIndex_t index, int64_t* v) { return guarded([=] { *v = index_of<ivf_pq_index>(index).dim; }); }
+cuvsError_t cuvsIvfPqIndexGetSize(cuvsIvfPqIndex_t index, int64_t* v) { return guarded([=] { *v = index_of<ivf_pq_index>(index).lists.size; }); }
+cuvsError_t cuvsIvfPqIndexGetPqDim(cuvsIvfPqIndex_t index, int64_t* v) { return guarded([=] { *v = index_of<ivf_pq_index>(index).pq_dim; }); }
+cuvsError_t cuvsIvfPqIndexGetPqBits(cuvsIvfPqIndex_t index, int64_t* v) { return guarded([=] { *v = index_of<ivf_pq_index>(index).pq_bits; }); }
+cuvsError_t cuvsIvfPqIndexGetPqLen(cuvsIvfPqIndex_t index, int64_t* v) { return guarded([=] { *v = index_of<ivf_pq_index>(index).pq_len; }); }
 
 cuvsError_t cuvsIvfPqIndexGetCenters(cuvsIvfPqIndex_t index, DLManagedTensor* centers)
 {
   return guarded([=] {
-    auto& idx        = pq_of(index);
+    auto& idx        = index_of<ivf_pq_index>(index);
     int64_t shape[2] = {idx.n_lists, idx.dim};
     dl_fill_view(centers, idx.centers.data(), idx.device, DLDataType{kDLFloat, 32, 1}, 2, shape);
   });
@@ -1124,7 +1116,7 @@ cuvsError_t cuvsIvfPqIndexGetCenters(cuvsIvfPqIndex_t index, DLManagedTensor* ce
 cuvsError_t cuvsIvfPqIndexGetCentersPadded(cuvsIvfPqIndex_t index, DLManagedTensor* centers)
 {
   return guarded([=] {
-    auto& idx        = pq_of(index);
+    auto& idx        = index_of<ivf_pq_index>(index);
     int64_t shape[2] = {idx.n_lists, idx.dim_ext};
     dl_fill_view(centers, idx.centers_ext.data(), idx.device, DLDataType{kDLFloat, 32, 1}, 2, shape);
   });
@@ -1132,7 +1124,7 @@ cuvsError_t cuvsIvfPqIndexGetCentersPadded(cuvsIvfPqIndex_t index, DLManagedTens
 cuvsError_t cuvsIvfPqIndexGetPqCenters(cuvsIvfPqIndex_t index, DLManagedTensor* pq_centers)
 {
   return guarded([=] {
-    auto& idx        = pq_of(index);
+    auto& idx        = index_of<ivf_pq_index>(index);
     int64_t nb       = idx.codebook_kind == CUVS_IVF_PQ_CODEBOOK_GEN_PER_CLUSTER ? idx.n_lists : idx.pq_dim;
     int64_t shape[3] = {nb, idx.pq_len, idx.book()};
     dl_fill_view(pq_centers, idx.pq_centers.data(), idx.device, DLDataType{kDLFloat, 32, 1}, 3, shape);
@@ -1141,7 +1133,7 @@ cuvsError_t cuvsIvfPqIndexGetPqCenters(cuvsIvfPqIndex_t index, DLManagedTensor* 
 cuvsError_t cuvsIvfPqIndexGetCentersRot(cuvsIvfPqIndex_t index, DLManagedTensor* centers_rot)
 {
   return guarded([=] {
-    auto& idx        = pq_of(index);
+    auto& idx        = index_of<ivf_pq_index>(index);
     int64_t shape[2] = {idx.n_lists, idx.rot_dim};
     dl_fill_view(centers_rot, idx.centers_rot.data(), idx.device, DLDataType{kDLFloat, 32, 1}, 2, shape);
   });
@@ -1149,7 +1141,7 @@ cuvsError_t cuvsIvfPqIndexGetCentersRot(cuvsIvfPqIndex_t index, DLManagedTensor*
 cuvsError_t cuvsIvfPqIndexGetRotationMatrix(cuvsIvfPqIndex_t index, DLManagedTensor* rotation_matrix)
 {
   return guarded([=] {
-    auto& idx        = pq_of(index);
+    auto& idx        = index_of<ivf_pq_index>(index);
     int64_t shape[2] = {idx.rot_dim, idx.dim};
     dl_fill_view(rotation_matrix, idx.rotation.data(), idx.device, DLDataType{kDLFloat, 32, 1}, 2, shape);
   });
@@ -1157,7 +1149,7 @@ cuvsError_t cuvsIvfPqIndexGetRotationMatrix(cuvsIvfPqIndex_t index, DLManagedTen
 cuvsError_t cuvsIvfPqIndexGetListSizes(cuvsIvfPqIndex_t index, DLManagedTensor* list_sizes)
 {
   return guarded([=] {
-    auto& idx        = pq_of(index);
+    auto& idx        = index_of<ivf_pq_index>(index);
     int64_t shape[1] = {idx.n_lists};
     dl_fill_view(list_sizes, idx.lists.d_sizes.data(), idx.device, DLDataType{kDLUInt, 32, 1}, 1, shape);
   });
@@ -1183,7 +1175,7 @@ cuvsError_t cuvsIvfPqIndexUnpackContiguousListData(cuvsResources_t res, cuvsIvfP
 {
   return guarded([=] {
     auto r    = as_res(res);
-    const ivf_pq_index& idx = pq_of(index);
+    const ivf_pq_index& idx = index_of<ivf_pq_index>(index);
     B2_EXPECTS(label < idx.n_lists, "label %u out of range", label);
     const DLTensor& oc = out_codes->dl_tensor;
     B2_EXPECTS(dl_is(oc, kDLUInt, 8) && oc.ndim == 2 && dl_is_device(oc) && dl_is_c_contiguous(oc), "out_codes must be a device uint8 matrix");
@@ -1202,7 +1194,7 @@ cuvsError_t cuvsIvfPqIndexUnpackContiguousListData(cuvsResources_t res, cuvsIvfP
 cuvsError_t cuvsIvfPqIndexGetListIndices(cuvsIvfPqIndex_t index, uint32_t label, DLManagedTensor* out_labels)
 {
   return guarded([=] {
-    auto& idx = pq_of(index);
+    auto& idx = index_of<ivf_pq_index>(index);
     B2_EXPECTS(label < idx.n_lists, "label %u out of range", label);
     int64_t shape[1] = {idx.lists.h_sizes[label]};
     dl_fill_view(out_labels, idx.ids.data() + idx.lists.h_offsets[label], idx.device, DLDataType{kDLInt, 64, 1}, 1, shape);
@@ -1216,11 +1208,10 @@ cuvsError_t cuvsIvfPqBuild(cuvsResources_t res, cuvsIvfPqIndexParams_t params, D
     B2_EXPECTS(params && dataset && index, "null argument");
     const DLTensor& ds = dataset->dl_tensor;
     B2_EXPECTS(dl_is_dataset_dtype(ds), "Unsupported dataset DLtensor dtype: %d and bits: %d", ds.dtype.code, ds.dtype.bits);
-    if (index->addr) { delete reinterpret_cast<ivf_pq_index*>(index->addr); index->addr = 0; }
+    drop_index<ivf_pq_index>(index);
     f32_matrix w;  // float16 / int8 / uint8 datasets (c/src/neighbors/ivf_pq.cpp:80-103) are widened to fp32 rows
     widen_to_f32(r, ds, w);
-    index->addr  = reinterpret_cast<uintptr_t>(ivf_pq_build(r, *params, w.t));
-    index->dtype = ds.dtype;
+    set_index(index, ivf_pq_build(r, *params, w.t), ds.dtype);
   });
 }
 
@@ -1282,9 +1273,7 @@ cuvsError_t cuvsIvfPqBuildPrecomputed(cuvsResources_t res, cuvsIvfPqIndexParams_
     idx->codes.alloc(1);
     idx->ids.alloc(1);
     refresh_decoded(r, *idx);
-    if (index->addr) delete reinterpret_cast<ivf_pq_index*>(index->addr);
-    index->addr  = reinterpret_cast<uintptr_t>(idx.release());
-    index->dtype = DLDataType{kDLFloat, 32, 1};
+    set_index(index, idx.release(), DLDataType{kDLFloat, 32, 1});
   });
 }
 
@@ -1294,19 +1283,15 @@ cuvsError_t cuvsIvfPqSearch(cuvsResources_t res, cuvsIvfPqSearchParams_t params,
   return guarded([=] {
     auto r = as_res(res);
     B2_EXPECTS(params && queries_t && neighbors_t && distances_t, "null argument");
-    auto& idx = pq_of(index);
+    auto& idx = index_of<ivf_pq_index>(index);
     const DLTensor& queries   = queries_t->dl_tensor;
     const DLTensor& neighbors = neighbors_t->dl_tensor;
     const DLTensor& distances = distances_t->dl_tensor;
-    B2_EXPECTS(dl_is_device(queries), "queries should have device compatible memory");
-    B2_EXPECTS(dl_is_device(neighbors), "neighbors should have device compatible memory");
-    B2_EXPECTS(dl_is_device(distances), "distances should have device compatible memory");
-    B2_EXPECTS(dl_is(neighbors, kDLInt, 64), "neighbors should be of type int64_t");
-    B2_EXPECTS(dl_is(distances, kDLFloat, 32), "distances should be of type float32");
+    check_search_tensors(queries, neighbors, distances, idx.dim, false);
+    // any dataset type, whatever the index was built from (c/src/neighbors/ivf_pq.cpp:315-345 has no mismatch check)
     B2_EXPECTS(dl_is_dataset_dtype(queries), "Unsupported queries DLtensor dtype: %d and bits: %d", queries.dtype.code, queries.dtype.bits);
-    B2_EXPECTS(queries.ndim == 2 && neighbors.ndim == 2 && distances.ndim == 2, "queries/neighbors/distances must be 2-D");
-    B2_EXPECTS(dl_is_c_contiguous(queries) && dl_is_c_contiguous(neighbors) && dl_is_c_contiguous(distances), "tensors must be row-major contiguous");
-    f32_matrix w;
+    B2_EXPECTS(dl_is_c_contiguous(queries), "queries must be row-major contiguous");
+    f32_rows w;
     widen_to_f32(r, queries, w);
     ivf_pq_search(r, idx, *params, w.t, neighbors, distances);
   });
@@ -1316,11 +1301,11 @@ cuvsError_t cuvsIvfPqExtend(cuvsResources_t res, DLManagedTensor* new_vectors, D
 {
   return guarded([=] {
     auto r    = as_res(res);
-    auto& idx = pq_of(index);
+    auto& idx = index_of<ivf_pq_index>(index);
     B2_EXPECTS(new_vectors != nullptr, "new_vectors is null");
     B2_EXPECTS(dl_is_dataset_dtype(new_vectors->dl_tensor), "Unsupported new_vectors DLtensor dtype: %d and bits: %d",
                new_vectors->dl_tensor.dtype.code, new_vectors->dl_tensor.dtype.bits);
-    f32_matrix wv;
+    f32_rows wv;
     widen_to_f32(r, new_vectors->dl_tensor, wv);
     const DLTensor& v = wv.t;
     B2_EXPECTS(dl_is(v, kDLFloat, 32) && v.ndim == 2 && v.shape[1] == idx.dim && dl_is_c_contiguous(v), "new_vectors must be [n, dim] row-major");
@@ -1392,7 +1377,7 @@ cuvsError_t cuvsIvfPqSerialize(cuvsResources_t res, const char* filename, cuvsIv
 {
   return guarded([=] {
     auto r    = as_res(res);
-    const ivf_pq_index& idx = pq_of(index);
+    const ivf_pq_index& idx = index_of<ivf_pq_index>(index);
     std::ofstream os(filename, std::ios::out | std::ios::binary);
     B2_EXPECTS(bool(os), "Cannot open file %s", filename);
     npy::write_scalar<int32_t>(os, 4);
@@ -1520,9 +1505,7 @@ cuvsError_t cuvsIvfPqDeserialize(cuvsResources_t res, const char* filename, cuvs
       B2_CUDA(cudaStreamSynchronize(r->stream));
     }
     refresh_decoded(r, *idx);
-    if (index->addr) delete reinterpret_cast<ivf_pq_index*>(index->addr);
-    index->addr  = reinterpret_cast<uintptr_t>(idx.release());
-    index->dtype = DLDataType{kDLFloat, 32, 1};
+    set_index(index, idx.release(), DLDataType{kDLFloat, 32, 1});
   });
 }
 
@@ -1532,7 +1515,7 @@ cuvsError_t cuvsIvfPqTransform(cuvsResources_t res, cuvsIvfPqIndex_t index, DLMa
 {
   return guarded([=] {
     auto r    = as_res(res);
-    auto& idx = pq_of(index);
+    auto& idx = index_of<ivf_pq_index>(index);
     B2_EXPECTS(input_dataset && output_labels && output_dataset, "null argument");
     const DLTensor& x  = input_dataset->dl_tensor;
     const DLTensor& ol = output_labels->dl_tensor;

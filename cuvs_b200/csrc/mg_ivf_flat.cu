@@ -69,13 +69,6 @@ void check_c(cuvsError_t e, const char* what)
   }
 }
 
-DLManagedTensor make_dl(void* p, DLDeviceType dt, int dev, DLDataType ty, int ndim, int64_t* shape)
-{
-  DLManagedTensor m{};
-  m.dl_tensor.data = p; m.dl_tensor.device = DLDevice{dt, dev}; m.dl_tensor.ndim = ndim; m.dl_tensor.dtype = ty; m.dl_tensor.shape = shape;
-  return m;
-}
-
 }  // namespace
 }  // namespace b200
 
@@ -115,7 +108,7 @@ cuvsError_t cuvsMultiGpuIvfFlatIndexDestroy(cuvsMultiGpuIvfFlatIndex_t index)
 {
   return guarded([=] {
     if (!index) return;
-    delete reinterpret_cast<mg_index*>(index->addr);
+    drop_index<mg_index>(index);
     delete index;
   });
 }
@@ -156,9 +149,8 @@ cuvsError_t cuvsMultiGpuIvfFlatBuild(cuvsResources_t res, cuvsMultiGpuIvfFlatInd
       // REPLICATED (or a single device): the full index on every device
       for (int i = 0; i < nd; ++i) {
         device_guard g(mg->shards[i].device);
-        int64_t shape[2] = {n, d};
-        DLManagedTensor full = make_dl(const_cast<float*>(x), kDLCPU, 0, ds.dtype, 2, shape);
-        check_c(cuvsIvfFlatBuild(mg->shards[i].res, &p, &full, mg->shards[i].index), "cuvsIvfFlatBuild (replica)");
+        dl_view full(x, DLDevice{kDLCPU, 0}, ds.dtype, n, d);
+        check_c(cuvsIvfFlatBuild(mg->shards[i].res, &p, &full.m, mg->shards[i].index), "cuvsIvfFlatBuild (replica)");
       }
     } else {
       // SHARDED by IVF list.  (1) train the coarse centres once, on device 0, on the build's usual subsample.
@@ -167,9 +159,8 @@ cuvsError_t cuvsMultiGpuIvfFlatBuild(cuvsResources_t res, cuvsMultiGpuIvfFlatInd
       std::vector<float> centers(static_cast<size_t>(p.n_lists) * d);
       {
         device_guard g(mg->shards[0].device);
-        int64_t shape[2] = {n, d};
-        DLManagedTensor full = make_dl(const_cast<float*>(x), kDLCPU, 0, ds.dtype, 2, shape);
-        check_c(cuvsIvfFlatBuild(mg->shards[0].res, &p0, &full, mg->shards[0].index), "cuvsIvfFlatBuild (train)");
+        dl_view full(x, DLDevice{kDLCPU, 0}, ds.dtype, n, d);
+        check_c(cuvsIvfFlatBuild(mg->shards[0].res, &p0, &full.m, mg->shards[0].index), "cuvsIvfFlatBuild (train)");
         DLManagedTensor cv{};
         check_c(cuvsIvfFlatIndexGetCenters(mg->shards[0].index, &cv), "cuvsIvfFlatIndexGetCenters");
         B2_CUDA(cudaMemcpyAsync(centers.data(), cv.dl_tensor.data, centers.size() * sizeof(float), cudaMemcpyDeviceToHost, r->mg_streams[0]));
@@ -178,13 +169,12 @@ cuvsError_t cuvsMultiGpuIvfFlatBuild(cuvsResources_t res, cuvsMultiGpuIvfFlatInd
       // (2) every other device: an empty index with the SAME centres (bit-identical partition rule everywhere)
       for (int i = 1; i < nd; ++i) {
         device_guard g(mg->shards[i].device);
-        int64_t shape[2] = {static_cast<int64_t>(p.n_lists), d};
-        DLManagedTensor seed = make_dl(centers.data(), kDLCPU, 0, ds.dtype, 2, shape);
+        dl_view seed(centers.data(), DLDevice{kDLCPU, 0}, ds.dtype, p.n_lists, d);
         cuvsIvfFlatIndexParams pi = p0;
         pi.kmeans_n_iters           = 1;
         pi.kmeans_trainset_fraction = 1.0;
-        check_c(cuvsIvfFlatBuild(mg->shards[i].res, &pi, &seed, mg->shards[i].index), "cuvsIvfFlatBuild (empty shard)");
-        check_c(cuvsB200IvfFlatSetCenters(mg->shards[i].res, mg->shards[i].index, &seed), "cuvsB200IvfFlatSetCenters");
+        check_c(cuvsIvfFlatBuild(mg->shards[i].res, &pi, &seed.m, mg->shards[i].index), "cuvsIvfFlatBuild (empty shard)");
+        check_c(cuvsB200IvfFlatSetCenters(mg->shards[i].res, mg->shards[i].index, &seed.m), "cuvsB200IvfFlatSetCenters");
       }
       // (3) label the rows chunk by chunk on device 0 and route every row to the owner of its list (list % n_devices)
       //     with its GLOBAL row id
@@ -212,12 +202,11 @@ cuvsError_t cuvsMultiGpuIvfFlatBuild(cuvsResources_t res, cuvsMultiGpuIvfFlatInd
           device_guard g(mg->shards[0].device);
           auto st = r->mg_streams[0];
           B2_CUDA(cudaMemcpyAsync(d_x, x + r0 * d, sizeof(float) * rows * d, cudaMemcpyHostToDevice, st));
-          int64_t xs[2] = {rows, d}, cs[2] = {static_cast<int64_t>(p.n_lists), d}, ls[1] = {rows};
-          DLManagedTensor tx = make_dl(d_x, kDLCUDA, mg->shards[0].device, DLDataType{kDLFloat, 32, 1}, 2, xs);
-          DLManagedTensor tc = make_dl(d_c, kDLCUDA, mg->shards[0].device, DLDataType{kDLFloat, 32, 1}, 2, cs);
-          DLManagedTensor tl = make_dl(d_l, kDLCUDA, mg->shards[0].device, DLDataType{kDLInt, 32, 1}, 1, ls);
+          const DLDevice dev{kDLCUDA, mg->shards[0].device};
+          dl_view tx(d_x, dev, DLDataType{kDLFloat, 32, 1}, rows, d), tc(d_c, dev, DLDataType{kDLFloat, 32, 1}, p.n_lists, d);
+          dl_view tl(d_l, dev, DLDataType{kDLInt, 32, 1}, rows);
           double inertia = 0;
-          check_c(cuvsKMeansPredict(mg->shards[0].res, kp, &tx, nullptr, &tc, &tl, false, &inertia), "cuvsKMeansPredict (routing)");
+          check_c(cuvsKMeansPredict(mg->shards[0].res, kp, &tx.m, nullptr, &tc.m, &tl.m, false, &inertia), "cuvsKMeansPredict (routing)");
           B2_CUDA(cudaMemcpyAsync(labels.data(), d_l, sizeof(int) * rows, cudaMemcpyDeviceToHost, st));
           B2_CUDA(cudaStreamSynchronize(st));
         }
@@ -238,10 +227,9 @@ cuvsError_t cuvsMultiGpuIvfFlatBuild(cuvsResources_t res, cuvsMultiGpuIvfFlatInd
           B2_CUDA(cudaMallocAsync(reinterpret_cast<void**>(&di), sizeof(int64_t) * m, st));
           B2_CUDA(cudaMemcpyAsync(dv, rows_of[i].data(), sizeof(float) * m * d, cudaMemcpyHostToDevice, st));
           B2_CUDA(cudaMemcpyAsync(di, ids_of[i].data(), sizeof(int64_t) * m, cudaMemcpyHostToDevice, st));
-          int64_t vs[2] = {m, d}, is[1] = {m};
-          DLManagedTensor tv = make_dl(dv, kDLCUDA, mg->shards[i].device, DLDataType{kDLFloat, 32, 1}, 2, vs);
-          DLManagedTensor ti = make_dl(di, kDLCUDA, mg->shards[i].device, DLDataType{kDLInt, 64, 1}, 1, is);
-          check_c(cuvsIvfFlatExtend(mg->shards[i].res, &tv, &ti, mg->shards[i].index), "cuvsIvfFlatExtend (shard)");
+          dl_view tv(dv, DLDevice{kDLCUDA, mg->shards[i].device}, DLDataType{kDLFloat, 32, 1}, m, d);
+          dl_view ti(di, DLDevice{kDLCUDA, mg->shards[i].device}, DLDataType{kDLInt, 64, 1}, m);
+          check_c(cuvsIvfFlatExtend(mg->shards[i].res, &tv.m, &ti.m, mg->shards[i].index), "cuvsIvfFlatExtend (shard)");
           B2_CUDA(cudaFreeAsync(dv, st));
           B2_CUDA(cudaFreeAsync(di, st));
           B2_CUDA(cudaStreamSynchronize(st));  // the host staging vectors are reused by the next chunk
@@ -257,9 +245,7 @@ cuvsError_t cuvsMultiGpuIvfFlatBuild(cuvsResources_t res, cuvsMultiGpuIvfFlatInd
       check_c(cuvsKMeansParamsDestroy(kp), "cuvsKMeansParamsDestroy");
       mg->comm = make_local_comm_group(r->mg_devices);
     }
-    if (index->addr) delete reinterpret_cast<mg_index*>(index->addr);
-    index->addr  = reinterpret_cast<uintptr_t>(mg.release());
-    index->dtype = ds.dtype;
+    set_index(index, mg.release(), ds.dtype);
   });
 }
 
@@ -268,8 +254,8 @@ cuvsError_t cuvsMultiGpuIvfFlatSearch(cuvsResources_t res, cuvsMultiGpuIvfFlatSe
 {
   return guarded([=] {
     as_res(res);
-    B2_EXPECTS(params && index && index->addr && queries_tensor && neighbors_tensor && distances_tensor, "null argument");
-    auto& mg = *reinterpret_cast<mg_index*>(index->addr);
+    B2_EXPECTS(params && queries_tensor && neighbors_tensor && distances_tensor, "null argument");
+    auto& mg = index_of<mg_index>(index);
     const DLTensor& q  = queries_tensor->dl_tensor;
     const DLTensor& nb = neighbors_tensor->dl_tensor;
     const DLTensor& dd = distances_tensor->dl_tensor;
@@ -297,11 +283,10 @@ cuvsError_t cuvsMultiGpuIvfFlatSearch(cuvsResources_t res, cuvsMultiGpuIvfFlatSe
       B2_CUDA(cudaMallocAsync(reinterpret_cast<void**>(&pt.di), sizeof(int64_t) * pt.qn * k, pt.st));
       B2_CUDA(cudaMallocAsync(reinterpret_cast<void**>(&pt.dv), sizeof(float) * pt.qn * k, pt.st));
       B2_CUDA(cudaMemcpyAsync(pt.dq, dl_ptr<float>(q) + pt.q0 * mg.dim, sizeof(float) * pt.qn * mg.dim, cudaMemcpyHostToDevice, pt.st));
-      int64_t qs[2] = {pt.qn, mg.dim}, os[2] = {pt.qn, k};
-      DLManagedTensor tq = make_dl(pt.dq, kDLCUDA, sh.device, DLDataType{kDLFloat, 32, 1}, 2, qs);
-      DLManagedTensor ti = make_dl(pt.di, kDLCUDA, sh.device, DLDataType{kDLInt, 64, 1}, 2, os);
-      DLManagedTensor tv = make_dl(pt.dv, kDLCUDA, sh.device, DLDataType{kDLFloat, 32, 1}, 2, os);
-      check_c(cuvsIvfFlatSearch(sh.res, params->base_params, sh.index, &tq, &ti, &tv, cuvsFilter{0, NO_FILTER}), "cuvsIvfFlatSearch (shard)");
+      const DLDevice dev{kDLCUDA, sh.device};
+      dl_view tq(pt.dq, dev, DLDataType{kDLFloat, 32, 1}, pt.qn, mg.dim), ti(pt.di, dev, DLDataType{kDLInt, 64, 1}, pt.qn, k),
+          tv(pt.dv, dev, DLDataType{kDLFloat, 32, 1}, pt.qn, k);
+      check_c(cuvsIvfFlatSearch(sh.res, params->base_params, sh.index, &tq.m, &ti.m, &tv.m, cuvsFilter{0, NO_FILTER}), "cuvsIvfFlatSearch (shard)");
       if (!sharded) {
         B2_CUDA(cudaMemcpyAsync(out_i + pt.q0 * k, pt.di, sizeof(int64_t) * pt.qn * k, cudaMemcpyDeviceToHost, pt.st));
         B2_CUDA(cudaMemcpyAsync(out_v + pt.q0 * k, pt.dv, sizeof(float) * pt.qn * k, cudaMemcpyDeviceToHost, pt.st));

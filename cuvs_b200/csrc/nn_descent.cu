@@ -1033,11 +1033,6 @@ struct nnd_index {
   owned<uint32_t> graph;
   owned<float> dist;  // empty when built without distances
 };
-nnd_index& nnd_of(cuvsNNDescentIndex_t index)
-{
-  B2_EXPECTS(index != nullptr && index->addr != 0, "index is not built");
-  return *reinterpret_cast<nnd_index*>(index->addr);
-}
 // copies rows x cols elements of `es` bytes from device `src` into a row-major host or device tensor
 void copy_out(resources* r, const void* src, const DLTensor& dst, int64_t rows, int64_t cols, DLDataType dt, const char* what)
 {
@@ -1073,7 +1068,7 @@ cuvsError_t cuvsNNDescentIndexDestroy(cuvsNNDescentIndex_t index)
 {
   return guarded([=] {
     if (!index) return;
-    delete reinterpret_cast<nnd_index*>(index->addr);
+    drop_index<nnd_index>(index);
     delete index;
   });
 }
@@ -1111,9 +1106,7 @@ cuvsError_t cuvsNNDescentBuild(cuvsResources_t res, cuvsNNDescentIndexParams_t p
                      static_cast<int>(params->dist_comp_dtype), idx->graph.data(), idx->dist.data());
     B2_CUDA(cudaStreamSynchronize(s));
     if (graph_t) copy_out(r, idx->graph.data(), graph_t->dl_tensor, n, idx->degree, DLDataType{kDLUInt, 32, 1}, "graph");
-    delete reinterpret_cast<nnd_index*>(index->addr);
-    index->dtype = ds.dtype;
-    index->addr  = reinterpret_cast<uintptr_t>(idx.release());
+    set_index(index, idx.release(), ds.dtype);
   });
 }
 
@@ -1121,7 +1114,7 @@ cuvsError_t cuvsNNDescentIndexGetGraph(cuvsResources_t res, cuvsNNDescentIndex_t
 {
   return guarded([=] {
     auto r   = as_res(res);
-    auto& ix = nnd_of(index);
+    auto& ix = index_of<nnd_index>(index);
     B2_EXPECTS(graph != nullptr, "graph is null");
     copy_out(r, ix.graph.data(), graph->dl_tensor, ix.n, ix.degree, DLDataType{kDLUInt, 32, 1}, "graph");
   });
@@ -1131,7 +1124,7 @@ cuvsError_t cuvsNNDescentIndexGetDistances(cuvsResources_t res, cuvsNNDescentInd
 {
   return guarded([=] {
     auto r   = as_res(res);
-    auto& ix = nnd_of(index);
+    auto& ix = index_of<nnd_index>(index);
     B2_EXPECTS(distances != nullptr, "distances is null");
     B2_EXPECTS(ix.dist.data() != nullptr, "nn-descent index doesn't contain distances - set return_distances when building");
     copy_out(r, ix.dist.data(), distances->dl_tensor, ix.n, ix.degree, DLDataType{kDLFloat, 32, 1}, "distances");

@@ -15,7 +15,10 @@
 #pragma once
 #include "common.hpp"
 
+#include <library_types.h>
+
 #include <cstdint>
+#include <cstdlib>
 #include <cstring>
 #include <istream>
 #include <ostream>
@@ -156,6 +159,41 @@ inline void read_array(std::istream& is, T* host, int64_t count, const char* wha
   is.read(reinterpret_cast<char*>(host), static_cast<std::streamsize>(count * sizeof(T)));
   B2_EXPECTS(bool(is), "%s: truncated file", what);
   if (shape_out) *shape_out = h.shape;
+}
+
+/**
+ * The element types an index file can hold: the 4-byte tag in front of a CAGRA or IVF-Flat file (kind and size, the reader
+ * dispatches on them: c/src/neighbors/cagra.cpp:881-899, ivf_flat.cpp:307-325), the NPY descr of its data records (float16
+ * is kind 'e' in the tag and 'f' to NumPy), the cudaDataType of CAGRA's strided dataset record (dataset_serialize.hpp:83-99)
+ * and the element size.
+ */
+struct file_dtype {
+  DLDataType dl;
+  const char* tag;  // three characters; written with the terminating zero
+  const char* descr;
+  cudaDataType cuda;
+  int size;
+};
+inline const file_dtype kFileDtypes[] = {{{kDLFloat, 32, 1}, "<f4", "<f4", CUDA_R_32F, 4},
+                                         {{kDLFloat, 16, 1}, "<e2", "<f2", CUDA_R_16F, 2},
+                                         {{kDLInt, 8, 1}, "|i1", "|i1", CUDA_R_8I, 1},
+                                         {{kDLUInt, 8, 1}, "|u1", "|u1", CUDA_R_8U, 1}};
+inline const file_dtype& file_dtype_for(DLDataType t)
+{
+  for (const file_dtype& f : kFileDtypes)
+    if (f.dl.code == t.code && f.dl.bits == t.bits) return f;
+  B2_FAIL("index files hold float32, float16, int8 or uint8 rows (got dtype code %d, bits %d)", int(t.code), int(t.bits));
+}
+/** The type a tag or an NPY descr names: byte order '<', '|' or '=', then kind and item size; null when it is none of the
+ *  four. */
+inline const file_dtype* file_dtype_named(const std::string& s)
+{
+  if (s.size() < 3 || (s[0] != '<' && s[0] != '|' && s[0] != '=')) return nullptr;
+  const char kind = s[1] == 'e' ? 'f' : s[1];
+  const int size  = std::atoi(s.c_str() + 2);
+  for (const file_dtype& f : kFileDtypes)
+    if (f.descr[1] == kind && f.size == size) return &f;
+  return nullptr;
 }
 
 /** Reads an array of exactly `count` elements of `item_size` bytes whatever their kind (float16 is '<f2' to NumPy and '<e2'
