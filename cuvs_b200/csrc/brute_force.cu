@@ -17,8 +17,13 @@
 //      path.  Result: identical to oracle/oracle.c::oracle_knn, bit for bit.
 // Filtered search and shapes the tensor-core kernel does not cover (dim > 2048, k > 64)
 // run on the exact SIMT path.
+//
+// Row types (DESIGN.md §3 "Row types"): float16, int8 and uint8 rows are kept in their own type.  float16 rows are scanned on
+// fp16 wgmma, int8 / uint8 rows on the integer tensor cores (exact integer scores); cosine keeps the bf16 planes of the unit
+// rows.  The re-score and the exact path read the typed rows and widen each element on load.
 #include "common.hpp"
 #include "exact.cuh"
+#include "npy_io.hpp"
 #include "scan_tc.cuh"
 #include "select_k.cuh"
 #include "timing.hpp"
@@ -36,26 +41,72 @@
 
 namespace b200 {
 
+// The element type of a brute-force index's rows (cuvsB200BruteForceIndexInfo's row_type)
+constexpr int kBfF32 = 0, kBfF16 = 1, kBfS8 = 2, kBfU8 = 3;
+
 struct bf_index {
   int64_t n   = 0;
   int d       = 0;
   int device  = 0;
   cuvsDistanceType metric = L2Expanded;
   float metric_arg        = 2.0f;
-  const float* data       = nullptr;  // [n, d] row-major on the device (view or data_own)
+  int row_type            = kBfF32;
+  const float* data       = nullptr;  // float32 rows: [n, d] row-major on the device (view or data_own)
   owned<float> data_own;
-  owned<float> norms;  // |x|^2 (always kept: the certificate needs max norm)
+  // float16 / int8 / uint8 rows, `ld` elements apart: the scan's zero-padded operand [rows_pad, Kp] when the scan reads them
+  // (f16_scan, i8_scan), else [n, d]
+  owned<uint8_t> rows;
+  int64_t ld = 0;
+  owned<float> norms;  // |x|^2 of the (widened) rows in the oracle's order (always kept: the certificate needs max norm)
   float xn_max = 0.f;
   // tensor-core side
   bool tc      = false;
-  int Kp       = 0;
+  int Kp       = 0;  // padded K of the scan's operands (8-bit scans: tc_pad_k_i8)
   int64_t rows_pad = 0;
-  owned<__nv_bfloat16> hi, lo;
-  owned<__nv_bfloat16> hx;  // [rows_pad, 16] half-norm plane (scan_tc.cuh)
+  owned<__nv_bfloat16> hi, lo;  // float32 rows, and cosine on every row type
+  owned<__nv_bfloat16> hx;  // [rows_pad, 16] half-norm plane (scan_tc.cuh) of the bf16 and fp16 scans
   owned<float> inv_norm;  // cosine only
+  owned<int> norms8;      // 8-bit scans: [rows_pad] exact |x|^2, kI8PadNorm on padding rows
+  bool f16_scan() const { return tc && row_type == kBfF16 && metric != CosineExpanded; }
+  bool i8_scan() const { return tc && (row_type == kBfS8 || row_type == kBfU8) && metric != CosineExpanded; }
+  template <typename T>
+  const T* rows_as() const { return reinterpret_cast<const T*>(rows.data()); }
+  int64_t device_bytes() const
+  {
+    return static_cast<int64_t>(data_own.size() * 4 + rows.size() + norms.size() * 4 + (hi.size() + lo.size() + hx.size()) * 2 +
+                                inv_norm.size() * 4 + norms8.size() * 4);
+  }
 };
 
 namespace {
+
+int row_type_of(DLDataType t)
+{
+  if (t.code == kDLFloat) return t.bits == 16 ? kBfF16 : kBfF32;
+  return t.code == kDLInt ? kBfS8 : kBfU8;
+}
+DLDataType dtype_of(int row_type)
+{
+  switch (row_type) {
+    case kBfF16: return {kDLFloat, 16, 1};
+    case kBfS8: return {kDLInt, 8, 1};
+    case kBfU8: return {kDLUInt, 8, 1};
+    default: return {kDLFloat, 32, 1};
+  }
+}
+int elem_bytes(int row_type) { return row_type == kBfF32 ? 4 : (row_type == kBfF16 ? 2 : 1); }
+
+// f(rows, ld): the index's rows in their own element type
+template <typename F>
+void with_rows(const bf_index& idx, F&& f)
+{
+  switch (idx.row_type) {
+    case kBfF16: return f(idx.rows_as<__half>(), idx.ld);
+    case kBfS8: return f(idx.rows_as<int8_t>(), idx.ld);
+    case kBfU8: return f(idx.rows_as<uint8_t>(), idx.ld);
+    default: return f(idx.data, static_cast<int64_t>(idx.d));
+  }
+}
 
 bool metric_supported(cuvsDistanceType m)
 {
@@ -71,6 +122,85 @@ __global__ void transpose_kernel(const float* __restrict__ in, float* __restrict
   int64_t r = t / d;
   int c     = static_cast<int>(t % d);
   out[t]    = in[static_cast<int64_t>(c) * n + r];
+}
+
+// column-major [n, d] elements of E bytes -> rows `ld` elements apart
+template <typename E>
+__global__ void transpose_into_kernel(const E* __restrict__ in, E* __restrict__ out, int64_t n, int d, int64_t ld)
+{
+  int64_t t = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x;
+  if (t >= n * d) return;
+  const int64_t r = t / d;
+  const int c     = static_cast<int>(t % d);
+  out[r * ld + c] = in[static_cast<int64_t>(c) * n + r];
+}
+
+// norms[r] = |x_r|^2 exactly over a padded 8-bit plane [rows_pad, Kp8], kI8PadNorm for r >= n.  One warp per row.
+template <bool U8>
+__global__ void i8_norms_kernel(const uint8_t* __restrict__ rows, int64_t n, int64_t rows_pad, int Kp8, int* __restrict__ norms)
+{
+  const int64_t r = (blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x) >> 5;
+  const int lane  = threadIdx.x & 31;
+  if (r >= rows_pad) return;
+  int acc = 0;
+  for (int j = lane; j < Kp8; j += 32) {
+    const int v = U8 ? static_cast<int>(rows[r * Kp8 + j]) : static_cast<int>(static_cast<int8_t>(rows[r * Kp8 + j]));
+    acc += v * v;
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
+  if (lane == 0) norms[r] = r < n ? acc : kI8PadNorm;
+}
+
+// The A operand of a narrow scan from fp32 query rows that hold values of type T (exact): [rows_pad, Kp], zero padded
+template <typename T>
+__global__ void pack_queries_kernel(const float* __restrict__ q, int64_t nq, int d, int Kp, int64_t rows_pad, T* __restrict__ out)
+{
+  const int64_t t = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x;
+  if (t >= rows_pad * Kp) return;
+  const int64_t r = t / Kp;
+  const int c     = static_cast<int>(t % Kp);
+  const float v   = r < nq && c < d ? q[r * d + c] : 0.f;
+  if constexpr (std::is_same_v<T, __half>) out[t] = __float2half_rn(v);
+  else out[t] = static_cast<T>(static_cast<int>(v));
+}
+
+// fp32 query rows against fp16 rows: row r scaled by 2^e, e putting its largest |component| in [2^14, 2^15) (e clamped to
+// [-60, 60]; a zero row keeps e = 0), then split into fp16 hi + lo.  scale[r] = 2^e (1 on padding rows).  One warp per row.
+__global__ void split_f16_queries_kernel(const float* __restrict__ q, int64_t nq, int d, int Kp, int64_t rows_pad,
+                                         __half* __restrict__ hi, __half* __restrict__ lo, float* __restrict__ scale)
+{
+  const int64_t r = (blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x) >> 5;
+  const int lane  = threadIdx.x & 31;
+  if (r >= rows_pad) return;
+  float m = 0.f;
+  if (r < nq)
+    for (int c = lane; c < d; c += 32) m = fmaxf(m, fabsf(q[r * d + c]));
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
+  int ex = 0;
+  if (m > 0.f) {
+    frexpf(m, &ex);  // m in [2^(ex-1), 2^ex)
+    ex = min(60, max(-60, 15 - ex));
+  }
+  const float sc = ldexpf(1.0f, ex);
+  for (int c = lane; c < Kp; c += 32) {
+    const float v  = r < nq && c < d ? q[r * d + c] * sc : 0.f;
+    const __half h = __float2half_rn(v);
+    hi[r * Kp + c] = h;
+    lo[r * Kp + c] = __float2half_rn(v - __half2float(h));
+  }
+  if (lane == 0) scale[r] = sc;
+}
+
+// 8-bit scan keys (tc_i8_key) -> the bf16 scan's units s = hn - q.x: half the integer score for L2, the score itself for inner
+// product; +inf (empty slots) stays
+__global__ void i8_keys_to_scores_kernel(float* __restrict__ v, int64_t count, float mul)
+{
+  const int64_t i = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x;
+  if (i >= count) return;
+  const float key = v[i];
+  if (key < INFINITY) v[i] = mul * static_cast<float>(tc_i8_score(key));
 }
 
 __global__ void max_kernel(const float* __restrict__ v, int64_t n, float* __restrict__ out)
@@ -129,12 +259,41 @@ static bf_index* bf_build(resources* res, const DLTensor& ds, cuvsDistanceType m
   idx->metric     = metric;
   idx->metric_arg = metric_arg;
   idx->device     = res->device;
+  idx->row_type   = row_type_of(ds.dtype);
   auto stream     = res->stream;
   const bool c_contig = dl_is_c_contiguous(ds), f_contig = dl_is_f_contiguous(ds);
   B2_EXPECTS(c_contig || f_contig, "dataset input to cuvsBruteForceBuild must be contiguous (non-strided)");
   const float* src = dl_ptr<float>(ds);
   const size_t count = static_cast<size_t>(idx->n) * idx->d;
-  if (dl_is_device(ds) && ds.device.device_type != kDLCUDAHost && c_contig) {
+  idx->tc = tc_supported(res->device, idx->d) && idx->n >= 1 && idx->n < (int64_t(1) << 31);
+  const bool l2 = (metric != InnerProduct && metric != CosineExpanded);
+  if (idx->row_type != kBfF32) {
+    // float16 / int8 / uint8: the rows in their own type, in the scan's padded operand when the scan reads them
+    const int es   = elem_bytes(idx->row_type);
+    idx->rows_pad  = tc_pad_rows(idx->n);
+    const bool pad = idx->f16_scan() || idx->i8_scan();
+    idx->Kp        = idx->row_type == kBfF16 || metric == CosineExpanded ? tc_pad_k(idx->d) : tc_pad_k_i8(idx->d);
+    idx->ld        = pad ? idx->Kp : idx->d;
+    const int64_t rows = pad ? idx->rows_pad : idx->n;
+    idx->rows.alloc(static_cast<size_t>(rows * idx->ld * es));
+    if (pad) B2_CUDA(cudaMemsetAsync(idx->rows.data(), 0, idx->rows.size(), stream));
+    if (count == 0) {
+    } else if (c_contig) {
+      B2_CUDA(cudaMemcpy2DAsync(idx->rows.data(), idx->ld * es, ds.data, static_cast<size_t>(idx->d) * es,
+                                static_cast<size_t>(idx->d) * es, idx->n, cudaMemcpyDefault, stream));
+    } else {
+      dbuf<uint8_t> tmp(count * es, stream);
+      B2_CUDA(cudaMemcpyAsync(tmp.data(), ds.data, count * es, cudaMemcpyDefault, stream));
+      count_launch();
+      if (es == 2)
+        transpose_into_kernel<<<blocks_for(static_cast<int64_t>(count), 256), 256, 0, stream>>>(
+          reinterpret_cast<const uint16_t*>(tmp.data()), reinterpret_cast<uint16_t*>(idx->rows.data()), idx->n, idx->d, idx->ld);
+      else
+        transpose_into_kernel<<<blocks_for(static_cast<int64_t>(count), 256), 256, 0, stream>>>(
+          tmp.data(), idx->rows.data(), idx->n, idx->d, idx->ld);
+      B2_CUDA(cudaGetLastError());
+    }
+  } else if (dl_is_device(ds) && ds.device.device_type != kDLCUDAHost && c_contig) {
     idx->data = src;  // non-owning view, like the reference (brute_force.cu:60-75)
   } else {
     idx->data_own.alloc(count);
@@ -149,7 +308,7 @@ static bf_index* bf_build(resources* res, const DLTensor& ds, cuvsDistanceType m
     idx->data = idx->data_own.data();
   }
   idx->norms.alloc(static_cast<size_t>(std::max<int64_t>(idx->n, 1)));
-  row_norms(stream, idx->data, idx->n, idx->d, idx->d, idx->norms.data());
+  with_rows(*idx, [&](auto x, int64_t ld) { row_norms(stream, x, idx->n, idx->d, ld, idx->norms.data()); });
   {
     dbuf<float> mx(1, stream);
     B2_CUDA(cudaMemsetAsync(mx.data(), 0, sizeof(float), stream));
@@ -158,8 +317,18 @@ static bf_index* bf_build(resources* res, const DLTensor& ds, cuvsDistanceType m
     B2_CUDA(cudaMemcpyAsync(&idx->xn_max, mx.data(), sizeof(float), cudaMemcpyDeviceToHost, stream));
     B2_CUDA(cudaStreamSynchronize(stream));
   }
-  idx->tc = tc_supported(res->device, idx->d) && idx->n >= 1 && idx->n < (int64_t(1) << 31);
-  if (idx->tc) {
+  if (idx->i8_scan()) {
+    idx->norms8.alloc(static_cast<size_t>(idx->rows_pad));
+    count_launch();
+    if (idx->row_type == kBfU8)
+      i8_norms_kernel<true><<<blocks_for(idx->rows_pad * 32, 256), 256, 0, stream>>>(idx->rows.data(), idx->n, idx->rows_pad, idx->Kp, idx->norms8.data());
+    else
+      i8_norms_kernel<false><<<blocks_for(idx->rows_pad * 32, 256), 256, 0, stream>>>(idx->rows.data(), idx->n, idx->rows_pad, idx->Kp, idx->norms8.data());
+    B2_CUDA(cudaGetLastError());
+  } else if (idx->f16_scan()) {
+    idx->hx.alloc(static_cast<size_t>(idx->rows_pad) * 16);
+    tc_half_norms(stream, l2 ? idx->norms.data() : nullptr, idx->n, idx->rows_pad, idx->hx.data());
+  } else if (idx->tc) {
     idx->Kp       = tc_pad_k(idx->d);
     idx->rows_pad = tc_pad_rows(idx->n);
     idx->hi.alloc(static_cast<size_t>(idx->rows_pad) * idx->Kp);
@@ -171,8 +340,20 @@ static bf_index* bf_build(resources* res, const DLTensor& ds, cuvsDistanceType m
       rsqrt_rows(stream, idx->norms.data(), idx->n, idx->inv_norm.data());
       scale = idx->inv_norm.data();
     }
-    tc_split_planes(stream, idx->data, idx->n, idx->d, idx->d, idx->Kp, idx->hi.data(), idx->lo.data(), idx->rows_pad, scale);
-    const bool l2 = (metric != InnerProduct && metric != CosineExpanded);
+    if (idx->row_type == kBfF32) {
+      tc_split_planes(stream, idx->data, idx->n, idx->d, idx->d, idx->Kp, idx->hi.data(), idx->lo.data(), idx->rows_pad, scale);
+    } else {
+      // cosine over narrow rows: the planes of the unit rows from bounded chunks of widened rows, which are not kept
+      const int64_t chunk = std::max<int64_t>(kTcTile, ((int64_t(1) << 24) / idx->d) / kTcTile * kTcTile);
+      dbuf<float> w(static_cast<size_t>(std::min(chunk, idx->n) * idx->d), stream);
+      for (int64_t r0 = 0; r0 < idx->n; r0 += chunk) {
+        const int64_t c   = std::min(chunk, idx->n - r0);
+        const int64_t pad = r0 + chunk >= idx->n ? idx->rows_pad - r0 : c;  // the last chunk zeroes the padding rows
+        widen_async(stream, idx->rows.data() + r0 * idx->ld * elem_bytes(idx->row_type), dtype_of(idx->row_type), c * idx->d, w.data());
+        tc_split_planes(stream, w.data(), c, idx->d, idx->d, idx->Kp, idx->hi.data() + r0 * idx->Kp, idx->lo.data() + r0 * idx->Kp,
+                        pad, scale + r0);
+      }
+    }
     tc_half_norms(stream, l2 ? idx->norms.data() : nullptr, idx->n, idx->rows_pad, idx->hx.data());
   }
   return idx.release();
@@ -197,8 +378,10 @@ static void search_exact(resources* res, const bf_index& idx, const float* q, in
   dbuf<float> dist(static_cast<size_t>(chunk * n_cols), stream);
   for (int64_t q0 = 0; q0 < nq; q0 += chunk) {
     int64_t qc = std::min(chunk, nq - q0);
-    exact_distance_tile(stream, q + q0 * idx.d, qc, idx.d, idx.data, idx.n, idx.d, idx.d, need_norms ? qn.data() + q0 : nullptr,
-                        need_norms ? idx.norms.data() : nullptr, idx.metric, dist.data(), idx.n, filt, q_row0 + q0);
+    with_rows(idx, [&](auto x, int64_t ld) {
+      exact_distance_tile(stream, q + q0 * idx.d, qc, idx.d, x, idx.n, ld, idx.d, need_norms ? qn.data() + q0 : nullptr,
+                          need_norms ? idx.norms.data() : nullptr, idx.metric, dist.data(), idx.n, filt, q_row0 + q0);
+    });
     select_k(stream, dist.data(), nullptr, IDX_NONE, qc, idx.n, idx.n, k, out_dist + q0 * k, out_idx + q0 * k, IDX_I64,
              select_min);
   }
@@ -235,28 +418,61 @@ __global__ void list_floor_kernel(const float* __restrict__ cs, int64_t nq, int6
   if (lane == 0) out[q] = m;
 }
 
-// Stage 1+2 of the search: split-bf16 wgmma scan over `splits` dataset ranges (lists of KC per column half and split) +
+// Stage 1+2 of the search: wgmma scan over `splits` dataset ranges (lists of KC per column half and split) +
 // merge to KCm per query (KCm == KC: the merged set's worst entry bounds everything outside it; KCm > KC, used for k above
-// the fused list length: `out.floor` carries the bound for the rows that never entered a list).
-static void bf_tc_candidates(resources* res, const bf_index& idx, const float* q, int64_t nq, int KC, bf_cands& out, int KCm = 0)
+// the fused list length: `out.floor` carries the bound for the rows that never entered a list).  The scan is split-bf16 over
+// the bf16 planes, fp16 over fp16 rows (q_narrow: the queries hold fp16 values, one pass; else the scaled two-pass split) or
+// 8-bit over 8-bit rows (q_narrow).  Scores come out in the bf16 scan's units, s = hn - q.x.
+static void bf_tc_candidates(resources* res, const bf_index& idx, const float* q, int64_t nq, bool q_narrow, int KC, bf_cands& out,
+                             int KCm = 0)
 {
   if (KCm <= 0) KCm = KC;
   auto stream           = res->stream;
   const int64_t nq_pad  = tc_pad_rows(nq);
   const int m_tiles     = static_cast<int>(nq_pad / 128);
   const int64_t b_tiles = idx.rows_pad / 128;
-  const int splits      = pick_splits(m_tiles, b_tiles, res->sm_count ? res->sm_count : 132);
+  int splits            = pick_splits(m_tiles, b_tiles, res->sm_count ? res->sm_count : 132);
+  // 8-bit lists of 16 at k > 16: enough lists per query that the merged width covers KCm
+  if (idx.i8_scan()) splits = std::max(splits, (KCm + kTcListsPerItem * KC - 1) / (kTcListsPerItem * KC));
   const int n_items     = m_tiles * splits;
 
   out.qn.alloc(static_cast<size_t>(nq), stream);
   row_norms(stream, q, nq, idx.d, idx.d, out.qn.data());
   dbuf<float> qscale;
-  if (idx.metric == CosineExpanded) {
-    qscale.alloc(static_cast<size_t>(nq), stream);
-    rsqrt_rows(stream, out.qn.data(), nq, qscale.data());
+  dbuf<__nv_bfloat16> qhi, qlo;
+  dbuf<__half> qh, ql;
+  dbuf<uint8_t> q8;
+  const int64_t a_elems = nq_pad * idx.Kp;
+  if (idx.i8_scan()) {
+    B2_EXPECTS(q_narrow, "brute_force: an 8-bit index is scanned with queries of its own type");
+    q8.alloc(static_cast<size_t>(a_elems), stream);
+    count_launch();
+    if (idx.row_type == kBfU8)
+      pack_queries_kernel<<<blocks_for(a_elems, 256), 256, 0, stream>>>(q, nq, idx.d, idx.Kp, nq_pad, q8.data());
+    else
+      pack_queries_kernel<<<blocks_for(a_elems, 256), 256, 0, stream>>>(q, nq, idx.d, idx.Kp, nq_pad, reinterpret_cast<int8_t*>(q8.data()));
+    B2_CUDA(cudaGetLastError());
+  } else if (idx.f16_scan()) {
+    qh.alloc(static_cast<size_t>(a_elems), stream);
+    count_launch();
+    if (q_narrow) {
+      pack_queries_kernel<<<blocks_for(a_elems, 256), 256, 0, stream>>>(q, nq, idx.d, idx.Kp, nq_pad, qh.data());
+    } else {
+      ql.alloc(static_cast<size_t>(a_elems), stream);
+      qscale.alloc(static_cast<size_t>(nq_pad), stream);
+      split_f16_queries_kernel<<<blocks_for(nq_pad * 32, 256), 256, 0, stream>>>(q, nq, idx.d, idx.Kp, nq_pad, qh.data(), ql.data(),
+                                                                                 qscale.data());
+    }
+    B2_CUDA(cudaGetLastError());
+  } else {
+    if (idx.metric == CosineExpanded) {
+      qscale.alloc(static_cast<size_t>(nq), stream);
+      rsqrt_rows(stream, out.qn.data(), nq, qscale.data());
+    }
+    qhi.alloc(static_cast<size_t>(a_elems), stream);
+    qlo.alloc(static_cast<size_t>(a_elems), stream);
+    tc_split_planes(stream, q, nq, idx.d, idx.d, idx.Kp, qhi.data(), qlo.data(), nq_pad, qscale.data());
   }
-  dbuf<__nv_bfloat16> qhi(static_cast<size_t>(nq_pad) * idx.Kp, stream), qlo(static_cast<size_t>(nq_pad) * idx.Kp, stream);
-  tc_split_planes(stream, q, nq, idx.d, idx.d, idx.Kp, qhi.data(), qlo.data(), nq_pad, qscale.data());
 
   dbuf<tc_item> items(static_cast<size_t>(n_items), stream);
   const int KCW = KC * kTcListsPerItem;  // candidates per (item, query row)
@@ -272,9 +488,21 @@ static void bf_tc_candidates(resources* res, const bf_index& idx, const float* q
   B2_CUDA(cudaMemsetAsync(bkeys.data(), tc_bound_init_byte, sizeof(int) * nq_pad, stream));
   tc_bound bnd;
   bnd.keys = bkeys.data();
-  tc_scan_topk(stream, res->device, qhi.data(), qlo.data(), nq_pad, idx.hi.data(), idx.lo.data(), idx.rows_pad, idx.Kp,
-               idx.hx.data(), items.data(), n_items, nullptr, KC, 3, cs.data(), cp.data(), row_stride, &bnd,
-               false /*equal-sized items in split-major order: static round-robin keeps each column range L2 resident*/);
+  // equal-sized items in split-major order: static round-robin keeps each column range L2 resident
+  if (idx.i8_scan()) {
+    tc_scan_i8(stream, res->device, idx.row_type == kBfU8, q8.data(), nq_pad, idx.rows.data(), idx.rows_pad, idx.Kp, idx.norms8.data(),
+               idx.metric != InnerProduct, items.data(), n_items, nullptr, KC, cs.data(), cp.data(), row_stride, &bnd, false);
+    count_launch();
+    const int64_t cnt = nq_pad * row_stride;
+    i8_keys_to_scores_kernel<<<blocks_for(cnt, 256), 256, 0, stream>>>(cs.data(), cnt, idx.metric == InnerProduct ? 1.0f : 0.5f);
+    B2_CUDA(cudaGetLastError());
+  } else if (idx.f16_scan()) {
+    tc_scan_f16(stream, res->device, qh.data(), ql.data(), qscale.data(), nq_pad, idx.rows_as<__half>(), idx.rows_pad, idx.Kp,
+                idx.hx.data(), items.data(), n_items, KC, cs.data(), cp.data(), row_stride, &bnd, false);
+  } else {
+    tc_scan_topk(stream, res->device, qhi.data(), qlo.data(), nq_pad, idx.hi.data(), idx.lo.data(), idx.rows_pad, idx.Kp,
+                 idx.hx.data(), items.data(), n_items, nullptr, KC, 3, cs.data(), cp.data(), row_stride, &bnd, false);
+  }
   if (KCm > KC) {
     out.floor.alloc(static_cast<size_t>(nq), stream);
     count_launch();
@@ -305,7 +533,12 @@ static approx_map bf_approx_map(const bf_index& idx)
   // Relative to |q|^2 + max|x|^2 (DESIGN.md §3): the split-bf16 products are within 3*2^-18*2|q||x| <= 2^-16.4 of exact, and
   // the fp32 accumulation of Kp products adds up to ~Kp*2^-24 (Kp/16 wgmma k-steps of 16).  max(2^-15, 2^-16 + Kp*2^-24)
   // covers both; it is 2^-15 up to Kp = 256 (so the d <= 128 searches keep their budget) and 2^-13 + 2^-16 at Kp = 2048.
+  // fp16 scans (exact products, or a split query within 2^-21 |q||x|) stay inside the same budget.
   am.eps_rel = std::max(1.0f / 32768.0f, 1.0f / 65536.0f + static_cast<float>(idx.Kp) / 16777216.0f);
+  // 8-bit scans score exact integers; the budget covers the fp32 re-score's rounding against them (<= 2d ulps of
+  // |q|^2 + |x|^2 for a sum of d products or squared differences and its finish) and the scores' conversion to fp32.  Below
+  // |q|^2 + max|x|^2 = 2^23 there is no rounding at all and the budget is 0 (bf_certify_kernel<true>).
+  if (idx.i8_scan()) am.eps_rel = static_cast<float>(2 * idx.Kp + 8) / 16777216.0f;
   if (idx.metric == InnerProduct) { am.sa = -1.f; am.eq = 1.f; am.ec = idx.xn_max; }
   else if (idx.metric == CosineExpanded) { am.sa = 1.f; am.sc = 1.f; am.eq = 0.f; am.ec = 2.f; }
   else { am.sa = 2.f; am.sb = 1.f; am.eq = 1.f; am.ec = idx.xn_max; }
@@ -316,6 +549,9 @@ static approx_map bf_approx_map(const bf_index& idx)
 // out_dist[q, k-1] (selection form, before postprocess_distances) beats the worst approximate score A of the rows outside the
 // candidates by more than eps_rel * (eq |q|^2 + ec).  Such rows exist when the candidate list is full and score worse than its
 // worst entry; with a floor (raw engine units, +inf: none), the bound of the rows that never entered a list, also worse than it.
+// kExactInts (8-bit scans): while m = |q|^2 + max|x|^2 < 2^23, every value the scan keys, the re-score and this kernel form is an
+// integer below 2^24 in magnitude (norms and partial sums <= m, distances <= 2m), so all of them are exact and eps is 0.
+template <bool kExactInts>
 __global__ void bf_certify_kernel(const float* __restrict__ cand_score, const uint32_t* __restrict__ cand_pos, int kc,
                                   const float* __restrict__ approx_floor, const float* __restrict__ qn,
                                   const float* __restrict__ out_dist, int k, approx_map amap, bool select_min, int64_t nq,
@@ -352,7 +588,9 @@ __global__ void bf_certify_kernel(const float* __restrict__ cand_score, const ui
     }
   }
   if (outside) {
-    float eps = amap.eps_rel * (amap.eq * qnv + amap.ec);
+    const float mag = amap.eq * qnv + amap.ec;
+    float eps       = amap.eps_rel * mag;
+    if (kExactInts && mag < 8388608.0f) eps = 0.f;
     bool ok   = select_min ? (kth < worst_approx - eps) : (kth > worst_approx + eps);
     flag      = ok ? 0 : 1;
   }
@@ -360,8 +598,9 @@ __global__ void bf_certify_kernel(const float* __restrict__ cand_score, const ui
   if (flag) atomicAdd(flags + nq, 1);
 }
 
+// qt: fp32 queries; q_narrow when they are the widened values of queries of the index's own narrow type
 static void bf_search(resources* res, const bf_index& idx, const DLTensor& qt, const DLTensor& nt, const DLTensor& dt,
-                      cuvsFilter prefilter)
+                      cuvsFilter prefilter, bool q_narrow)
 {
   auto stream      = res->stream;
   const int64_t nq = qt.shape[0];
@@ -401,22 +640,27 @@ static void bf_search(resources* res, const bf_index& idx, const DLTensor& qt, c
   }
 
   // ---- tensor-core candidate scan
-  const int KC  = k <= 10 ? 16 : 32;
-  const int KCm = k <= 24 ? KC : (k <= 48 ? 64 : 96);
+  // (the fused 8-bit top-32 exists at Kp = 128 only: wider 8-bit rows take lists of 16, merged to KCm with the floor bound)
+  const bool kc32 = !idx.i8_scan() || idx.Kp == 128;
+  const int KC    = k <= 10 || !kc32 ? 16 : 32;
+  const int KCm   = k <= 10 ? 16 : (k <= 24 ? 32 : (k <= 48 ? 64 : 96));
   bf_cands cand;
-  bf_tc_candidates(res, idx, q, nq, KC, cand, KCm);
+  bf_tc_candidates(res, idx, q, nq, q_narrow, KC, cand, KCm);
 
   // ---- exact re-scoring
   const bool need_xn = (idx.metric == L2Expanded || idx.metric == L2SqrtExpanded || idx.metric == CosineExpanded);
-  rescore_topk(stream, q, nq, idx.d, idx.data, idx.d, idx.d, cand.qn.data(), need_xn ? idx.norms.data() : nullptr, idx.metric,
-               cand.pos.data(), cand.width, nullptr, k, out_idx, out_dist, -1);
+  with_rows(idx, [&](auto x, int64_t ld) {
+    rescore_topk(stream, q, nq, idx.d, x, ld, idx.d, cand.qn.data(), need_xn ? idx.norms.data() : nullptr, idx.metric,
+                 cand.pos.data(), cand.width, nullptr, k, out_idx, out_dist, -1);
+  });
 
   // ---- certificate, and the exact path for flagged queries (rare: exact ties / duplicates at the k' boundary)
   dbuf<int> flags(static_cast<size_t>(nq) + 1, stream);
   B2_CUDA(cudaMemsetAsync(flags.data() + nq, 0, sizeof(int), stream));
   count_launch();
-  bf_certify_kernel<<<blocks_for(nq * 32, 256), 256, 0, stream>>>(cand.score.data(), cand.pos.data(), cand.width, cand.floor.data(),
-                                                                  cand.qn.data(), out_dist, k, bf_approx_map(idx), select_min, nq,
+  auto certify = idx.i8_scan() ? bf_certify_kernel<true> : bf_certify_kernel<false>;
+  certify<<<blocks_for(nq * 32, 256), 256, 0, stream>>>(cand.score.data(), cand.pos.data(), cand.width, cand.floor.data(),
+                                                        cand.qn.data(), out_dist, k, bf_approx_map(idx), select_min, nq,
                                                                   flags.data());
   B2_CUDA(cudaGetLastError());
   // search_exact answers every query on its own, and these run unfiltered, so the gathered rows get the same bits
@@ -459,20 +703,10 @@ cuvsError_t cuvsBruteForceBuild(cuvsResources_t res, DLManagedTensor* dataset_te
     auto r = as_res(res);
     B2_EXPECTS(dataset_tensor != nullptr && index != nullptr, "null argument");
     const DLTensor& ds = dataset_tensor->dl_tensor;
-    if (dl_is(ds, kDLFloat, 32)) {
-      drop_index<bf_index>(index);
-      set_index(index, bf_build(r, ds, metric, metric_arg), ds.dtype);
-    } else if (dl_is_dataset_dtype(ds)) {
-      // float16 / int8 / uint8 (c/src/neighbors/brute_force.cpp:60-110): widened once, the index owns the fp32 copy
-      f32_matrix w;
-      widen_to_f32(r, ds, w);
-      drop_index<bf_index>(index);
-      bf_index* b = bf_build(r, w.t, metric, metric_arg);
-      if (b->data == w.own.data()) b->data_own = std::move(w.own);
-      set_index(index, b, ds.dtype);
-    } else {
-      B2_FAIL("Unsupported dataset DLtensor dtype: %d and bits: %d", ds.dtype.code, ds.dtype.bits);
-    }
+    // float32, float16, int8 or uint8 rows (c/src/neighbors/brute_force.cpp:60-110), each kept in its own type
+    B2_EXPECTS(dl_is_dataset_dtype(ds), "Unsupported dataset DLtensor dtype: %d and bits: %d", ds.dtype.code, ds.dtype.bits);
+    drop_index<bf_index>(index);
+    set_index(index, bf_build(r, ds, metric, metric_arg), ds.dtype);
   });
 }
 
@@ -489,11 +723,11 @@ cuvsError_t cuvsBruteForceSearch(cuvsResources_t res, cuvsBruteForceIndex_t inde
     check_search_tensors(queries, neighbors, distances, idx.d, false);
     B2_EXPECTS(queries.dtype.code == index->dtype.code, "type mismatch between index and queries");
     if (dl_is(queries, kDLFloat, 32)) {
-      bf_search(r, idx, queries, neighbors, distances, prefilter);
+      bf_search(r, idx, queries, neighbors, distances, prefilter, false);
     } else if (dl_is_dataset_dtype(queries) && queries.dtype.bits == index->dtype.bits) {
       f32_rows w;
       widen_to_f32(r, queries, w);
-      bf_search(r, idx, w.t, neighbors, distances, prefilter);
+      bf_search(r, idx, w.t, neighbors, distances, prefilter, true);
     } else {
       B2_FAIL("Unsupported queries DLtensor dtype: %d and bits: %d", queries.dtype.code, queries.dtype.bits);
     }
@@ -511,19 +745,27 @@ cuvsError_t cuvsB200BruteForceCandidates(cuvsResources_t res, cuvsBruteForceInde
     const DLTensor& cp  = cand_pos->dl_tensor;
     const DLTensor& cs  = cand_score->dl_tensor;
     B2_EXPECTS(idx.tc, "index has no tensor-core planes on this device");
-    B2_EXPECTS(dl_is(q, kDLFloat, 32) && dl_is_device(q) && dl_is_c_contiguous(q) && q.ndim == 2 && q.shape[1] == idx.d, "bad queries");
+    // float32 queries, or (as cuvsBruteForceSearch accepts them) queries of the index's own type
+    const bool q_f32 = dl_is(q, kDLFloat, 32);
+    B2_EXPECTS((q_f32 || (dl_is_dataset_dtype(q) && q.dtype.bits == index->dtype.bits)) && dl_is_device(q) && dl_is_c_contiguous(q) &&
+                 q.ndim == 2 && q.shape[1] == idx.d, "bad queries");
+    B2_EXPECTS(q.dtype.code == index->dtype.code, "type mismatch between index and queries");
     const int KC = static_cast<int>(cp.shape[1]);
     B2_EXPECTS((KC == 16 || KC == 32) && dl_is(cp, kDLUInt, 32) && dl_is(cs, kDLFloat, 32) && cp.shape[0] == q.shape[0] &&
                  cs.shape[0] == q.shape[0] && cs.shape[1] == KC, "bad candidate tensors");
+    B2_EXPECTS(KC == 16 || !idx.i8_scan() || idx.Kp == 128, "the 8-bit scan keeps lists of 32 at padded widths of 128 only");
+    f32_rows w;
+    widen_to_f32(r, q, w);
     bf_cands c;
-    bf_tc_candidates(r, idx, dl_ptr<float>(q), q.shape[0], KC, c);
+    bf_tc_candidates(r, idx, dl_ptr<float>(w.t), q.shape[0], !q_f32, KC, c);
     B2_CUDA(cudaMemcpyAsync(dl_ptr<void>(cp), c.pos.data(), sizeof(uint32_t) * q.shape[0] * KC, cudaMemcpyDeviceToDevice, r->stream));
     B2_CUDA(cudaMemcpyAsync(dl_ptr<void>(cs), c.score.data(), sizeof(float) * q.shape[0] * KC, cudaMemcpyDeviceToDevice, r->stream));
     B2_CUDA(cudaStreamSynchronize(r->stream));
   });
 }
 
-// Serialization: 4-char numpy-style dtype tag ("<f4\0"), then n, dim, metric, metric_arg, rows.
+// Serialization: 4-char numpy-style dtype tag of the rows ("<f4\0", "<f2\0", "|i1\0" or "|u1\0"), then n, dim, metric,
+// metric_arg, the n x dim rows in that type.
 // (Own container; the reference's brute_force_serialize.cu writes RAFT mdspans — compatibility is a
 // "next" item, SURVEY §8f n1.)
 cuvsError_t cuvsBruteForceSerialize(cuvsResources_t res, const char* filename, cuvsBruteForceIndex_t index)
@@ -531,13 +773,19 @@ cuvsError_t cuvsBruteForceSerialize(cuvsResources_t res, const char* filename, c
   return guarded([=] {
     auto r = as_res(res);
     B2_EXPECTS(filename, "null argument");
-    auto& idx = index_of<bf_index>(index);
-    std::vector<float> host(static_cast<size_t>(idx.n) * idx.d);
-    B2_CUDA(cudaMemcpyAsync(host.data(), idx.data, host.size() * sizeof(float), cudaMemcpyDeviceToHost, r->stream));
+    auto& idx    = index_of<bf_index>(index);
+    const int es = elem_bytes(idx.row_type);
+    std::vector<char> host(static_cast<size_t>(idx.n) * idx.d * es);
+    const void* src      = idx.row_type == kBfF32 ? static_cast<const void*>(idx.data) : idx.rows.data();
+    const size_t pitch   = static_cast<size_t>(idx.row_type == kBfF32 ? idx.d : idx.ld) * es;
+    if (!host.empty())
+      B2_CUDA(cudaMemcpy2DAsync(host.data(), static_cast<size_t>(idx.d) * es, src, pitch, static_cast<size_t>(idx.d) * es, idx.n,
+                                cudaMemcpyDeviceToHost, r->stream));
     B2_CUDA(cudaStreamSynchronize(r->stream));
     std::ofstream os(filename, std::ios::out | std::ios::binary);
     B2_EXPECTS(bool(os), "Cannot open file %s", filename);
-    const char tag[4] = {'<', 'f', '4', 0};
+    const char* descr = npy::file_dtype_for(dtype_of(idx.row_type)).descr;  // "<f4", "<f2", "|i1", "|u1"
+    const char tag[4] = {descr[0], descr[1], descr[2], 0};
     os.write(tag, 4);
     int64_t n = idx.n, d = idx.d;
     int32_t m = int(idx.metric);
@@ -545,7 +793,7 @@ cuvsError_t cuvsBruteForceSerialize(cuvsResources_t res, const char* filename, c
     os.write(reinterpret_cast<const char*>(&d), 8);
     os.write(reinterpret_cast<const char*>(&m), 4);
     os.write(reinterpret_cast<const char*>(&idx.metric_arg), 4);
-    os.write(reinterpret_cast<const char*>(host.data()), static_cast<std::streamsize>(host.size() * sizeof(float)));
+    os.write(host.data(), static_cast<std::streamsize>(host.size()));
     B2_EXPECTS(bool(os), "Error writing %s", filename);
   });
 }
@@ -559,7 +807,8 @@ cuvsError_t cuvsBruteForceDeserialize(cuvsResources_t res, const char* filename,
     B2_EXPECTS(bool(is), "Cannot open file %s", filename);
     char tag[4]{};
     B2_EXPECTS(bool(is.read(tag, 4)), "Invalid or truncated index header in file %s", filename);
-    B2_EXPECTS(tag[0] == '<' && tag[1] == 'f' && tag[2] == '4', "Unsupported index dtype in %s", filename);
+    const npy::file_dtype* ft = npy::file_dtype_named(std::string(tag, 3));
+    B2_EXPECTS(ft != nullptr, "Unsupported index dtype in %s", filename);
     int64_t n = 0, d = 0;
     int32_t m = 0;
     float marg = 0;
@@ -568,12 +817,22 @@ cuvsError_t cuvsBruteForceDeserialize(cuvsResources_t res, const char* filename,
     is.read(reinterpret_cast<char*>(&m), 4);
     is.read(reinterpret_cast<char*>(&marg), 4);
     B2_EXPECTS(bool(is) && n >= 0 && d > 0, "Invalid index header in file %s", filename);
-    std::vector<float> host(static_cast<size_t>(n) * d);
-    is.read(reinterpret_cast<char*>(host.data()), static_cast<std::streamsize>(host.size() * sizeof(float)));
+    std::vector<char> host(static_cast<size_t>(n) * d * ft->size);
+    is.read(host.data(), static_cast<std::streamsize>(host.size()));
     B2_EXPECTS(bool(is), "Truncated index file %s", filename);
-    const dl_view rows(host.data(), DLDevice{kDLCPU, 0}, DLDataType{kDLFloat, 32, 1}, n, d);
+    const dl_view rows(host.data(), DLDevice{kDLCPU, 0}, ft->dl, n, d);
     drop_index<bf_index>(index);
     set_index(index, bf_build(r, rows.t(), static_cast<cuvsDistanceType>(m), marg), rows.t().dtype);
+  });
+}
+
+cuvsError_t cuvsB200BruteForceIndexInfo(cuvsBruteForceIndex_t index, int* row_type, int64_t* device_bytes)
+{
+  return guarded([=] {
+    B2_EXPECTS(row_type && device_bytes, "null argument");
+    auto& idx     = index_of<bf_index>(index);
+    *row_type     = idx.row_type;
+    *device_bytes = idx.device_bytes();
   });
 }
 

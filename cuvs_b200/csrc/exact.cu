@@ -9,18 +9,22 @@
 #include "timing.hpp"
 
 #include <cfloat>
+#include <type_traits>
 #include <vector>
 
 namespace b200 {
 namespace {
 
-__global__ void row_norms_kernel(const float* __restrict__ x, int64_t n, int d, int64_t ld, float* __restrict__ out)
+template <typename T>
+__global__ void row_norms_kernel(const T* __restrict__ x, int64_t n, int d, int64_t ld, float* __restrict__ out)
 {
   int64_t i = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x;
   if (i >= n) return;
-  const float* r = x + i * ld;
-  float acc      = 0.f;
-  if ((d & 3) == 0 && (ld & 3) == 0 && (reinterpret_cast<uintptr_t>(x) & 15) == 0) {
+  const T* r = x + i * ld;
+  float acc  = 0.f;
+  if constexpr (!std::is_same_v<T, float>) {
+    for (int k = 0; k < d; ++k) { const float v = widen(r[k]); acc = fmaf(v, v, acc); }
+  } else if ((d & 3) == 0 && (ld & 3) == 0 && (reinterpret_cast<uintptr_t>(x) & 15) == 0) {
     const float4* r4 = reinterpret_cast<const float4*>(r);
     for (int k = 0; k < d / 4; ++k) {
       float4 v = r4[k];
@@ -61,9 +65,9 @@ constexpr int TM = 64, TN = 64, TK = 16;
 
 // 64x64 output tile per CTA, 256 threads, 4x4 micro-tile per thread; every output accumulates over
 // k = 0..d-1 in order (one fmaf per k), which is the oracle's order.
-template <bool SqDiff>
+template <bool SqDiff, typename T>
 __global__ void __launch_bounds__(256) exact_tile_kernel(const float* __restrict__ q, int64_t nq, int64_t ldq,
-                                                           const float* __restrict__ x, int64_t n, int64_t ldx, int d,
+                                                           const T* __restrict__ x, int64_t n, int64_t ldx, int d,
                                                            const float* __restrict__ qn, const float* __restrict__ xn,
                                                            int metric, float* __restrict__ out, int64_t ldo,
                                                            filter_view filt, int64_t q_row0)
@@ -86,7 +90,7 @@ __global__ void __launch_bounds__(256) exact_tile_kernel(const float* __restrict
       int r = idx >> 4, kk = idx & 15;
       int64_t gr = row0 + r, gc = col0 + r;
       As[kk][r] = (gr < nq && k0 + kk < d) ? q[gr * ldq + k0 + kk] : 0.f;
-      Bs[kk][r] = (gc < n && k0 + kk < d) ? x[gc * ldx + k0 + kk] : 0.f;
+      Bs[kk][r] = (gc < n && k0 + kk < d) ? widen(x[gc * ldx + k0 + kk]) : 0.f;
     }
     __syncthreads();
     const int kmax = min(TK, d - k0);
@@ -131,8 +135,9 @@ constexpr int kMaxCand      = 256;   // one warp per query
 constexpr int kMaxCandBlock = 2048;  // one CTA per query
 
 // one warp per query
+template <typename T>
 __global__ void __launch_bounds__(128) rescore_kernel(const float* __restrict__ q, int64_t nq, int64_t ldq,
-                                                       const float* __restrict__ x, int64_t ldx, int d,
+                                                       const T* __restrict__ x, int64_t ldx, int d,
                                                        const float* __restrict__ qn, const float* __restrict__ xn,
                                                        int metric, const uint32_t* __restrict__ cand_pos, int kc,
                                                        const int64_t* __restrict__ src_ids, int k,
@@ -149,7 +154,8 @@ __global__ void __launch_bounds__(128) rescore_kernel(const float* __restrict__ 
   const bool select_min = metric != InnerProduct;
   const float* qr       = q + qi * ldq;
   const float qnv       = qn ? qn[qi] : 0.f;
-  const bool vec4       = exact_vec4(q, ldq, x, ldx, d);
+  bool vec4             = false;
+  if constexpr (std::is_same_v<T, float>) vec4 = exact_vec4(q, ldq, x, ldx, d);
 
   for (int c = lane; c < kc; c += 32) {
     uint32_t pos = cand_pos[qi * kc + c];
@@ -190,7 +196,8 @@ __global__ void __launch_bounds__(128) rescore_kernel(const float* __restrict__ 
 // More candidates than one warp's shared memory holds (refine with 257..2048 candidates): one CTA per query.  Every candidate
 // is scored by one thread with exact_accumulate, as in rescore_kernel, then the kc entries are sorted by rescore_kernel's
 // ranking rule, (distance, id, slot), with a bitonic sort over kpow2 entries; the padding entries (slot >= kc) rank last.
-__global__ void __launch_bounds__(256) rescore_block_kernel(const float* __restrict__ q, int64_t ldq, const float* __restrict__ x,
+template <typename T>
+__global__ void __launch_bounds__(256) rescore_block_kernel(const float* __restrict__ q, int64_t ldq, const T* __restrict__ x,
                                                              int64_t ldx, int d, const float* __restrict__ qn,
                                                              const float* __restrict__ xn, int metric,
                                                              const uint32_t* __restrict__ cand_pos, int kc, int kpow2,
@@ -205,7 +212,8 @@ __global__ void __launch_bounds__(256) rescore_block_kernel(const float* __restr
   const bool select_min = metric != InnerProduct;
   const float* qr       = q + qi * ldq;
   const float qnv       = qn ? qn[qi] : 0.f;
-  const bool vec4       = exact_vec4(q, ldq, x, ldx, d);
+  bool vec4             = false;
+  if constexpr (std::is_same_v<T, float>) vec4 = exact_vec4(q, ldq, x, ldx, d);
   for (int c = threadIdx.x; c < kpow2; c += blockDim.x) {
     float dist = select_min ? FLT_MAX : -FLT_MAX;
     int64_t id = INT64_MAX;
@@ -257,7 +265,8 @@ __global__ void copy_rows_kernel(const T* __restrict__ src, const int64_t* __res
 
 }  // namespace
 
-void row_norms(cudaStream_t stream, const float* x, int64_t n, int d, int64_t ld, float* out)
+template <typename T>
+void row_norms(cudaStream_t stream, const T* x, int64_t n, int d, int64_t ld, float* out)
 {
   if (n == 0) return;
   count_launch();
@@ -284,7 +293,8 @@ void normalize_rows(cudaStream_t stream, float* x, int64_t n, int d, int64_t ld)
   B2_CUDA(cudaGetLastError());
 }
 
-void exact_distance_tile(cudaStream_t stream, const float* q, int64_t nq, int64_t ldq, const float* x, int64_t n,
+template <typename T>
+void exact_distance_tile(cudaStream_t stream, const float* q, int64_t nq, int64_t ldq, const T* x, int64_t n,
                          int64_t ldx, int d, const float* qn, const float* xn, cuvsDistanceType metric, float* out,
                          int64_t ldo, filter_view filt, int64_t q_row0)
 {
@@ -295,13 +305,14 @@ void exact_distance_tile(cudaStream_t stream, const float* q, int64_t nq, int64_
   count_launch();
   timed_section ts("exact_tile", stream);
   if (sq)
-    exact_tile_kernel<true><<<grid, 256, 0, stream>>>(q, nq, ldq, x, n, ldx, d, qn, xn, int(metric), out, ldo, filt, q_row0);
+    exact_tile_kernel<true, T><<<grid, 256, 0, stream>>>(q, nq, ldq, x, n, ldx, d, qn, xn, int(metric), out, ldo, filt, q_row0);
   else
-    exact_tile_kernel<false><<<grid, 256, 0, stream>>>(q, nq, ldq, x, n, ldx, d, qn, xn, int(metric), out, ldo, filt, q_row0);
+    exact_tile_kernel<false, T><<<grid, 256, 0, stream>>>(q, nq, ldq, x, n, ldx, d, qn, xn, int(metric), out, ldo, filt, q_row0);
   B2_CUDA(cudaGetLastError());
 }
 
-void rescore_topk(cudaStream_t stream, const float* q, int64_t nq, int64_t ldq, const float* x, int64_t ldx, int d,
+template <typename T>
+void rescore_topk(cudaStream_t stream, const float* q, int64_t nq, int64_t ldq, const T* x, int64_t ldx, int d,
                   const float* qn, const float* xn, cuvsDistanceType metric, const uint32_t* cand_pos, int kc,
                   const int64_t* src_ids, int k, int64_t* out_idx, float* out_dist, int64_t pad_id)
 {
@@ -312,7 +323,7 @@ void rescore_topk(cudaStream_t stream, const float* q, int64_t nq, int64_t ldq, 
     while (kpow2 < kc) kpow2 <<= 1;
     const size_t smem = static_cast<size_t>(kpow2) * (sizeof(int64_t) + sizeof(float) + sizeof(int));
     count_launch();
-    rescore_block_kernel<<<static_cast<unsigned>(nq), 256, smem, stream>>>(q, ldq, x, ldx, d, qn, xn, int(metric), cand_pos, kc, kpow2,
+    rescore_block_kernel<T><<<static_cast<unsigned>(nq), 256, smem, stream>>>(q, ldq, x, ldx, d, qn, xn, int(metric), cand_pos, kc, kpow2,
                                                                           src_ids, k, out_idx, out_dist, pad_id);
     B2_CUDA(cudaGetLastError());
     return;
@@ -321,10 +332,23 @@ void rescore_topk(cudaStream_t stream, const float* q, int64_t nq, int64_t ldq, 
   const int warps = 4;
   size_t smem     = static_cast<size_t>(warps) * kc * (sizeof(float) + sizeof(int64_t));
   count_launch();
-  rescore_kernel<<<static_cast<unsigned>((nq + warps - 1) / warps), warps * 32, smem, stream>>>(
+  rescore_kernel<T><<<static_cast<unsigned>((nq + warps - 1) / warps), warps * 32, smem, stream>>>(
     q, nq, ldq, x, ldx, d, qn, xn, int(metric), cand_pos, kc, src_ids, k, out_idx, out_dist, pad_id);
   B2_CUDA(cudaGetLastError());
 }
+
+#define B2_EXACT_ROW_TYPE(T)                                                                                            \
+  template void row_norms<T>(cudaStream_t, const T*, int64_t, int, int64_t, float*);                                  \
+  template void exact_distance_tile<T>(cudaStream_t, const float*, int64_t, int64_t, const T*, int64_t, int64_t, int,    \
+                                       const float*, const float*, cuvsDistanceType, float*, int64_t, filter_view, int64_t); \
+  template void rescore_topk<T>(cudaStream_t, const float*, int64_t, int64_t, const T*, int64_t, int, const float*,     \
+                                const float*, cuvsDistanceType, const uint32_t*, int, const int64_t*, int, int64_t*, float*, \
+                                int64_t);
+B2_EXACT_ROW_TYPE(float)
+B2_EXACT_ROW_TYPE(__half)
+B2_EXACT_ROW_TYPE(int8_t)
+B2_EXACT_ROW_TYPE(uint8_t)
+#undef B2_EXACT_ROW_TYPE
 
 template <typename T>
 void copy_rows(cudaStream_t s, const T* src, const int64_t* src_rows, T* dst, const int64_t* dst_rows, int64_t n, int64_t width)

@@ -5,6 +5,7 @@
 // are (a) the re-scoring stage behind every tensor-core candidate scan, (b) the certified fallback
 // of brute force, (c) the filtered / exotic-shape path.
 #pragma once
+#include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <cstdint>
 #include <functional>
@@ -15,8 +16,12 @@
 
 namespace b200 {
 
+// Row types: the rows x of row_norms, exact_distance_tile and rescore_topk are float, __half, int8_t or uint8_t.  Narrow
+// elements are widened on load, so a narrow row gives the same bits as its fp32 copy.  Queries are always fp32.
+
 /** out[i] = sum_k x[i,k]^2 (ascending k, fmaf). */
-void row_norms(cudaStream_t stream, const float* x, int64_t n, int d, int64_t ld, float* out);
+template <typename T>
+void row_norms(cudaStream_t stream, const T* x, int64_t n, int d, int64_t ld, float* out);
 
 /** out[i] = 1 / sqrt(xn[i]) from squared norms, and 0 where xn[i] is 0: the per-row scale of the cosine metric.  A zero row
  *  scales to the zero vector, so its cosine distance to anything is 1.  out may alias xn. */
@@ -31,7 +36,8 @@ void normalize_rows(cudaStream_t stream, float* x, int64_t n, int d, int64_t ld)
  * (needed for L2*Expanded and Cosine, may be null otherwise).  Filtered-out pairs get the worst
  * value.  `q_row0` is the global query index of row 0 (bitmap addressing).
  */
-void exact_distance_tile(cudaStream_t stream, const float* q, int64_t nq, int64_t ldq, const float* x, int64_t n,
+template <typename T>
+void exact_distance_tile(cudaStream_t stream, const float* q, int64_t nq, int64_t ldq, const T* x, int64_t n,
                          int64_t ldx, int d, const float* qn, const float* xn, cuvsDistanceType metric, float* out,
                          int64_t ldo, filter_view filt, int64_t q_row0);
 
@@ -43,7 +49,8 @@ void exact_distance_tile(cudaStream_t stream, const float* q, int64_t nq, int64_
  * id `pad_id` and +/-FLT_MAX.  kc <= 256 runs one warp per query; 256 < kc <= 2048 (k <= kc) one CTA per query with the
  * same arithmetic and ranking.
  */
-void rescore_topk(cudaStream_t stream, const float* q, int64_t nq, int64_t ldq, const float* x, int64_t ldx, int d,
+template <typename T>
+void rescore_topk(cudaStream_t stream, const float* q, int64_t nq, int64_t ldq, const T* x, int64_t ldx, int d,
                   const float* qn, const float* xn, cuvsDistanceType metric, const uint32_t* cand_pos, int kc,
                   const int64_t* src_ids, int k, int64_t* out_idx, float* out_dist, int64_t pad_id);
 

@@ -1,6 +1,7 @@
 // Device side of the exact fp32 layer (exact.cuh).  Every kernel that must return oracle/oracle.c's bits scores a candidate
 // with exact_accumulate and finish_distance, so the re-score and the exact fallbacks cannot drift apart.
 #pragma once
+#include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <cstdint>
 
@@ -61,6 +62,27 @@ __device__ __forceinline__ float exact_accumulate(const float* __restrict__ qr, 
       if (sqdiff) { float t = qr[kk] - xr[kk]; acc = fmaf(t, t, acc); }
       else acc = fmaf(qr[kk], xr[kk], acc);
     }
+  }
+  return acc;
+}
+
+/** A row element as fp32: every float16, int8 and uint8 value is exactly representable, so the narrow row types give the
+ *  same sums as their widened fp32 copies. */
+__device__ __forceinline__ float widen(float v) { return v; }
+__device__ __forceinline__ float widen(__half v) { return __half2float(v); }
+__device__ __forceinline__ float widen(int8_t v) { return static_cast<float>(v); }
+__device__ __forceinline__ float widen(uint8_t v) { return static_cast<float>(v); }
+
+/** exact_accumulate over rows stored as float16, int8 or uint8: each element widened on load, same order and fmaf as above. */
+template <typename T>
+__device__ __forceinline__ float exact_accumulate(const float* __restrict__ qr, const T* __restrict__ xr, int d, bool, int metric)
+{
+  const bool sqdiff = (metric == L2Unexpanded || metric == L2SqrtUnexpanded);
+  float acc         = 0.f;
+  for (int kk = 0; kk < d; ++kk) {
+    const float x = widen(xr[kk]);
+    if (sqdiff) { float t = qr[kk] - x; acc = fmaf(t, t, acc); }
+    else acc = fmaf(qr[kk], x, acc);
   }
   return acc;
 }

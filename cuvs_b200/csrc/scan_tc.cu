@@ -69,8 +69,9 @@ struct cfg {
   static_assert(stages >= 2, "tc_scan_kernel: shared memory budget exceeded");
 };
 
-// Operand types of the scan: bf16 planes (fp32 accumulators), or 8-bit integer rows (s32 accumulators, tc_scan_i8).
-constexpr int kOpBf16 = 0, kOpS8 = 1, kOpU8 = 2;
+// Operand types of the scan: bf16 planes (fp32 accumulators), 8-bit integer rows (s32 accumulators, tc_scan_i8), or fp16 rows
+// (fp32 accumulators, tc_scan_f16).
+constexpr int kOpBf16 = 0, kOpS8 = 1, kOpU8 = 2, kOpF16 = 3;
 
 __device__ __forceinline__ float acc_bits(float x) { return x; }
 __device__ __forceinline__ float acc_bits(uint32_t x) { return __uint_as_float(x); }
@@ -91,18 +92,25 @@ __device__ __forceinline__ uint32_t i8_t_bits(uint32_t acc, int n, int l2)
 // stands for the item's own width, n_tiles * 128.
 // OP = kOpS8 / kOpU8: one pass over 8-bit rows (a k-block is 128 bytes = 128 components), no half-norm step: the epilogue adds
 // the row norms col_norm[b row] itself (i8_t_bits); scores are order-preserving keys of exact integers.
+// OP = kOpF16: the bf16 layout with fp16 operands (m64n128k16.f32.f16.f16); the half-norm step stays a bf16 wgmma on the hx
+// plane into the same accumulator.  PASSES = 2 there is an fp32 query split into fp16 hi + lo after scaling row r by a power of
+// two a_scale[r] (so that its components stay clear of fp16's subnormals); the half-norm step's A rows then hold a_scale[r]
+// instead of 1, the accumulator is a_scale[r] (q.x - hn), and the lists and the bound are scaled back exactly.
 template <int KB, int PASSES, int KC, int OP = kOpBf16>
 __global__ void __launch_bounds__(128 + kEpiThreads, 1)
 tc_scan_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant__ CUtensorMap tmA_lo,
                const __grid_constant__ CUtensorMap tmB_hi, const __grid_constant__ CUtensorMap tmB_lo,
                const __grid_constant__ CUtensorMap tmB_x, const tc_item* __restrict__ items, int n_items_host,
                const int* __restrict__ n_items_dev, int kblocks_rt, int* __restrict__ sched_counter, float* __restrict__ out_score, uint32_t* __restrict__ out_pos,
-               int64_t out_row_stride, tc_bound bound, const int* __restrict__ col_norm, int l2)
+               int64_t out_row_stride, tc_bound bound, const int* __restrict__ col_norm, int l2, const float* __restrict__ a_scale)
 {
-  static_assert(OP == kOpBf16 || PASSES == 1, "8-bit scans are single-pass");
+  constexpr bool kI8     = OP == kOpS8 || OP == kOpU8;
+  constexpr bool kScaled = OP == kOpF16 && PASSES == 2;  // per-row power-of-two query scale (a_scale)
+  static_assert(!kI8 || PASSES == 1, "8-bit scans are single-pass");
+  static_assert(OP != kOpF16 || (PASSES <= 2 && KC > 0), "fp16 scans: 1 or 2 passes, fused top-k epilogue");
   using C = cfg<KB, PASSES>;
-  constexpr int kBlockK = OP == kOpBf16 ? 64 : 128;  // components of one 128-byte k-block
-  using acc_t = std::conditional_t<OP == kOpBf16, float, uint32_t>;
+  constexpr int kBlockK = kI8 ? 128 : 64;  // components of one 128-byte k-block
+  using acc_t = std::conditional_t<kI8, uint32_t, float>;
   constexpr int NA = C::NA, NB = C::NB;
   const int nkb = C::streamed ? kblocks_rt : KB;  // k-blocks of 64 per tile
   const int n_items = n_items_dev ? *n_items_dev : n_items_host;
@@ -205,7 +213,7 @@ tc_scan_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
         for (int kb = 0; kb < nkb; ++kb) {
           ptx::mbar_wait(&empty[stage], phase ^ 1);
           if (ptx::elect_one()) {
-            ptx::mbar_arrive_expect_tx(&full[stage], C::x_off + (OP == kOpBf16 && kb == 0 ? kExtBytes : 0));
+            ptx::mbar_arrive_expect_tx(&full[stage], C::x_off + (!kI8 && kb == 0 ? kExtBytes : 0));
             uint8_t* dst = sB + stage * C::stage_bytes;
             if constexpr (C::streamed) {
               ptx::tma_load_2d(dst, &tmA_hi, &full[stage], kb * kBlockK, static_cast<int32_t>(item.a_row0));
@@ -213,7 +221,7 @@ tc_scan_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
             }
             ptx::tma_load_2d(dst + C::b_off, &tmB_hi, &full[stage], kb * kBlockK, brow);
             if (NB == 2) ptx::tma_load_2d(dst + C::b_off + kTileBytes, &tmB_lo, &full[stage], kb * kBlockK, brow);
-            if (OP == kOpBf16 && kb == 0) ptx::tma_load_2d(dst + C::x_off, &tmB_x, &full[stage], 0, brow);
+            if (!kI8 && kb == 0) ptx::tma_load_2d(dst + C::x_off, &tmB_x, &full[stage], 0, brow);
           }
           if (++stage == C::stages) { stage = 0; phase ^= 1; }
         }
@@ -231,7 +239,8 @@ tc_scan_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
     const int col0    = half * kCols;
     const uint32_t a_lo0   = ptx::smem_desc_lo(ptx::smem_u32(sA)) + wg * 512;  // + 64 rows of 128 B
     const uint32_t b_lo0   = ptx::smem_desc_lo(ptx::smem_u32(sB));
-    const uint32_t ones_lo = ptx::smem_desc_lo(ptx::smem_u32(sOnes));
+    // (scaled fp16 scans: each warpgroup reads its own 64 rows of 32 bytes)
+    const uint32_t ones_lo = ptx::smem_desc_lo(ptx::smem_u32(sOnes)) + (kScaled ? wg * 128 : 0);
     // this thread's accumulator fragment inside the staging tile (see ptx::wgmma_bf16), and its epilogue row
     float* stg_frag       = sStg + (64 * wg + 16 * (warp & 3) + (lane >> 2)) * kStgLd + 2 * (lane & 3);
     const float* stg_row  = sStg + row * kStgLd + col0;
@@ -263,8 +272,14 @@ tc_scan_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
           // (16 KB >> 4).  Streamed A: the planes lead the stage, the B planes follow at b_off.
           const uint32_t ah = (C::streamed ? b_lo + wg * 512 : a_lo0 + (0 * KB + kb) * 1024) + k * 2;
           const uint32_t bh = b_lo + (C::b_off >> 4) + k * 2;
-          if constexpr (OP != kOpBf16) {
+          if constexpr (kI8) {
             ptx::wgmma_i8_128<OP == kOpU8>(d, ptx::desc(ah, ptx::kDescHiSw128), ptx::desc(bh, ptx::kDescHiSw128), (kb | k) != 0 ? 1u : 0u);
+          } else if constexpr (OP == kOpF16) {
+            ptx::wgmma_f16_128(d, ptx::desc(ah, ptx::kDescHiSw128), ptx::desc(bh, ptx::kDescHiSw128), (kb | k) != 0 ? 1u : 0u);
+            if (NA == 2) {
+              const uint32_t al = (C::streamed ? b_lo + wg * 512 + 1024 : a_lo0 + (1 * KB + kb) * 1024) + k * 2;
+              ptx::wgmma_f16_128(d, ptx::desc(al, ptx::kDescHiSw128), ptx::desc(bh, ptx::kDescHiSw128), 1u);
+            }
           } else {
             ptx::wgmma_bf16<128>(d, ptx::desc(ah, ptx::kDescHiSw128), ptx::desc(bh, ptx::kDescHiSw128), (kb | k) != 0 ? 1u : 0u);
             if (NA == 2) {
@@ -277,7 +292,7 @@ tc_scan_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
             }
           }
         }
-        if constexpr (OP == kOpBf16) {
+        if constexpr (!kI8) {
           if (kb == 0)  // -= |x|^2/2  (ones rows: all identical, both warpgroups read rows 0..63)
             ptx::wgmma_bf16<128>(d, ptx::desc(ones_lo, ptx::kDescHiSw32), ptx::desc(b_lo + (C::x_off >> 4), ptx::kDescHiSw32), 1u);
         }
@@ -305,7 +320,7 @@ tc_scan_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
     // 8-bit scans: 32 accumulator columns to the epilogue's t (i8_t_bits), nrm their row norms.  Done per 32 columns, just before
     // they are used: converting all 64 at once makes the fused epilogues spill.
     auto to_t = [&](uint32_t (&v)[32], const int* nrm) {
-      if constexpr (OP != kOpBf16) {
+      if constexpr (kI8) {
 #pragma unroll
         for (int c4 = 0; c4 < 8; ++c4) {
           const int4 n = __ldg(reinterpret_cast<const int4*>(nrm) + c4);
@@ -318,7 +333,7 @@ tc_scan_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
     };
     // the norms of this thread's columns of tile t of an item (8-bit scans only)
     auto tile_norms = [&](const tc_item& item, uint32_t t) -> const int* {
-      if constexpr (OP == kOpBf16) return nullptr;
+      if constexpr (!kI8) return nullptr;
       else return col_norm + item.b_row0 + t * 128 + col0;
     };
     auto begin_item = [&]() {
@@ -362,6 +377,18 @@ tc_scan_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
       for (int it = next_item(); it >= 0; it = next_item()) {
         const tc_item item = items[it];
         begin_item();
+        float q_scale = 1.f;  // kScaled: this row's a_scale (a power of two), the factor of the accumulator
+        if constexpr (kScaled) {
+          q_scale = a_scale[item.a_row0 + row];
+          if (half == 0) {  // row `row` of the half-norm step's A tile: {s, s, s, 0, ...} in both 16-byte chunks (see sOnes)
+            const uint32_t b = __bfloat16_as_ushort(__float2bfloat16_rn(q_scale));
+            const uint4 v    = make_uint4(b | (b << 16), b, 0u, 0u);
+            reinterpret_cast<uint4*>(sOnes)[2 * row]     = v;
+            reinterpret_cast<uint4*>(sOnes)[2 * row + 1] = v;
+          }
+          ptx::fence_proxy_async();
+          ptx::named_bar_sync(1 + wg, 128);  // the previous item's MMAs are done (fetch_tile's barrier); the new rows are visible
+        }
         float lv[KC > 0 ? KC : 1];
         uint32_t li[KC > 0 ? KC : 1];
 #pragma unroll
@@ -376,6 +403,7 @@ tc_scan_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
           const int kb        = *reinterpret_cast<volatile int*>(b_key);
           const float bv      = __int_as_float(kb >= 0 ? kb : kb ^ 0x7fffffff);
           thr0                = (bv - b_add) / bound.scale;
+          if constexpr (kScaled) thr0 *= q_scale;
         }
         const bool live_row = static_cast<uint32_t>(row) < item.valid_rows;
         if (!live_row) thr0 = -INFINITY;  // rows past the item's queries never collect candidates
@@ -453,7 +481,12 @@ tc_scan_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
         }
         end_item();
         flush();
-        const float my_kth = kth_best();
+        float my_kth = kth_best();
+        if constexpr (kScaled) {
+          my_kth /= q_scale;
+#pragma unroll
+          for (int j = 0; j < KC; ++j) lv[j] /= q_scale;
+        }
         if (b_key != nullptr && my_kth < INFINITY) {
           const float pub = __fmaf_rn(bound.scale, my_kth, b_add);  // same expression as the consumers of the bound
           const int kp    = __float_as_int(pub);
@@ -490,14 +523,15 @@ encode_fn_t get_encode_fn()
   return fn;
 }
 
-CUtensorMap make_plane_map(const __nv_bfloat16* ptr, int64_t rows, int Kp)
+// [rows, Kp] 2-byte plane (bf16, or fp16 rows and queries of tc_scan_f16), 64-element k-blocks, 128-byte swizzle
+CUtensorMap make_plane_map(const void* ptr, int64_t rows, int Kp, CUtensorMapDataType dt = CU_TENSOR_MAP_DATA_TYPE_BFLOAT16)
 {
   CUtensorMap m;
   cuuint64_t gdim[2]    = {static_cast<cuuint64_t>(Kp), static_cast<cuuint64_t>(rows)};
   cuuint64_t gstride[1] = {static_cast<cuuint64_t>(Kp) * sizeof(__nv_bfloat16)};
   cuuint32_t box[2]     = {64, 128};
   cuuint32_t estr[2]    = {1, 1};
-  CUresult r = get_encode_fn()(&m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<__nv_bfloat16*>(ptr), gdim, gstride, box,
+  CUresult r = get_encode_fn()(&m, dt, 2, const_cast<void*>(ptr), gdim, gstride, box,
                                estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
                                CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   B2_EXPECTS(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled failed with code %d (rows=%lld Kp=%d)", int(r), (long long)rows, Kp);
@@ -538,7 +572,7 @@ template <int KB, int PASSES, int KC, int OP = kOpBf16>
 void launch(cudaStream_t stream, int sm_count, const CUtensorMap& a_hi, const CUtensorMap& a_lo, const CUtensorMap& b_hi,
             const CUtensorMap& b_lo, const CUtensorMap& b_x, const tc_item* items, int n_items, const int* n_items_dev,
             float* out_score, uint32_t* out_pos, int64_t out_row_stride, const tc_bound& bound, bool dynamic, int kblocks,
-            const int* col_norm = nullptr, int l2 = 0)
+            const int* col_norm = nullptr, int l2 = 0, const float* a_scale = nullptr)
 {
   auto kern = tc_scan_kernel<KB, PASSES, KC, OP>;
   using C   = cfg<KB, PASSES>;
@@ -555,7 +589,7 @@ void launch(cudaStream_t stream, int sm_count, const CUtensorMap& a_hi, const CU
   timed_section ts("tc_scan", stream);
   count_launch();
   kern<<<grid, C::threads, C::smem, stream>>>(a_hi, a_lo, b_hi, b_lo, b_x, items, n_items, n_items_dev, kblocks, sched.data(), out_score,
-                                               out_pos, out_row_stride, bound, col_norm, l2);
+                                               out_pos, out_row_stride, bound, col_norm, l2, a_scale);
   B2_CUDA(cudaGetLastError());
 }
 
@@ -692,7 +726,8 @@ void tc_scan_topk(cudaStream_t stream, int device, const __nv_bfloat16* a_hi, co
 
 void tc_scan_i8(cudaStream_t stream, int device, bool is_unsigned, const void* a, int64_t a_rows_pad, const void* b,
                 int64_t b_rows_pad, int Kp, const int* b_norm, bool l2, const tc_item* items_dev, int n_items,
-                const int* n_items_dev, int KC, float* out_score, uint32_t* out_pos, int64_t out_row_stride, const tc_bound* bound)
+                const int* n_items_dev, int KC, float* out_score, uint32_t* out_pos, int64_t out_row_stride, const tc_bound* bound,
+                bool dynamic_schedule)
 {
   if (n_items == 0) return;
   B2_EXPECTS(Kp >= 128 && Kp % 128 == 0 && Kp <= kTcMaxK, "tc_scan_i8: padded K must be a multiple of 128 up to %d (got %d)", kTcMaxK, Kp);
@@ -706,13 +741,39 @@ void tc_scan_i8(cudaStream_t stream, int device, bool is_unsigned, const void* a
 #define B2_I8_CASE(KB_, KC_, OP_)                                                                                       \
   if (kb_case == KB_ && KC == KC_ && (OP_ == kOpU8) == is_unsigned)                                                     \
     return launch<KB_, 1, KC_, OP_>(stream, sms, mA, mA, mB, mB, mB, items_dev, n_items, n_items_dev, out_score, out_pos,  \
-                                    out_row_stride, bnd, true, Kp / 128, b_norm, l2 ? 1 : 0);
+                                    out_row_stride, bnd, dynamic_schedule, Kp / 128, b_norm, l2 ? 1 : 0);
   B2_I8_CASE(1, 16, kOpS8) B2_I8_CASE(1, 32, kOpS8) B2_I8_CASE(1, 0, kOpS8) B2_I8_CASE(2, 16, kOpS8) B2_I8_CASE(2, 0, kOpS8)
   B2_I8_CASE(0, 16, kOpS8) B2_I8_CASE(0, 0, kOpS8)
   B2_I8_CASE(1, 16, kOpU8) B2_I8_CASE(1, 32, kOpU8) B2_I8_CASE(1, 0, kOpU8) B2_I8_CASE(2, 16, kOpU8) B2_I8_CASE(2, 0, kOpU8)
   B2_I8_CASE(0, 16, kOpU8) B2_I8_CASE(0, 0, kOpU8)
 #undef B2_I8_CASE
   B2_FAIL("tc_scan_i8: no kernel for Kp=%d KC=%d", Kp, KC);
+}
+
+void tc_scan_f16(cudaStream_t stream, int device, const __half* a_hi, const __half* a_lo, const float* a_scale, int64_t a_rows_pad,
+                 const __half* b, int64_t b_rows_pad, int Kp, const __nv_bfloat16* hx, const tc_item* items_dev, int n_items, int KC,
+                 float* out_score, uint32_t* out_pos, int64_t out_row_stride, const tc_bound* bound, bool dynamic_schedule)
+{
+  if (n_items == 0) return;
+  B2_EXPECTS(Kp >= 64 && Kp % 64 == 0 && Kp <= kTcMaxK, "tc_scan_f16: padded K must be a multiple of 64 up to %d (got %d)", kTcMaxK, Kp);
+  B2_EXPECTS(KC == 16 || KC == 32, "tc_scan_f16: KC must be 16 or 32");
+  B2_EXPECTS((a_lo == nullptr) == (a_scale == nullptr), "tc_scan_f16: a split query needs its row scales");
+  const int passes   = a_lo ? 2 : 1;
+  const int sms      = sm_count_of(device);
+  const tc_bound bnd = bound ? *bound : tc_bound{};
+  CUtensorMap mA     = make_plane_map(a_hi, a_rows_pad, Kp, CU_TENSOR_MAP_DATA_TYPE_FLOAT16);
+  CUtensorMap mAl    = a_lo ? make_plane_map(a_lo, a_rows_pad, Kp, CU_TENSOR_MAP_DATA_TYPE_FLOAT16) : mA;
+  CUtensorMap mB     = make_plane_map(b, b_rows_pad, Kp, CU_TENSOR_MAP_DATA_TYPE_FLOAT16);
+  CUtensorMap mBx    = make_ext_map(hx, b_rows_pad);
+  const int kb_case  = Kp <= 128 ? Kp / 64 : 0;  // 0 = streamed A (any K)
+#define B2_F16_CASE(KB_, P_, KC_)                                                                                        \
+  if (kb_case == KB_ && passes == P_ && KC == KC_)                                                                       \
+    return launch<KB_, P_, KC_, kOpF16>(stream, sms, mA, mAl, mB, mB, mBx, items_dev, n_items, nullptr, out_score, out_pos,  \
+                                        out_row_stride, bnd, dynamic_schedule, Kp / 64, nullptr, 0, a_scale);
+  B2_F16_CASE(1, 1, 16) B2_F16_CASE(1, 1, 32) B2_F16_CASE(2, 1, 16) B2_F16_CASE(2, 1, 32) B2_F16_CASE(0, 1, 16) B2_F16_CASE(0, 1, 32)
+  B2_F16_CASE(1, 2, 16) B2_F16_CASE(1, 2, 32) B2_F16_CASE(2, 2, 16) B2_F16_CASE(2, 2, 32) B2_F16_CASE(0, 2, 16) B2_F16_CASE(0, 2, 32)
+#undef B2_F16_CASE
+  B2_FAIL("tc_scan_f16: no kernel for Kp=%d passes=%d KC=%d", Kp, passes, KC);
 }
 
 }  // namespace b200

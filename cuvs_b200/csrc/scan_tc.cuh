@@ -7,6 +7,7 @@
 // metric.  See scan_tc.cu for the kernel and DESIGN.md §3 for the layout.
 #pragma once
 #include <cuda_bf16.h>
+#include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <cstdint>
 
@@ -105,12 +106,22 @@ inline int tc_pad_k_i8(int d) { return (d + 127) / 128 * 128; }
 /**
  * tc_scan_topk over 8-bit rows: A [a_rows_pad, Kp] and B [b_rows_pad, Kp] int8 (uint8 when `is_unsigned`), K-major, Kp a
  * multiple of 128; b_norm [b_rows_pad] the exact |x|^2 of each B row (kI8PadNorm: excluded), `l2` false for inner product.
- * Same work items, epilogues and outputs as tc_scan_topk with passes = 1 (dynamic schedule), the scores being tc_i8_key's.
+ * Same work items, epilogues and outputs as tc_scan_topk with passes = 1, the scores being tc_i8_key's.
  * KC = 32 needs Kp = 128.
  */
 void tc_scan_i8(cudaStream_t stream, int device, bool is_unsigned, const void* a, int64_t a_rows_pad, const void* b,
                 int64_t b_rows_pad, int Kp, const int* b_norm, bool l2, const tc_item* items_dev, int n_items,
                 const int* n_items_dev, int KC, float* out_score, uint32_t* out_pos, int64_t out_row_stride,
-                const tc_bound* bound = nullptr);
+                const tc_bound* bound = nullptr, bool dynamic_schedule = true);
+
+/**
+ * tc_scan_topk over fp16 rows b [b_rows_pad, Kp] (zero padded, the bf16 planes' layout) with their half-norm plane hx, fused
+ * top-KC (16 or 32) only.  fp16 queries: a_hi the query rows, a_lo and a_scale null; one pass of exact products.  fp32
+ * queries: row r scaled by the power of two a_scale[r] [a_rows_pad] and split into fp16 a_hi + a_lo, two passes (hi + lo) * b;
+ * the scores come out unscaled.  Scores and lists as tc_scan_topk's.
+ */
+void tc_scan_f16(cudaStream_t stream, int device, const __half* a_hi, const __half* a_lo, const float* a_scale, int64_t a_rows_pad,
+                 const __half* b, int64_t b_rows_pad, int Kp, const __nv_bfloat16* hx, const tc_item* items_dev, int n_items, int KC,
+                 float* out_score, uint32_t* out_pos, int64_t out_row_stride, const tc_bound* bound, bool dynamic_schedule);
 
 }  // namespace b200

@@ -28,14 +28,18 @@ typedef cuvsBruteForceIndex* cuvsBruteForceIndex_t;
 CUVS_EXPORT cuvsError_t cuvsBruteForceIndexCreate(cuvsBruteForceIndex_t* index);
 CUVS_EXPORT cuvsError_t cuvsBruteForceIndexDestroy(cuvsBruteForceIndex_t index);
 
-/* dataset: [n, dim] f32, host or device, C- or F-contiguous. */
+/* dataset: [n, dim] float32, float16, int8 or uint8, host or device, C- or F-contiguous.  A float32 dataset that is
+ * C-contiguous in device memory is viewed, not copied, and must outlive the index.  float16, int8 and uint8 rows are copied
+ * into the index and kept in their own type (into the scan's zero-padded layout where the scan reads them), even when they
+ * are in device memory. */
 CUVS_EXPORT cuvsError_t cuvsBruteForceBuild(cuvsResources_t res,
                                             DLManagedTensor* dataset,
                                             cuvsDistanceType metric,
                                             float metric_arg,
                                             cuvsBruteForceIndex_t index);
 
-/* queries [nq, dim] f32 device; neighbors [nq, k] int64; distances [nq, k] f32. */
+/* queries [nq, dim] device, of the index's own type (a float16 index also takes float32 queries);
+ * neighbors [nq, k] int64; distances [nq, k] f32. */
 CUVS_EXPORT cuvsError_t cuvsBruteForceSearch(cuvsResources_t res,
                                              cuvsBruteForceIndex_t index,
                                              DLManagedTensor* queries,

@@ -29,12 +29,18 @@ CUVS_EXPORT int cuvsB200LastFlagged(void);
 CUVS_EXPORT long long cuvsB200KernelLaunches(void);
 
 /* Raw candidate output of the tensor-core scan of brute force (after the per-split merge):
- * cand_pos [nq, kc] uint32, cand_score [nq, kc] f32 (approximate selection-form distance). kc in {16, 32}. */
+ * cand_pos [nq, kc] uint32, cand_score [nq, kc] f32, the scan's score s = |x|^2/2 - q.x (L2 metrics), -q.x (inner product)
+ * or -cos of the unit rows (cosine), kc in {16, 32}.  queries: float32, or the index's own row type, as
+ * cuvsBruteForceSearch takes them.  On int8 / uint8 L2 and inner-product indexes the scores are exact (half the integer
+ * |x|^2 - 2 q.x for L2), and kc = 32 needs a dimension of at most 128. */
 CUVS_EXPORT cuvsError_t cuvsB200BruteForceCandidates(cuvsResources_t res,
                                                      cuvsBruteForceIndex_t index,
                                                      DLManagedTensor* queries,
                                                      DLManagedTensor* cand_pos,
                                                      DLManagedTensor* cand_score);
+/* Brute force: the element type the index keeps its rows in (*row_type: 0 float32, 1 float16, 2 int8, 3 uint8) and the device
+ * bytes the index owns (a float32 index built on a device view does not own the rows). */
+CUVS_EXPORT cuvsError_t cuvsB200BruteForceIndexInfo(cuvsBruteForceIndex_t index, int* row_type, int64_t* device_bytes);
 /* IVF-Flat list introspection (the reference exposes the equivalent only for IVF-PQ:
  * cuvsIvfPqIndexGetListSizes / cuvsIvfPqIndexGetListIndices).  Non-owning views into the index. */
 CUVS_EXPORT cuvsError_t cuvsB200IvfFlatGetListSizes(cuvsIvfFlatIndex_t index, DLManagedTensor* list_sizes /*[n_lists] u32*/);
