@@ -11,7 +11,7 @@
 //      register top-k' per query row per dataset split, no distance matrix in HBM;
 //   2. merge of the per-split lists (select_k.cu);
 //   3. exact fp32 re-scoring of the k' candidates in the oracle's arithmetic (exact.cu);
-//   4. a certificate (bf_certify_kernel): if the k-th exact distance is not strictly below the worst
+//   4. a certificate (certify_candidates): if the k-th exact distance is not strictly below the worst
 //      candidate's approximate distance minus the error budget, the query is flagged;
 //   5. flagged queries (ties / duplicates at the k' boundary) are recomputed by the exact SIMT
 //      path.  Result: identical to oracle/oracle.c::oracle_knn, bit for bit.
@@ -403,21 +403,6 @@ struct bf_cands {
   int width = 0;        // entries per query row in score / pos (KCm, or everything the scan kept when that is less)
 };
 
-// floor[q] = min over the query's lists of the list's last (= worst, lists are sorted best-first) entry; a list that is not
-// full ends in +inf and constrains nothing.  Every row the scan rejected — by a list's own k'-th entry or by the bound shared
-// between the splits, which is some full list's k'-th entry at an earlier time and only ever decreases — scores above it.
-__global__ void list_floor_kernel(const float* __restrict__ cs, int64_t nq, int64_t row_stride, int KC, float* __restrict__ out)
-{
-  const int64_t q = (blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x) >> 5;
-  const int lane  = threadIdx.x & 31;
-  if (q >= nq) return;
-  float m = INFINITY;
-  for (int64_t l = lane; l * KC < row_stride; l += 32) m = fminf(m, cs[q * row_stride + l * KC + KC - 1]);
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) m = fminf(m, __shfl_xor_sync(0xffffffffu, m, o));
-  if (lane == 0) out[q] = m;
-}
-
 // Stage 1+2 of the search: wgmma scan over `splits` dataset ranges (lists of KC per column half and split) +
 // merge to KCm per query (KCm == KC: the merged set's worst entry bounds everything outside it; KCm > KC, used for k above
 // the fused list length: `out.floor` carries the bound for the rows that never entered a list).  The scan is split-bf16 over
@@ -505,9 +490,7 @@ static void bf_tc_candidates(resources* res, const bf_index& idx, const float* q
   }
   if (KCm > KC) {
     out.floor.alloc(static_cast<size_t>(nq), stream);
-    count_launch();
-    list_floor_kernel<<<static_cast<unsigned>((nq * 32 + 255) / 256), 256, 0, stream>>>(cs.data(), nq, row_stride, KC, out.floor.data());
-    B2_CUDA(cudaGetLastError());
+    list_floors(stream, cs.data(), nq, row_stride, KC, out.floor.data());
   }
   out.width = static_cast<int>(std::min<int64_t>(row_stride, KCm));
   if (row_stride > KCm) {
@@ -520,13 +503,6 @@ static void bf_tc_candidates(resources* res, const bf_index& idx, const float* q
   }
 }
 
-/** How a raw scan score s of the tensor-core engine maps to the metric's selection form, and the
- *  error budget of that approximation:  A = sa*s + sb*|q|^2 + sc,  eps = eps_rel * (eq*|q|^2 + ec). */
-struct approx_map {
-  float sa = 1.f, sb = 0.f, sc = 0.f;
-  float eps_rel = 0.f, eq = 0.f, ec = 0.f;
-};
-
 static approx_map bf_approx_map(const bf_index& idx)
 {
   approx_map am;
@@ -537,65 +513,12 @@ static approx_map bf_approx_map(const bf_index& idx)
   am.eps_rel = std::max(1.0f / 32768.0f, 1.0f / 65536.0f + static_cast<float>(idx.Kp) / 16777216.0f);
   // 8-bit scans score exact integers; the budget covers the fp32 re-score's rounding against them (<= 2d ulps of
   // |q|^2 + |x|^2 for a sum of d products or squared differences and its finish) and the scores' conversion to fp32.  Below
-  // |q|^2 + max|x|^2 = 2^23 there is no rounding at all and the budget is 0 (bf_certify_kernel<true>).
+  // |q|^2 + max|x|^2 = 2^23 there is no rounding at all and the budget is 0 (certify_candidates' exact_ints).
   if (idx.i8_scan()) am.eps_rel = static_cast<float>(2 * idx.Kp + 8) / 16777216.0f;
   if (idx.metric == InnerProduct) { am.sa = -1.f; am.eq = 1.f; am.ec = idx.xn_max; }
   else if (idx.metric == CosineExpanded) { am.sa = 1.f; am.sc = 1.f; am.eq = 0.f; am.ec = 2.f; }
   else { am.sa = 2.f; am.sb = 1.f; am.eq = 1.f; am.ec = idx.xn_max; }
   return am;
-}
-
-// The certificate (DESIGN.md §3), one warp per query: flags[q] = 1 (flags[nq] counts them) unless the exact k-th distance
-// out_dist[q, k-1] (selection form, before postprocess_distances) beats the worst approximate score A of the rows outside the
-// candidates by more than eps_rel * (eq |q|^2 + ec).  Such rows exist when the candidate list is full and score worse than its
-// worst entry; with a floor (raw engine units, +inf: none), the bound of the rows that never entered a list, also worse than it.
-// kExactInts (8-bit scans): while m = |q|^2 + max|x|^2 < 2^23, every value the scan keys, the re-score and this kernel form is an
-// integer below 2^24 in magnitude (norms and partial sums <= m, distances <= 2m), so all of them are exact and eps is 0.
-template <bool kExactInts>
-__global__ void bf_certify_kernel(const float* __restrict__ cand_score, const uint32_t* __restrict__ cand_pos, int kc,
-                                  const float* __restrict__ approx_floor, const float* __restrict__ qn,
-                                  const float* __restrict__ out_dist, int k, approx_map amap, bool select_min, int64_t nq,
-                                  int* __restrict__ flags)
-{
-  const int64_t qi = (blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x) >> 5;
-  const int lane   = threadIdx.x & 31;
-  if (qi >= nq) return;
-  const float qnv    = qn[qi];
-  float worst_approx = select_min ? -FLT_MAX : FLT_MAX;
-  int n_valid        = 0;
-  for (int c = lane; c < kc; c += 32) {
-    if (cand_pos[qi * kc + c] == 0xffffffffu) continue;
-    ++n_valid;
-    float a      = amap.sa * cand_score[qi * kc + c] + amap.sb * qnv + amap.sc;
-    worst_approx = select_min ? fmaxf(worst_approx, a) : fminf(worst_approx, a);
-  }
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) {
-    n_valid += __shfl_xor_sync(0xffffffffu, n_valid, o);
-    float t = __shfl_xor_sync(0xffffffffu, worst_approx, o);
-    worst_approx = select_min ? fmaxf(worst_approx, t) : fminf(worst_approx, t);
-  }
-  if (lane != 0) return;
-  const float kth = out_dist[qi * k + k - 1];
-  int flag        = 0;
-  bool outside    = n_valid == kc;  // candidate list is full: rows outside it exist (dropped by the merge to kc)
-  if (approx_floor != nullptr) {
-    const float fl = approx_floor[qi];
-    if (fl < FLT_MAX) {
-      const float a = amap.sa * fl + amap.sb * qnv + amap.sc;
-      worst_approx  = !outside ? a : (select_min ? fminf(worst_approx, a) : fmaxf(worst_approx, a));
-      outside       = true;
-    }
-  }
-  if (outside) {
-    const float mag = amap.eq * qnv + amap.ec;
-    float eps       = amap.eps_rel * mag;
-    if (kExactInts && mag < 8388608.0f) eps = 0.f;
-    bool ok   = select_min ? (kth < worst_approx - eps) : (kth > worst_approx + eps);
-    flag      = ok ? 0 : 1;
-  }
-  flags[qi] = flag;
-  if (flag) atomicAdd(flags + nq, 1);
 }
 
 // qt: fp32 queries; q_narrow when they are the widened values of queries of the index's own narrow type
@@ -656,13 +579,8 @@ static void bf_search(resources* res, const bf_index& idx, const DLTensor& qt, c
 
   // ---- certificate, and the exact path for flagged queries (rare: exact ties / duplicates at the k' boundary)
   dbuf<int> flags(static_cast<size_t>(nq) + 1, stream);
-  B2_CUDA(cudaMemsetAsync(flags.data() + nq, 0, sizeof(int), stream));
-  count_launch();
-  auto certify = idx.i8_scan() ? bf_certify_kernel<true> : bf_certify_kernel<false>;
-  certify<<<blocks_for(nq * 32, 256), 256, 0, stream>>>(cand.score.data(), cand.pos.data(), cand.width, cand.floor.data(),
-                                                        cand.qn.data(), out_dist, k, bf_approx_map(idx), select_min, nq,
-                                                                  flags.data());
-  B2_CUDA(cudaGetLastError());
+  certify_candidates(stream, cand.score.data(), cand.pos.data(), cand.width, cand.floor.data(), cand.qn.data(), out_dist, k,
+                     bf_approx_map(idx), select_min, idx.i8_scan(), nq, flags.data());
   // search_exact answers every query on its own, and these run unfiltered, so the gathered rows get the same bits
   rerun_flagged(stream, flags.data(), nq, k, out_idx, out_dist, [&](const int64_t* rows, int64_t n, int64_t* fi, float* fd) {
     dbuf<float> fq(static_cast<size_t>(n) * idx.d, stream);

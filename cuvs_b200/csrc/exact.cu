@@ -70,7 +70,7 @@ __global__ void __launch_bounds__(256) exact_tile_kernel(const float* __restrict
                                                            const T* __restrict__ x, int64_t n, int64_t ldx, int d,
                                                            const float* __restrict__ qn, const float* __restrict__ xn,
                                                            int metric, float* __restrict__ out, int64_t ldo,
-                                                           filter_view filt, int64_t q_row0)
+                                                           filter_view filt, int64_t q_row0, bool self_clamp)
 {
   __shared__ float As[TK][TM + 1];
   __shared__ float Bs[TK][TN + 1];
@@ -124,7 +124,7 @@ __global__ void __launch_bounds__(256) exact_tile_kernel(const float* __restrict
     for (int j = 0; j < 4; ++j) {
       int64_t gc = col0 + tx * 4 + j;
       if (gc >= n) continue;
-      float v = finish_distance(acc[i][j], qnv, xn ? xn[gc] : 0.f, metric);
+      float v = finish_distance(acc[i][j], qnv, xn ? xn[gc] : 0.f, metric, self_clamp);
       if (!keep_sample(filt, q_row0 + gr, gc)) v = select_min ? FLT_MAX : -FLT_MAX;
       out[gr * ldo + gc] = v;
     }
@@ -142,7 +142,7 @@ __global__ void __launch_bounds__(128) rescore_kernel(const float* __restrict__ 
                                                        int metric, const uint32_t* __restrict__ cand_pos, int kc,
                                                        const int64_t* __restrict__ src_ids, int k,
                                                        int64_t* __restrict__ out_idx, float* __restrict__ out_dist,
-                                                       int64_t pad_id)
+                                                       int64_t pad_id, bool self_clamp)
 {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   const int warps = blockDim.x >> 5, wid = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -163,7 +163,7 @@ __global__ void __launch_bounds__(128) rescore_kernel(const float* __restrict__ 
     int64_t id   = INT64_MAX;
     if (pos != 0xffffffffu) {
       const float acc = exact_accumulate(qr, x + static_cast<int64_t>(pos) * ldx, d, vec4, metric);
-      dist            = finish_distance(acc, qnv, xn ? xn[pos] : 0.f, metric);
+      dist            = finish_distance(acc, qnv, xn ? xn[pos] : 0.f, metric, self_clamp);
       id   = src_ids ? src_ids[pos] : static_cast<int64_t>(pos);
     }
     sd[c] = dist;
@@ -202,7 +202,8 @@ __global__ void __launch_bounds__(256) rescore_block_kernel(const float* __restr
                                                              const float* __restrict__ xn, int metric,
                                                              const uint32_t* __restrict__ cand_pos, int kc, int kpow2,
                                                              const int64_t* __restrict__ src_ids, int k,
-                                                             int64_t* __restrict__ out_idx, float* __restrict__ out_dist, int64_t pad_id)
+                                                             int64_t* __restrict__ out_idx, float* __restrict__ out_dist, int64_t pad_id,
+                                                             bool self_clamp)
 {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   int64_t* si = reinterpret_cast<int64_t*>(smem_raw);
@@ -220,7 +221,7 @@ __global__ void __launch_bounds__(256) rescore_block_kernel(const float* __restr
     const uint32_t pos = c < kc ? cand_pos[qi * kc + c] : 0xffffffffu;
     if (pos != 0xffffffffu) {
       const float acc = exact_accumulate(qr, x + static_cast<int64_t>(pos) * ldx, d, vec4, metric);
-      dist            = finish_distance(acc, qnv, xn ? xn[pos] : 0.f, metric);
+      dist            = finish_distance(acc, qnv, xn ? xn[pos] : 0.f, metric, self_clamp);
       id   = src_ids ? src_ids[pos] : static_cast<int64_t>(pos);
     }
     sd[c] = dist;
@@ -263,6 +264,74 @@ __global__ void copy_rows_kernel(const T* __restrict__ src, const int64_t* __res
   dst[(dst_rows ? dst_rows[i] : i) * width + j] = src[(src_rows ? src_rows[i] : i) * width + j];
 }
 
+// floor[q] = min over the query's lists of the list's last (= worst, lists are sorted best-first) entry; a list that is not
+// full ends in +inf and constrains nothing.  Every row the scan rejected — by a list's own k'-th entry or by the bound shared
+// between the splits, which is some full list's k'-th entry at an earlier time and only ever decreases — scores above it.
+__global__ void list_floor_kernel(const float* __restrict__ cs, int64_t nq, int64_t row_stride, int KC, float* __restrict__ out)
+{
+  const int64_t q = (blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x) >> 5;
+  const int lane  = threadIdx.x & 31;
+  if (q >= nq) return;
+  float m = INFINITY;
+  for (int64_t l = lane; l * KC < row_stride; l += 32) m = fminf(m, cs[q * row_stride + l * KC + KC - 1]);
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) m = fminf(m, __shfl_xor_sync(0xffffffffu, m, o));
+  if (lane == 0) out[q] = m;
+}
+
+// The certificate (DESIGN.md §3), one warp per query: flags[q] = 1 (flags[nq] counts them) unless the exact k-th distance
+// out_dist[q, k-1] (selection form, before postprocess_distances) beats the worst approximate score A of the rows outside the
+// candidates by more than eps_rel * (eq |q|^2 + ec).  Such rows exist when the candidate list is full and score worse than its
+// worst entry; with a floor (raw engine units, +inf: none), the bound of the rows that never entered a list, also worse than it.
+// kExactInts (8-bit scans): while m = |q|^2 + max|x|^2 < 2^23, every value the scan keys, the re-score and this kernel form is an
+// integer below 2^24 in magnitude (norms and partial sums <= m, distances <= 2m), so all of them are exact and eps is 0.
+template <bool kExactInts>
+__global__ void certify_kernel(const float* __restrict__ cand_score, const uint32_t* __restrict__ cand_pos, int kc,
+                                  const float* __restrict__ approx_floor, const float* __restrict__ qn,
+                                  const float* __restrict__ out_dist, int k, approx_map amap, bool select_min, int64_t nq,
+                                  int* __restrict__ flags)
+{
+  const int64_t qi = (blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x) >> 5;
+  const int lane   = threadIdx.x & 31;
+  if (qi >= nq) return;
+  const float qnv    = qn[qi];
+  float worst_approx = select_min ? -FLT_MAX : FLT_MAX;
+  int n_valid        = 0;
+  for (int c = lane; c < kc; c += 32) {
+    if (cand_pos[qi * kc + c] == 0xffffffffu) continue;
+    ++n_valid;
+    float a      = amap.sa * cand_score[qi * kc + c] + amap.sb * qnv + amap.sc;
+    worst_approx = select_min ? fmaxf(worst_approx, a) : fminf(worst_approx, a);
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    n_valid += __shfl_xor_sync(0xffffffffu, n_valid, o);
+    float t = __shfl_xor_sync(0xffffffffu, worst_approx, o);
+    worst_approx = select_min ? fmaxf(worst_approx, t) : fminf(worst_approx, t);
+  }
+  if (lane != 0) return;
+  const float kth = out_dist[qi * k + k - 1];
+  int flag        = 0;
+  bool outside    = n_valid == kc;  // candidate list is full: rows outside it exist (dropped by the merge to kc)
+  if (approx_floor != nullptr) {
+    const float fl = approx_floor[qi];
+    if (fl < FLT_MAX) {
+      const float a = amap.sa * fl + amap.sb * qnv + amap.sc;
+      worst_approx  = !outside ? a : (select_min ? fminf(worst_approx, a) : fmaxf(worst_approx, a));
+      outside       = true;
+    }
+  }
+  if (outside) {
+    const float mag = amap.eq * qnv + amap.ec;
+    float eps       = amap.eps_rel * mag;
+    if (kExactInts && mag < 8388608.0f) eps = 0.f;
+    bool ok   = select_min ? (kth < worst_approx - eps) : (kth > worst_approx + eps);
+    flag      = ok ? 0 : 1;
+  }
+  flags[qi] = flag;
+  if (flag) atomicAdd(flags + nq, 1);
+}
+
 }  // namespace
 
 template <typename T>
@@ -296,7 +365,7 @@ void normalize_rows(cudaStream_t stream, float* x, int64_t n, int d, int64_t ld)
 template <typename T>
 void exact_distance_tile(cudaStream_t stream, const float* q, int64_t nq, int64_t ldq, const T* x, int64_t n,
                          int64_t ldx, int d, const float* qn, const float* xn, cuvsDistanceType metric, float* out,
-                         int64_t ldo, filter_view filt, int64_t q_row0)
+                         int64_t ldo, filter_view filt, int64_t q_row0, bool self_clamp)
 {
   if (nq == 0 || n == 0) return;
   dim3 grid(static_cast<unsigned>((n + TN - 1) / TN), static_cast<unsigned>((nq + TM - 1) / TM));
@@ -305,16 +374,18 @@ void exact_distance_tile(cudaStream_t stream, const float* q, int64_t nq, int64_
   count_launch();
   timed_section ts("exact_tile", stream);
   if (sq)
-    exact_tile_kernel<true, T><<<grid, 256, 0, stream>>>(q, nq, ldq, x, n, ldx, d, qn, xn, int(metric), out, ldo, filt, q_row0);
+    exact_tile_kernel<true, T><<<grid, 256, 0, stream>>>(q, nq, ldq, x, n, ldx, d, qn, xn, int(metric), out, ldo, filt, q_row0,
+                                                                         self_clamp);
   else
-    exact_tile_kernel<false, T><<<grid, 256, 0, stream>>>(q, nq, ldq, x, n, ldx, d, qn, xn, int(metric), out, ldo, filt, q_row0);
+    exact_tile_kernel<false, T><<<grid, 256, 0, stream>>>(q, nq, ldq, x, n, ldx, d, qn, xn, int(metric), out, ldo, filt, q_row0,
+                                                                         self_clamp);
   B2_CUDA(cudaGetLastError());
 }
 
 template <typename T>
 void rescore_topk(cudaStream_t stream, const float* q, int64_t nq, int64_t ldq, const T* x, int64_t ldx, int d,
                   const float* qn, const float* xn, cuvsDistanceType metric, const uint32_t* cand_pos, int kc,
-                  const int64_t* src_ids, int k, int64_t* out_idx, float* out_dist, int64_t pad_id)
+                  const int64_t* src_ids, int k, int64_t* out_idx, float* out_dist, int64_t pad_id, bool self_clamp)
 {
   if (nq == 0) return;
   if (kc > kMaxCand) {
@@ -324,7 +395,7 @@ void rescore_topk(cudaStream_t stream, const float* q, int64_t nq, int64_t ldq, 
     const size_t smem = static_cast<size_t>(kpow2) * (sizeof(int64_t) + sizeof(float) + sizeof(int));
     count_launch();
     rescore_block_kernel<T><<<static_cast<unsigned>(nq), 256, smem, stream>>>(q, ldq, x, ldx, d, qn, xn, int(metric), cand_pos, kc, kpow2,
-                                                                          src_ids, k, out_idx, out_dist, pad_id);
+                                                                          src_ids, k, out_idx, out_dist, pad_id, self_clamp);
     B2_CUDA(cudaGetLastError());
     return;
   }
@@ -333,17 +404,17 @@ void rescore_topk(cudaStream_t stream, const float* q, int64_t nq, int64_t ldq, 
   size_t smem     = static_cast<size_t>(warps) * kc * (sizeof(float) + sizeof(int64_t));
   count_launch();
   rescore_kernel<T><<<static_cast<unsigned>((nq + warps - 1) / warps), warps * 32, smem, stream>>>(
-    q, nq, ldq, x, ldx, d, qn, xn, int(metric), cand_pos, kc, src_ids, k, out_idx, out_dist, pad_id);
+    q, nq, ldq, x, ldx, d, qn, xn, int(metric), cand_pos, kc, src_ids, k, out_idx, out_dist, pad_id, self_clamp);
   B2_CUDA(cudaGetLastError());
 }
 
 #define B2_EXACT_ROW_TYPE(T)                                                                                            \
   template void row_norms<T>(cudaStream_t, const T*, int64_t, int, int64_t, float*);                                  \
   template void exact_distance_tile<T>(cudaStream_t, const float*, int64_t, int64_t, const T*, int64_t, int64_t, int,    \
-                                       const float*, const float*, cuvsDistanceType, float*, int64_t, filter_view, int64_t); \
+                                       const float*, const float*, cuvsDistanceType, float*, int64_t, filter_view, int64_t, bool); \
   template void rescore_topk<T>(cudaStream_t, const float*, int64_t, int64_t, const T*, int64_t, int, const float*,     \
                                 const float*, cuvsDistanceType, const uint32_t*, int, const int64_t*, int, int64_t*, float*, \
-                                int64_t);
+                                int64_t, bool);
 B2_EXACT_ROW_TYPE(float)
 B2_EXACT_ROW_TYPE(__half)
 B2_EXACT_ROW_TYPE(int8_t)
@@ -385,6 +456,26 @@ void rerun_flagged(cudaStream_t s, const int* flags, int64_t nq, int k, int64_t*
   copy_rows(s, fi.data(), nullptr, out_idx, rows.data(), n_flagged, k);
   copy_rows(s, fd.data(), nullptr, out_dist, rows.data(), n_flagged, k);
   B2_CUDA(cudaStreamSynchronize(s));  // hrows is host memory read by the copy above
+}
+
+void list_floors(cudaStream_t s, const float* cs, int64_t nq, int64_t row_stride, int KC, float* out)
+{
+  if (nq == 0) return;
+  count_launch();
+  list_floor_kernel<<<blocks_for(nq * 32, 256), 256, 0, s>>>(cs, nq, row_stride, KC, out);
+  B2_CUDA(cudaGetLastError());
+}
+
+void certify_candidates(cudaStream_t s, const float* cand_score, const uint32_t* cand_pos, int kc, const float* floor,
+                        const float* qn, const float* out_dist, int k, const approx_map& amap, bool select_min, bool exact_ints,
+                        int64_t nq, int* flags)
+{
+  B2_CUDA(cudaMemsetAsync(flags + nq, 0, sizeof(int), s));
+  if (nq == 0) return;
+  count_launch();
+  auto kernel = exact_ints ? certify_kernel<true> : certify_kernel<false>;
+  kernel<<<blocks_for(nq * 32, 256), 256, 0, s>>>(cand_score, cand_pos, kc, floor, qn, out_dist, k, amap, select_min, nq, flags);
+  B2_CUDA(cudaGetLastError());
 }
 
 void postprocess_distances(cudaStream_t stream, float* dist, int64_t count, cuvsDistanceType metric)

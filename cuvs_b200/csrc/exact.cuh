@@ -34,12 +34,13 @@ void normalize_rows(cudaStream_t stream, float* x, int64_t n, int d, int64_t ld)
  * Dense distance tile: out[i, j] = dist(q_i, x_j) for i < nq, j < n, in the metric's *selection*
  * form (squared for the L2Sqrt variants; plain dot for InnerProduct).  qn/xn: squared row norms
  * (needed for L2*Expanded and Cosine, may be null otherwise).  Filtered-out pairs get the worst
- * value.  `q_row0` is the global query index of row 0 (bitmap addressing).
+ * value.  `q_row0` is the global query index of row 0 (bitmap addressing).  self_clamp: finish_distance's self-neighbour rule
+ * for expanded L2 (false: clamp at 0 only, as k-means assignment does).
  */
 template <typename T>
 void exact_distance_tile(cudaStream_t stream, const float* q, int64_t nq, int64_t ldq, const T* x, int64_t n,
                          int64_t ldx, int d, const float* qn, const float* xn, cuvsDistanceType metric, float* out,
-                         int64_t ldo, filter_view filt, int64_t q_row0);
+                         int64_t ldo, filter_view filt, int64_t q_row0, bool self_clamp = true);
 
 /**
  * Re-score candidates exactly and keep the best k per query.
@@ -47,12 +48,12 @@ void exact_distance_tile(cudaStream_t stream, const float* q, int64_t nq, int64_
  *   src_ids            optional int64 map position -> source id (null: identity)
  * Output rows are sorted best-first, ties towards the smaller *source id*; missing entries get
  * id `pad_id` and +/-FLT_MAX.  kc <= 256 runs one warp per query; 256 < kc <= 2048 (k <= kc) one CTA per query with the
- * same arithmetic and ranking.
+ * same arithmetic and ranking.  self_clamp: as for exact_distance_tile.
  */
 template <typename T>
 void rescore_topk(cudaStream_t stream, const float* q, int64_t nq, int64_t ldq, const T* x, int64_t ldx, int d,
                   const float* qn, const float* xn, cuvsDistanceType metric, const uint32_t* cand_pos, int kc,
-                  const int64_t* src_ids, int k, int64_t* out_idx, float* out_dist, int64_t pad_id);
+                  const int64_t* src_ids, int k, int64_t* out_idx, float* out_dist, int64_t pad_id, bool self_clamp = true);
 
 /** dst[dst_rows[i]] = src[src_rows[i]] for n rows of `width` elements (a null row map is the identity).  T: float, int64_t,
  *  uint32_t. */
@@ -64,6 +65,29 @@ void copy_rows(cudaStream_t s, const T* src, const int64_t* src_rows, T* dst, co
  *  ascending) to idx / dist [n, k], which replace those rows of out_idx / out_dist [nq, k].  Synchronises the stream. */
 void rerun_flagged(cudaStream_t s, const int* flags, int64_t nq, int k, int64_t* out_idx, float* out_dist,
                    const std::function<void(const int64_t* rows, int64_t n, int64_t* idx, float* dist)>& answer);
+
+/** How a raw scan score s of the tensor-core engine maps to the metric's selection form, and the
+ *  error budget of that approximation:  A = sa*s + sb*|q|^2 + sc,  eps = eps_rel * (eq*|q|^2 + ec). */
+struct approx_map {
+  float sa = 1.f, sb = 0.f, sc = 0.f;
+  float eps_rel = 0.f, eq = 0.f, ec = 0.f;
+};
+
+/** out[q] = the smallest last entry of the sorted lists of KC (score) in row q of cs [nq, row_stride]: every row a full list
+ *  dropped scores at least that much (+inf when no list is full). */
+void list_floors(cudaStream_t s, const float* cs, int64_t nq, int64_t row_stride, int KC, float* out);
+
+/**
+ * The certificate of a candidate scan (DESIGN.md §3), one warp per query: flags[q] = 1 (flags[nq] counts them; this call
+ * zeroes it first) unless the exact k-th distance out_dist[q, k-1] (selection form) beats the approximate score A of every
+ * row outside the kc candidates (cand_score / cand_pos [nq, kc], raw engine units) by more than the budget of `amap`.  Rows
+ * outside exist when the candidate list is full, or, with a floor (raw units, +inf: none), below the rows that never entered
+ * a list.  exact_ints (8-bit scans): the budget is 0 while eq |q|^2 + ec < 2^23, where every value involved is an exact
+ * integer.
+ */
+void certify_candidates(cudaStream_t s, const float* cand_score, const uint32_t* cand_pos, int kc, const float* floor,
+                        const float* qn, const float* out_dist, int k, const approx_map& amap, bool select_min, bool exact_ints,
+                        int64_t nq, int* flags);
 
 /** In-place sqrt (L2Sqrt*) or sign/offset fix-ups applied after selection. */
 void postprocess_distances(cudaStream_t stream, float* dist, int64_t count, cuvsDistanceType metric);

@@ -9,14 +9,17 @@
 
 namespace b200 {
 
-__device__ __forceinline__ float finish_distance(float acc, float qn, float xn, int metric)
+/** The distance in selection form from exact_accumulate's sum.  Expanded L2 is clamped at 0 and, with `self_clamp` (searches:
+ *  l2_exp.cuh's self-neighbour rule), zeroed below 1e-3 between rows of equal norm; k-means assignment, like
+ *  oracle_kmeans_assign, clamps at 0 only. */
+__device__ __forceinline__ float finish_distance(float acc, float qn, float xn, int metric, bool self_clamp = true)
 {
   switch (metric) {
     case L2Expanded:
     case L2SqrtExpanded: {
       float val = fmaf(-2.0f, acc, qn + xn);
       if (!(val > 0.0f)) val = 0.0f;
-      if (val * val < 1e-6f && qn == xn) val = 0.0f;
+      if (self_clamp && val * val < 1e-6f && qn == xn) val = 0.0f;
       return val;
     }
     case CosineExpanded: return 1.0f - acc / (sqrtf(qn) * sqrtf(xn));

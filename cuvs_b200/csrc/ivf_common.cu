@@ -2,6 +2,7 @@
 #include "ivf_common.cuh"
 
 #include "exact.cuh"
+#include "exact_device.cuh"
 #include "hash.cuh"
 #include "select_k.cuh"
 #include "timing.hpp"
@@ -10,6 +11,7 @@
 #include <cfloat>
 #include <cmath>
 #include <cstdlib>
+#include <cstring>
 #include <functional>
 #include <vector>
 
@@ -554,17 +556,26 @@ __global__ void reseed_small_kernel(const float* __restrict__ x, int64_t n, int 
   }
 }
 
-// Inertia / convergence sum in a fixed order: per-warp partials of a fixed grid, then one warp adds them up (a double atomic
-// would round differently depending on arrival order, and `tol` would stop training after a different number of iterations).
-constexpr int kSumBlocks = 256, kSumThreads = 256, kSumParts = kSumBlocks * kSumThreads / 32;
-__global__ void __launch_bounds__(kSumThreads) sum_scores_kernel(const float* __restrict__ s, const float* __restrict__ xn, int64_t n,
-                                                                 double* __restrict__ parts)
+// The k-means cost in a fixed order: per-warp partials of a fixed grid, then one warp adds them up (a double atomic would round
+// differently depending on arrival order, and `tol` would stop training after a different number of iterations).  A row's
+// term is w_i * dist_i with dist_i = |x_i - c_{l_i}|^2 summed as the oracle's sqdiff (fmaf, ascending components), or its root;
+// w_i is 1 without weights and weights[i] * n / *w_sum with a weight sum.  x == null: the terms are the weights alone.
+constexpr int kCostBlocks = 256, kCostThreads = 256, kCostParts = kCostBlocks * kCostThreads / 32;
+__global__ void __launch_bounds__(kCostThreads) cost_parts_kernel(const float* __restrict__ x, int64_t n, int d,
+                                                                  const float* __restrict__ centers, const uint32_t* __restrict__ labels,
+                                                                  const float* __restrict__ w, const double* __restrict__ w_sum,
+                                                                  bool sqrt_dist, double* __restrict__ parts)
 {
-  double acc = 0;
+  const double scale = w_sum ? static_cast<double>(n) / *w_sum : 1.0;
+  const bool vec4    = x != nullptr && exact_vec4(x, d, centers, d, d);
+  double acc         = 0;
   for (int64_t i = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x; i < n;
        i += static_cast<int64_t>(gridDim.x) * blockDim.x) {
-    float dist = fmaf(2.0f, s[i], xn[i]);  // |x|^2 + 2 (|c|^2/2 - x.c)
-    acc += dist > 0.f ? dist : 0.0;
+    if (x == nullptr) { acc += static_cast<double>(w[i]); continue; }
+    const float dist = exact_accumulate(x + i * d, centers + static_cast<int64_t>(labels[i]) * d, d, vec4, L2Unexpanded);
+    double t         = sqrt_dist ? sqrt(static_cast<double>(dist)) : static_cast<double>(dist);
+    if (w) t *= static_cast<double>(w[i]) * scale;
+    acc += t;
   }
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
@@ -574,19 +585,45 @@ __global__ void __launch_bounds__(kSumThreads) sum_scores_kernel(const float* __
 __global__ void sum_parts_kernel(const double* __restrict__ parts, double* __restrict__ out)
 {
   double acc = 0;
-  for (int i = threadIdx.x; i < kSumParts; i += 32) acc += parts[i];
+  for (int i = threadIdx.x; i < kCostParts; i += 32) acc += parts[i];
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
   if (threadIdx.x == 0) *out = acc;
 }
 
-void sum_scores(cudaStream_t s, const float* scores, const float* xn, int64_t n, double* out)
+// one warp per row of dist [n, k]: the smallest entry, ties to the smaller column (the oracle's first minimum)
+__global__ void row_argmin_kernel(const float* __restrict__ dist, int64_t n, int k, int64_t* __restrict__ idx, float* __restrict__ out)
 {
-  dbuf<double> parts(static_cast<size_t>(kSumParts), s);
-  count_launch(2);
-  sum_scores_kernel<<<kSumBlocks, kSumThreads, 0, s>>>(scores, xn, n, parts.data());
-  sum_parts_kernel<<<1, 32, 0, s>>>(parts.data(), out);
-  B2_CUDA(cudaGetLastError());
+  const int64_t r = (blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x) >> 5;
+  const int lane  = threadIdx.x & 31;
+  if (r >= n) return;
+  float best = INFINITY;
+  int bj     = k;
+  for (int j = lane; j < k; j += 32) {
+    const float v = dist[r * k + j];
+    if (v < best) { best = v; bj = j; }
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    const float v = __shfl_xor_sync(0xffffffffu, best, o);
+    const int j   = __shfl_xor_sync(0xffffffffu, bj, o);
+    if (v < best || (v == best && j < bj)) { best = v; bj = j; }
+  }
+  if (lane == 0) { idx[r] = bj < k ? bj : 0; out[r] = best; }
+}
+
+// a row whose scan kept no candidate at all (every score NaN or infinite) has no re-scored best: certify_candidates sees no
+// row outside the empty list, so it is flagged here and takes the exact path
+__global__ void flag_empty_rows_kernel(const int64_t* __restrict__ best_id, int64_t n, int* __restrict__ flags)
+{
+  const int64_t i = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x;
+  if (i < n && best_id[i] < 0 && !flags[i]) { flags[i] = 1; atomicAdd(flags + n, 1); }
+}
+
+__global__ void i64_to_u32_kernel(const int64_t* __restrict__ in, uint32_t* __restrict__ out, int64_t n)
+{
+  const int64_t i = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x;
+  if (i < n) out[i] = static_cast<uint32_t>(in[i]);
 }
 
 }  // namespace
@@ -727,6 +764,86 @@ void assign_nearest(resources* res, const __nv_bfloat16* x_hi, const __nv_bfloat
                                                                scores ? scores + r0 : nullptr);
     B2_CUDA(cudaGetLastError());
   }
+}
+
+void assign_exact(resources* res, const float* x, const float* xn, const tc_rows_tmp& xp, const float* centers, const float* cn,
+                  const tc_rows& cp, uint32_t* labels)
+{
+  auto s          = res->stream;
+  const int64_t n = xp.n;
+  const int d = xp.d, k = static_cast<int>(cp.n);
+  if (n == 0) return;
+  B2_EXPECTS(xp.Kp == cp.Kp, "assign_exact: dimension mismatch");
+  // the certificate's budget (brute force's, DESIGN.md §3): A = 2 s + |x|^2 is within eps_rel (|x|^2 + max |c|^2) of the
+  // exact distance (a non-finite max |c|^2 makes the budget infinite: every row then takes the exact path)
+  approx_map am;
+  am.sa = 2.f; am.sb = 1.f; am.eq = 1.f;
+  const uint32_t cmax_bits = abs_max_host(s, cn, k);
+  std::memcpy(&am.ec, &cmax_bits, sizeof(float));
+  am.eps_rel = std::max(1.0f / 32768.0f, 1.0f / 65536.0f + static_cast<float>(xp.Kp) / 16777216.0f);
+  const int KC        = 16;
+  const int KCW       = KC * kTcListsPerItem;
+  const int64_t chunk = int64_t(1) << 20;  // rows per launch: bounds the (score, pos) scratch to 256 MiB
+  const int64_t rows0 = std::min(chunk, tc_pad_rows(n));
+  dbuf<float> cs(static_cast<size_t>(rows0) * KCW, s), best(static_cast<size_t>(rows0), s), floor(static_cast<size_t>(rows0), s);
+  dbuf<uint32_t> cpos(static_cast<size_t>(rows0) * KCW, s);
+  dbuf<int64_t> best_id(static_cast<size_t>(rows0), s);
+  dbuf<int> flags(static_cast<size_t>(rows0) + 1, s);
+  dbuf<tc_item> items(static_cast<size_t>(rows0 / 128), s);
+  // flagged rows per exact launch: their gathered rows and their distance tile each stay within 2^26 floats (256 MiB)
+  const int64_t step = std::min<int64_t>(std::max<int64_t>(1, (int64_t(1) << 26) / std::max(k, d)), int64_t(64) * 65535);
+  for (int64_t r0 = 0; r0 < n; r0 += chunk) {
+    const int64_t rows = std::min(chunk, n - r0);
+    const int m_tiles  = static_cast<int>(tc_pad_rows(rows) / 128);
+    count_launch();
+    iota_items_kernel<<<blocks_for(m_tiles, 128), 128, 0, s>>>(items.data(), m_tiles, rows, static_cast<uint32_t>(cp.rows_pad / 128), KCW);
+    B2_CUDA(cudaGetLastError());
+    tc_scan_topk(s, res->device, xp.hi.data() + r0 * xp.Kp, xp.lo.data() + r0 * xp.Kp, xp.rows_pad - r0, cp.hi.data(), cp.lo.data(),
+                 cp.rows_pad, xp.Kp, cp.hx.data(), items.data(), m_tiles, nullptr, KC, 3, cs.data(), cpos.data(), KCW);
+    const float* xc  = x + r0 * d;
+    const float* xnc = xn + r0;
+    // oracle_kmeans_assign's arithmetic: expanded L2 clamped at 0, without the searches' self-neighbour rule
+    rescore_topk(s, xc, rows, d, centers, d, d, xnc, cn, L2Expanded, cpos.data(), KCW, nullptr, 1, best_id.data(), best.data(), -1,
+                 false);
+    list_floors(s, cs.data(), rows, KCW, KC, floor.data());
+    certify_candidates(s, cs.data(), cpos.data(), KCW, floor.data(), xnc, best.data(), 1, am, true, false, rows, flags.data());
+    count_launch();
+    flag_empty_rows_kernel<<<blocks_for(rows, 256), 256, 0, s>>>(best_id.data(), rows, flags.data());
+    B2_CUDA(cudaGetLastError());
+    // rows the certificate rejects: distances to every centre (exact_distance_tile, the re-score's arithmetic), first minimum
+    rerun_flagged(s, flags.data(), rows, 1, best_id.data(), best.data(), [&](const int64_t* fr, int64_t nf, int64_t* fi, float* fd) {
+      const int64_t m0 = std::min(step, nf);
+      dbuf<float> fx(static_cast<size_t>(m0) * d, s), fxn(static_cast<size_t>(m0), s), tile(static_cast<size_t>(m0) * k, s);
+      for (int64_t f0 = 0; f0 < nf; f0 += step) {
+        const int64_t m = std::min(step, nf - f0);
+        copy_rows(s, xc, fr + f0, fx.data(), nullptr, m, d);
+        copy_rows(s, xnc, fr + f0, fxn.data(), nullptr, m, 1);
+        exact_distance_tile(s, fx.data(), m, d, centers, k, d, d, fxn.data(), cn, L2Expanded, tile.data(), k, filter_view{}, 0, false);
+        count_launch();
+        row_argmin_kernel<<<blocks_for(m * 32, 256), 256, 0, s>>>(tile.data(), m, k, fi + f0, fd + f0);
+        B2_CUDA(cudaGetLastError());
+      }
+    });
+    count_launch();
+    i64_to_u32_kernel<<<blocks_for(rows, 256), 256, 0, s>>>(best_id.data(), labels + r0, rows);
+    B2_CUDA(cudaGetLastError());
+  }
+}
+
+void kmeans_cost(cudaStream_t s, const float* x, int64_t n, int d, const float* centers, const uint32_t* labels, const float* weights,
+                 bool normalize_weight, bool sqrt_dist, double* out)
+{
+  dbuf<double> parts(static_cast<size_t>(kCostParts), s), w_sum;
+  if (weights != nullptr && normalize_weight) {
+    w_sum.alloc(1, s);
+    count_launch(2);
+    cost_parts_kernel<<<kCostBlocks, kCostThreads, 0, s>>>(nullptr, n, 0, nullptr, nullptr, weights, nullptr, false, parts.data());
+    sum_parts_kernel<<<1, 32, 0, s>>>(parts.data(), w_sum.data());
+  }
+  count_launch(2);
+  cost_parts_kernel<<<kCostBlocks, kCostThreads, 0, s>>>(x, n, d, centers, labels, weights, w_sum.data(), sqrt_dist, parts.data());
+  sum_parts_kernel<<<1, 32, 0, s>>>(parts.data(), out);
+  B2_CUDA(cudaGetLastError());
 }
 
 void bucket_probes(resources* res, const uint32_t* probes, int64_t nq, int n_probes, int64_t n_lists,
@@ -894,6 +1011,21 @@ bool merge_probe_candidates(cudaStream_t s, const float* cs, const uint32_t* cp,
   return true;
 }
 
+uint32_t abs_max_host(cudaStream_t s, const float* x, int64_t count)
+{
+  dbuf<uint32_t> bits(1, s);
+  B2_CUDA(cudaMemsetAsync(bits.data(), 0, sizeof(uint32_t), s));
+  uint32_t h = 0;
+  if (count > 0) {
+    count_launch();
+    abs_max_kernel<<<static_cast<unsigned>(std::min<int64_t>(blocks_for(count, 256), 132 * 8)), 256, 0, s>>>(x, count, bits.data());
+    B2_CUDA(cudaGetLastError());
+  }
+  B2_CUDA(cudaMemcpyAsync(&h, bits.data(), sizeof(h), cudaMemcpyDeviceToHost, s));
+  B2_CUDA(cudaStreamSynchronize(s));
+  return h;
+}
+
 void abs_max_bits(cudaStream_t s, const float* x, int64_t count, uint32_t* out_bits)
 {
   B2_CUDA(cudaMemsetAsync(out_bits, 0, sizeof(uint32_t), s));
@@ -921,7 +1053,7 @@ void update_centers(cudaStream_t s, const float* x, int64_t n, int d, const uint
 }
 
 void kmeans_train(resources* res, const float* x, int64_t n, int d, int k, int n_iters, float* centers, bool init_from_data,
-                  bool balance, double* inertia, int* iters_done, double tol)
+                  bool balance, double* inertia, int* iters_done, double tol, bool sqrt_cost, bool exact_loop)
 {
   auto s = res->stream;
   B2_EXPECTS(n >= 1 && k >= 1, "kmeans: empty input");
@@ -934,8 +1066,7 @@ void kmeans_train(resources* res, const float* x, int64_t n, int d, int k, int n
   // data-side planes (the dataset plays the "query" role of the scan)
   tc_rows_tmp xp;
   xp.build(s, x, n, d, true);
-  dbuf<float> xn(static_cast<size_t>(n), s), cn(static_cast<size_t>(k), s), counts(static_cast<size_t>(k), s),
-    scores(static_cast<size_t>(n), s);
+  dbuf<float> xn(static_cast<size_t>(n), s), cn(static_cast<size_t>(k), s), counts(static_cast<size_t>(k), s);
   dbuf<uint32_t> x_max(1, s);
   abs_max_bits(s, x, n * d, x_max.data());
   dbuf<uint32_t> labels(static_cast<size_t>(n), s);
@@ -948,8 +1079,11 @@ void kmeans_train(resources* res, const float* x, int64_t n, int d, int k, int n
   for (; it < std::max(n_iters, 1); ++it) {
     row_norms(s, centers, k, d, d, cn.data());
     cp.build(s, centers, k, d, cn.data(), true);
-    assign_nearest(res, xp.hi.data(), xp.lo.data(), n, xp.rows_pad, xp.Kp, cp, labels.data(), scores.data());
+    if (exact_loop) assign_exact(res, x, xn.data(), xp, centers, cn.data(), cp, labels.data());
+    else assign_nearest(res, xp.hi.data(), xp.lo.data(), n, xp.rows_pad, xp.Kp, cp, labels.data(), nullptr);
     if (n_iters == 0) break;  // assignment only
+    // the convergence sum: the cost of this iteration's centres, before the update moves them
+    if (tol > 0.0) kmeans_cost(s, x, n, d, centers, labels.data(), nullptr, false, sqrt_cost, acc.data());
     update_centers(s, x, n, d, labels.data(), x_max.data(), k, centers, counts.data());
     if (balance && k > 1) {
       B2_CUDA(cudaMemsetAsync(n_reseeded.data(), 0, sizeof(int), s));
@@ -959,7 +1093,6 @@ void kmeans_train(resources* res, const float* x, int64_t n, int d, int k, int n
       B2_CUDA(cudaGetLastError());
     }
     if (tol > 0.0) {
-      sum_scores(s, scores.data(), xn.data(), n, acc.data());
       double cur = 0;
       B2_CUDA(cudaMemcpyAsync(&cur, acc.data(), sizeof(double), cudaMemcpyDeviceToHost, s));
       B2_CUDA(cudaStreamSynchronize(s));
@@ -969,11 +1102,11 @@ void kmeans_train(resources* res, const float* x, int64_t n, int d, int k, int n
   }
   if (iters_done) *iters_done = it;
   if (inertia) {
-    // inertia of the returned centres
+    // inertia of the returned centres: exact labels, cost from differences
     row_norms(s, centers, k, d, d, cn.data());
     cp.build(s, centers, k, d, cn.data(), true);
-    assign_nearest(res, xp.hi.data(), xp.lo.data(), n, xp.rows_pad, xp.Kp, cp, labels.data(), scores.data());
-    sum_scores(s, scores.data(), xn.data(), n, acc.data());
+    assign_exact(res, x, xn.data(), xp, centers, cn.data(), cp, labels.data());
+    kmeans_cost(s, x, n, d, centers, labels.data(), nullptr, false, sqrt_cost, acc.data());
     B2_CUDA(cudaMemcpyAsync(inertia, acc.data(), sizeof(double), cudaMemcpyDeviceToHost, s));
     B2_CUDA(cudaStreamSynchronize(s));
   }

@@ -53,6 +53,28 @@ void assign_nearest(resources* res, const __nv_bfloat16* x_hi, const __nv_bfloat
                     int Kp, const tc_rows& centers, uint32_t* labels, float* scores /*nullable*/);
 
 /**
+ * Exact nearest centres (DESIGN.md §8): labels[i] = the first j minimising the oracle's expanded distance
+ * fmaf(-2, x_i.c_j, |x_i|^2 + |c_j|^2), clamped at 0 (oracle_kmeans_assign: rescore_topk's L2Expanded arithmetic without the
+ * self-neighbour rule).  The scan of assign_nearest proposes 2 x 16 candidates per row, rescore_topk scores them exactly,
+ * certify_candidates checks with brute force's budget that no other centre can come first, and the rows it rejects, and rows
+ * with no candidate, are scored against every centre (exact_distance_tile), in launches of bounded size.  Every label is
+ * below k.
+ * x [n, d] fp32 rows with their squared norms xn (row_norms) and planes xp (with lo); centers [k, d] with cn and planes cp
+ * (with lo).  Synchronises the stream.
+ */
+void assign_exact(resources* res, const float* x, const float* xn, const tc_rows_tmp& xp, const float* centers, const float* cn,
+                  const tc_rows& cp, uint32_t* labels);
+
+/**
+ * The k-means cost sum_i w_i dist_i into *out (device double): dist_i = |x_i - c_{labels_i}|^2, summed in fp32 as the oracle's
+ * sqdiff (fmaf, ascending components), or with sqrt_dist its square root; w_i = 1 without weights, weights[i] with them, and
+ * weights[i] * n / sum(weights) with normalize_weight.  The terms are added in double in a fixed order, so a cost has the same
+ * bits in every run and for every caller.
+ */
+void kmeans_cost(cudaStream_t s, const float* x, int64_t n, int d, const float* centers, const uint32_t* labels, const float* weights,
+                 bool normalize_weight, bool sqrt_dist, double* out);
+
+/**
  * (query, probe) pairs bucketed by list, on the device.
  *   slot_of[q * n_probes + p]  -> row of the pair in list-major order (0xffffffff for padded probes)
  *   pair_query[slot]           -> query id
@@ -146,10 +168,14 @@ dbuf<float> train_subsample(cudaStream_t s, const DLTensor& ds, uint32_t n_lists
  * Balanced-ish Lloyd k-means on the device (fp32 data, wgmma assignment).  `centers` [k, d] is
  * initialised from evenly strided rows when `init_from_data`, then refined for `n_iters` iterations;
  * clusters smaller than 1/4 of the average are re-seeded from members of large clusters each iteration.
- * Returns inertia of the final assignment when `inertia` != null (approximate scores).
+ * Each iteration assigns with assign_exact when `exact_loop` (cuvsKMeansFit: every update is the mean over the oracle's
+ * labels), else with the approximate assign_nearest (IVF builds' coarse training, DESIGN.md §8).
+ * With `tol` > 0 training stops once the cost changes by at most tol x the previous cost.  `inertia` != null receives the
+ * kmeans_cost of the returned centres over exact labels (sqrt_cost: sum of distances, L2SqrtExpanded).
  */
 void kmeans_train(resources* res, const float* x, int64_t n, int d, int k, int n_iters, float* centers,
-                  bool init_from_data, bool balance, double* inertia, int* iters_done, double tol = 0.0);
+                  bool init_from_data, bool balance, double* inertia, int* iters_done, double tol = 0.0, bool sqrt_cost = false,
+                  bool exact_loop = false);
 
 /**
  * Deterministic sums for the training loops (k-means centres, PQ codebooks).  Float atomics round differently depending on
@@ -158,6 +184,9 @@ void kmeans_train(resources* res, const float* x, int64_t n, int d, int k, int n
  * largest |v| of the input (abs_max_bits) and the number of terms n so that no sum can overflow:  |v| * 2^e * n < 2^62.
  */
 void abs_max_bits(cudaStream_t s, const float* x, int64_t count, uint32_t* out_bits /*device, one word*/);
+/** max |v| over the count values of x as fp32 bits, on the host (0x7f800000 or more: x holds an infinity or a NaN).
+ *  Synchronises the stream. */
+uint32_t abs_max_host(cudaStream_t s, const float* x, int64_t count);
 __device__ __forceinline__ double fixed_scale(uint32_t max_bits, int64_t n)
 {
   int ex = 0;

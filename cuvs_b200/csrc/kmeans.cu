@@ -4,9 +4,10 @@
 //   cpp/src/cluster/detail/minClusterDistanceCompute.cu:18-165 — where the reference *disables* its fused
 //   kernel (kmeans_common.cuh:60-84) and runs cuBLAS GEMM into an n x k fp32 matrix + reduce_min_kernel
 //   (unfused_distance_nn.cuh:54-118), i.e. n*k*4 bytes written and read back through HBM per iteration.
-// Here the assignment is the wgmma scan kernel with its fused top-1 epilogue (ivf_common.cu: assign_nearest):
-// the n x k score block lives in registers and shared memory only.  Lloyd iterations, centroid update (fixed-point int64 sums, the
-// same in every run: ivf_common.cuh) and the inertia reduction (fixed order) are plain CUDA; C wrapper semantics follow c/src/cluster/kmeans.cpp.
+// Here the assignment is the wgmma scan kernel with its fused top-k epilogue, re-scored and certified in the oracle's arithmetic
+// (ivf_common.cu: assign_exact): the n x k score block lives in registers and shared memory only.  Lloyd iterations, centroid
+// update (fixed-point int64 sums, the same in every run: ivf_common.cuh) and the cost (kmeans_cost: squared differences, fixed
+// order) are plain CUDA; C wrapper semantics follow c/src/cluster/kmeans.cpp.
 #include "common.hpp"
 #include "exact.cuh"
 #include "hash.cuh"
@@ -28,31 +29,6 @@ __global__ void u32_to_i32_kernel(const uint32_t* in, int32_t* out, int64_t n)
 {
   int64_t i = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x;
   if (i < n) out[i] = static_cast<int32_t>(in[i]);
-}
-
-// cost in a fixed order (per-warp partials of a fixed grid, then one warp): the same value in every run
-constexpr int kCostBlocks = 256, kCostThreads = 256, kCostParts = kCostBlocks * kCostThreads / 32;
-__global__ void __launch_bounds__(kCostThreads) weighted_cost_kernel(const float* __restrict__ s, const float* __restrict__ xn,
-                                                                     const float* __restrict__ w, int64_t n, double* __restrict__ parts)
-{
-  double acc = 0;
-  for (int64_t i = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x; i < n; i += static_cast<int64_t>(gridDim.x) * blockDim.x) {
-    float dist = fmaf(2.0f, s[i], xn[i]);
-    if (dist < 0.f) dist = 0.f;  // unfused_distance_nn.cuh:79-83 clamps at 0
-    acc += static_cast<double>(w ? w[i] * dist : dist);
-  }
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
-  if ((threadIdx.x & 31) == 0) parts[(blockIdx.x * blockDim.x + threadIdx.x) >> 5] = acc;
-}
-
-__global__ void sum_cost_parts_kernel(const double* __restrict__ parts, double* __restrict__ out)
-{
-  double acc = 0;
-  for (int i = threadIdx.x; i < kCostParts; i += 32) acc += parts[i];
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
-  if (threadIdx.x == 0) *out = acc;
 }
 
 // ---- k-means++ seeding (D^2 sampling, one centre per step).  Sampling proportional to w_i is done as
@@ -129,26 +105,28 @@ void stage(resources* r, const DLTensor& t, dev_matrix& m, const char* name)
   }
 }
 
-// labels + inertia for fixed centroids
-void predict(resources* r, const float* x, int64_t n, int d, const float* centroids, int k, const float* weights, uint32_t* labels,
-             double* inertia)
+bool sqrt_metric(cuvsDistanceType m) { return m == L2SqrtExpanded || m == L2SqrtUnexpanded; }
+
+// exact labels (assign_exact) + the cost of fixed centroids (kmeans_cost: weights, their normalisation, sqrt metrics)
+void predict(resources* r, const float* x, int64_t n, int d, const float* centroids, int k, const float* weights, bool normalize_weight,
+             bool sqrt_cost, uint32_t* labels, double* inertia)
 {
   auto s = r->stream;
   B2_EXPECTS(tc_supported(r->device, d), "kmeans: dim %d is not supported: it pads to more than %d columns, the widest the tensor-core kernels take", d, kTcMaxK);
+  // fit refuses non-finite data (abs_max_bits); predict and cluster cost refuse it too, before any row is assigned
+  B2_EXPECTS(abs_max_host(s, x, n * d) < 0x7f800000u, "kmeans: X contains NaN or infinity");
+  B2_EXPECTS(abs_max_host(s, centroids, static_cast<int64_t>(k) * d) < 0x7f800000u, "kmeans: centroids contain NaN or infinity");
   tc_rows_tmp xp;
   xp.build(s, x, n, d, true);
-  dbuf<float> cn(static_cast<size_t>(k), s), xn(static_cast<size_t>(n), s), scores(static_cast<size_t>(n), s);
+  dbuf<float> cn(static_cast<size_t>(k), s), xn(static_cast<size_t>(n), s);
   row_norms(s, centroids, k, d, d, cn.data());
   row_norms(s, x, n, d, d, xn.data());
   tc_rows cp;
   cp.build(s, centroids, k, d, cn.data(), true);
-  assign_nearest(r, xp.hi.data(), xp.lo.data(), n, xp.rows_pad, xp.Kp, cp, labels, scores.data());
+  assign_exact(r, x, xn.data(), xp, centroids, cn.data(), cp, labels);
   if (inertia) {
     dbuf<double> acc(1, s);
-    dbuf<double> parts(static_cast<size_t>(kCostParts), s);
-    count_launch(2);
-    weighted_cost_kernel<<<kCostBlocks, kCostThreads, 0, s>>>(scores.data(), xn.data(), weights, n, parts.data());
-    sum_cost_parts_kernel<<<1, 32, 0, s>>>(parts.data(), acc.data());
+    kmeans_cost(s, x, n, d, centroids, labels, weights, normalize_weight, sqrt_cost, acc.data());
     B2_CUDA(cudaMemcpyAsync(inertia, acc.data(), sizeof(double), cudaMemcpyDeviceToHost, s));
     B2_CUDA(cudaStreamSynchronize(s));
   }
@@ -187,7 +165,8 @@ void fit(resources* r, const fit_args& a, DLManagedTensor* X, DLManagedTensor* s
     kmeanspp_init(r, x.p, x.n, x.d, a.n_clusters, c);
     strided = false;
   }
-  kmeans_train(r, x.p, x.n, x.d, a.n_clusters, max_iter, c, strided, a.balanced, &cost, &iters, a.balanced ? 0.0 : a.tol);
+  kmeans_train(r, x.p, x.n, x.d, a.n_clusters, max_iter, c, strided, a.balanced, &cost, &iters, a.balanced ? 0.0 : a.tol,
+               sqrt_metric(a.metric), true);
   if (inertia) *inertia = cost;
   if (n_iter) *n_iter = iters;
 }
@@ -236,11 +215,14 @@ cuvsError_t cuvsKMeansFit_v2(cuvsResources_t res, cuvsKMeansParams_v2_t p, DLMan
   });
 }
 
-static void predict_c(cuvsResources_t res, DLManagedTensor* X, DLManagedTensor* sample_weight, DLManagedTensor* centroids,
-                      DLManagedTensor* labels, bool normalize_weight, double* inertia)
+static void predict_c(cuvsResources_t res, cuvsDistanceType metric, DLManagedTensor* X, DLManagedTensor* sample_weight,
+                      DLManagedTensor* centroids, DLManagedTensor* labels, bool normalize_weight, double* inertia)
 {
   auto r = as_res(res);
   B2_EXPECTS(X && centroids && labels, "null argument");
+  // the reference's kmeans_predict takes these two only (detail/kmeans.cuh)
+  B2_EXPECTS(metric == L2Expanded || metric == L2SqrtExpanded, "kmeans only supports L2Expanded or L2SqrtExpanded distance metrics, got %d",
+             int(metric));
   dev_matrix x;
   stage(r, X->dl_tensor, x, "X");
   const DLTensor& ct = centroids->dl_tensor;
@@ -248,29 +230,34 @@ static void predict_c(cuvsResources_t res, DLManagedTensor* X, DLManagedTensor* 
   B2_EXPECTS(dl_is(ct, kDLFloat, 32) && ct.ndim == 2 && ct.shape[1] == x.d && dl_is_device(ct) && dl_is_c_contiguous(ct), "centroids must be a device float32 [k, dim] matrix");
   B2_EXPECTS((dl_is(lt, kDLInt, 32) || dl_is(lt, kDLUInt, 32)) && lt.shape[0] == x.n && dl_is_device(lt), "labels must be a device int32 [n] vector");
   const float* w = nullptr;
-  dbuf<float> wbuf;
   if (sample_weight) {
     const DLTensor& wt = sample_weight->dl_tensor;
     B2_EXPECTS(dl_is(wt, kDLFloat, 32) && wt.shape[0] == x.n && dl_is_device(wt), "sample_weight must be a device float32 [n] vector");
     w = dl_ptr<float>(wt);
-    (void)normalize_weight;  // weights are used as given for the cost; normalisation only rescales inertia in the reference
   }
   dbuf<uint32_t> tmp(static_cast<size_t>(x.n), r->stream);
-  predict(r, x.p, x.n, x.d, dl_ptr<float>(ct), static_cast<int>(ct.shape[0]), w, tmp.data(), inertia);
+  predict(r, x.p, x.n, x.d, dl_ptr<float>(ct), static_cast<int>(ct.shape[0]), w, normalize_weight, sqrt_metric(metric), tmp.data(),
+          inertia);
   count_launch();
   u32_to_i32_kernel<<<blocks_for(x.n, 256), 256, 0, r->stream>>>(tmp.data(), dl_ptr<int32_t>(lt), x.n);
   B2_CUDA(cudaGetLastError());
 }
 
-cuvsError_t cuvsKMeansPredict(cuvsResources_t res, cuvsKMeansParams_t, DLManagedTensor* X, DLManagedTensor* sample_weight,
+cuvsError_t cuvsKMeansPredict(cuvsResources_t res, cuvsKMeansParams_t p, DLManagedTensor* X, DLManagedTensor* sample_weight,
                               DLManagedTensor* centroids, DLManagedTensor* labels, bool normalize_weight, double* inertia)
 {
-  return guarded([=] { predict_c(res, X, sample_weight, centroids, labels, normalize_weight, inertia); });
+  return guarded([=] {
+    B2_EXPECTS(p != nullptr, "params is null");
+    predict_c(res, p->metric, X, sample_weight, centroids, labels, normalize_weight, inertia);
+  });
 }
-cuvsError_t cuvsKMeansPredict_v2(cuvsResources_t res, cuvsKMeansParams_v2_t, DLManagedTensor* X, DLManagedTensor* sample_weight,
+cuvsError_t cuvsKMeansPredict_v2(cuvsResources_t res, cuvsKMeansParams_v2_t p, DLManagedTensor* X, DLManagedTensor* sample_weight,
                                  DLManagedTensor* centroids, DLManagedTensor* labels, bool normalize_weight, double* inertia)
 {
-  return guarded([=] { predict_c(res, X, sample_weight, centroids, labels, normalize_weight, inertia); });
+  return guarded([=] {
+    B2_EXPECTS(p != nullptr, "params is null");
+    predict_c(res, p->metric, X, sample_weight, centroids, labels, normalize_weight, inertia);
+  });
 }
 
 cuvsError_t cuvsKMeansClusterCost(cuvsResources_t res, DLManagedTensor* X, DLManagedTensor* centroids, double* cost)
@@ -283,7 +270,7 @@ cuvsError_t cuvsKMeansClusterCost(cuvsResources_t res, DLManagedTensor* X, DLMan
     const DLTensor& ct = centroids->dl_tensor;
     B2_EXPECTS(dl_is(ct, kDLFloat, 32) && ct.ndim == 2 && ct.shape[1] == x.d && dl_is_device(ct) && dl_is_c_contiguous(ct), "centroids must be a device float32 [k, dim] matrix");
     dbuf<uint32_t> tmp(static_cast<size_t>(x.n), r->stream);
-    predict(r, x.p, x.n, x.d, dl_ptr<float>(ct), static_cast<int>(ct.shape[0]), nullptr, tmp.data(), cost);
+    predict(r, x.p, x.n, x.d, dl_ptr<float>(ct), static_cast<int>(ct.shape[0]), nullptr, false, false, tmp.data(), cost);
   });
 }
 
