@@ -23,6 +23,7 @@
 // rows.  The re-score and the exact path read the typed rows and widen each element on load.
 #include "common.hpp"
 #include "exact.cuh"
+#include "ivf_common.cuh"  // abs_max_host
 #include "npy_io.hpp"
 #include "scan_tc.cuh"
 #include "select_k.cuh"
@@ -41,16 +42,13 @@
 
 namespace b200 {
 
-// The element type of a brute-force index's rows (cuvsB200BruteForceIndexInfo's row_type)
-constexpr int kBfF32 = 0, kBfF16 = 1, kBfS8 = 2, kBfU8 = 3;
-
 struct bf_index {
   int64_t n   = 0;
   int d       = 0;
   int device  = 0;
   cuvsDistanceType metric = L2Expanded;
   float metric_arg        = 2.0f;
-  int row_type            = kBfF32;
+  row_type type          = row_type::f32;  // the element type of the rows
   const float* data       = nullptr;  // float32 rows: [n, d] row-major on the device (view or data_own)
   owned<float> data_own;
   // float16 / int8 / uint8 rows, `ld` elements apart: the scan's zero-padded operand [rows_pad, Kp] when the scan reads them
@@ -67,8 +65,8 @@ struct bf_index {
   owned<__nv_bfloat16> hx;  // [rows_pad, 16] half-norm plane (scan_tc.cuh) of the bf16 and fp16 scans
   owned<float> inv_norm;  // cosine only
   owned<int> norms8;      // 8-bit scans: [rows_pad] exact |x|^2, kI8PadNorm on padding rows
-  bool f16_scan() const { return tc && row_type == kBfF16 && metric != CosineExpanded; }
-  bool i8_scan() const { return tc && (row_type == kBfS8 || row_type == kBfU8) && metric != CosineExpanded; }
+  bool f16_scan() const { return tc && type == row_type::f16 && metric != CosineExpanded; }
+  bool i8_scan() const { return tc && row_bytes(type) == 1 && metric != CosineExpanded; }
   template <typename T>
   const T* rows_as() const { return reinterpret_cast<const T*>(rows.data()); }
   int64_t device_bytes() const
@@ -80,48 +78,21 @@ struct bf_index {
 
 namespace {
 
-int row_type_of(DLDataType t)
-{
-  if (t.code == kDLFloat) return t.bits == 16 ? kBfF16 : kBfF32;
-  return t.code == kDLInt ? kBfS8 : kBfU8;
-}
-DLDataType dtype_of(int row_type)
-{
-  switch (row_type) {
-    case kBfF16: return {kDLFloat, 16, 1};
-    case kBfS8: return {kDLInt, 8, 1};
-    case kBfU8: return {kDLUInt, 8, 1};
-    default: return {kDLFloat, 32, 1};
-  }
-}
-int elem_bytes(int row_type) { return row_type == kBfF32 ? 4 : (row_type == kBfF16 ? 2 : 1); }
-
 // f(rows, ld): the index's rows in their own element type
 template <typename F>
 void with_rows(const bf_index& idx, F&& f)
 {
-  switch (idx.row_type) {
-    case kBfF16: return f(idx.rows_as<__half>(), idx.ld);
-    case kBfS8: return f(idx.rows_as<int8_t>(), idx.ld);
-    case kBfU8: return f(idx.rows_as<uint8_t>(), idx.ld);
-    default: return f(idx.data, static_cast<int64_t>(idx.d));
-  }
+  with_row_type(idx.type, [&](auto t) {
+    using T = decltype(t);
+    if constexpr (std::is_same_v<T, float>) f(idx.data, static_cast<int64_t>(idx.d));
+    else f(idx.rows_as<T>(), idx.ld);
+  });
 }
 
 bool metric_supported(cuvsDistanceType m)
 {
   return m == L2Expanded || m == L2SqrtExpanded || m == L2Unexpanded || m == L2SqrtUnexpanded || m == InnerProduct ||
          m == CosineExpanded;
-}
-
-__global__ void transpose_kernel(const float* __restrict__ in, float* __restrict__ out, int64_t n, int d)
-{
-  // in: column-major [n, d] (element (r,c) at c*n + r) -> out row-major
-  int64_t t = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x;
-  if (t >= n * d) return;
-  int64_t r = t / d;
-  int c     = static_cast<int>(t % d);
-  out[t]    = in[static_cast<int64_t>(c) * n + r];
 }
 
 // column-major [n, d] elements of E bytes -> rows `ld` elements apart
@@ -133,23 +104,6 @@ __global__ void transpose_into_kernel(const E* __restrict__ in, E* __restrict__ 
   const int64_t r = t / d;
   const int c     = static_cast<int>(t % d);
   out[r * ld + c] = in[static_cast<int64_t>(c) * n + r];
-}
-
-// norms[r] = |x_r|^2 exactly over a padded 8-bit plane [rows_pad, Kp8], kI8PadNorm for r >= n.  One warp per row.
-template <bool U8>
-__global__ void i8_norms_kernel(const uint8_t* __restrict__ rows, int64_t n, int64_t rows_pad, int Kp8, int* __restrict__ norms)
-{
-  const int64_t r = (blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x) >> 5;
-  const int lane  = threadIdx.x & 31;
-  if (r >= rows_pad) return;
-  int acc = 0;
-  for (int j = lane; j < Kp8; j += 32) {
-    const int v = U8 ? static_cast<int>(rows[r * Kp8 + j]) : static_cast<int>(static_cast<int8_t>(rows[r * Kp8 + j]));
-    acc += v * v;
-  }
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
-  if (lane == 0) norms[r] = r < n ? acc : kI8PadNorm;
 }
 
 // The A operand of a narrow scan from fp32 query rows that hold values of type T (exact): [rows_pad, Kp], zero padded
@@ -203,35 +157,6 @@ __global__ void i8_keys_to_scores_kernel(float* __restrict__ v, int64_t count, f
   if (key < INFINITY) v[i] = mul * static_cast<float>(tc_i8_score(key));
 }
 
-__global__ void max_kernel(const float* __restrict__ v, int64_t n, float* __restrict__ out)
-{
-  float m = 0.f;
-  for (int64_t i = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x; i < n;
-       i += static_cast<int64_t>(gridDim.x) * blockDim.x)
-    m = fmaxf(m, v[i]);
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
-  if ((threadIdx.x & 31) == 0) atomicMax(reinterpret_cast<int*>(out), __float_as_int(m));  // m >= 0
-}
-
-__global__ void make_items_kernel(tc_item* items, int m_tiles, int splits, int64_t nq, uint32_t tiles_total, int KCW)
-{
-  int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= m_tiles * splits) return;
-  // item order: split-major, so that concurrently running CTAs stream the same dataset range (L2 reuse)
-  int s = i / m_tiles, m = i % m_tiles;
-  uint32_t per = (tiles_total + splits - 1) / splits;
-  uint32_t t0  = min(tiles_total, s * per), t1 = min(tiles_total, t0 + per);
-  tc_item it;
-  it.a_row0     = m * 128;
-  it.b_row0     = t0 * 128;
-  it.n_tiles    = t1 - t0;
-  int64_t valid = nq - static_cast<int64_t>(m) * 128;
-  it.valid_rows = valid > 128 ? 128 : static_cast<uint32_t>(valid);
-  it.out_off    = (static_cast<uint64_t>(m) * 128 * splits + s) * KCW;
-  items[i]      = it;
-}
-
 int pick_splits(int m_tiles, int64_t b_tiles, int sms)
 {
   int64_t s_max = std::max<int64_t>(1, std::min<int64_t>(32, b_tiles / 8));
@@ -259,7 +184,7 @@ static bf_index* bf_build(resources* res, const DLTensor& ds, cuvsDistanceType m
   idx->metric     = metric;
   idx->metric_arg = metric_arg;
   idx->device     = res->device;
-  idx->row_type   = row_type_of(ds.dtype);
+  idx->type       = row_type_of(ds.dtype);
   auto stream     = res->stream;
   const bool c_contig = dl_is_c_contiguous(ds), f_contig = dl_is_f_contiguous(ds);
   B2_EXPECTS(c_contig || f_contig, "dataset input to cuvsBruteForceBuild must be contiguous (non-strided)");
@@ -267,12 +192,12 @@ static bf_index* bf_build(resources* res, const DLTensor& ds, cuvsDistanceType m
   const size_t count = static_cast<size_t>(idx->n) * idx->d;
   idx->tc = tc_supported(res->device, idx->d) && idx->n >= 1 && idx->n < (int64_t(1) << 31);
   const bool l2 = (metric != InnerProduct && metric != CosineExpanded);
-  if (idx->row_type != kBfF32) {
+  if (idx->type != row_type::f32) {
     // float16 / int8 / uint8: the rows in their own type, in the scan's padded operand when the scan reads them
-    const int es   = elem_bytes(idx->row_type);
+    const int es   = static_cast<int>(row_bytes(idx->type));
     idx->rows_pad  = tc_pad_rows(idx->n);
     const bool pad = idx->f16_scan() || idx->i8_scan();
-    idx->Kp        = idx->row_type == kBfF16 || metric == CosineExpanded ? tc_pad_k(idx->d) : tc_pad_k_i8(idx->d);
+    idx->Kp        = idx->type == row_type::f16 || metric == CosineExpanded ? tc_pad_k(idx->d) : tc_pad_k_i8(idx->d);
     idx->ld        = pad ? idx->Kp : idx->d;
     const int64_t rows = pad ? idx->rows_pad : idx->n;
     idx->rows.alloc(static_cast<size_t>(rows * idx->ld * es));
@@ -302,29 +227,22 @@ static bf_index* bf_build(resources* res, const DLTensor& ds, cuvsDistanceType m
     } else {
       dbuf<float> tmp(count, stream);
       B2_CUDA(cudaMemcpyAsync(tmp.data(), src, count * sizeof(float), cudaMemcpyDefault, stream));
-      if (count) transpose_kernel<<<static_cast<unsigned>((count + 255) / 256), 256, 0, stream>>>(tmp.data(), idx->data_own.data(), idx->n, idx->d);
+      if (count)
+        transpose_into_kernel<<<blocks_for(static_cast<int64_t>(count), 256), 256, 0, stream>>>(tmp.data(), idx->data_own.data(), idx->n,
+                                                                                                idx->d, int64_t(idx->d));
       B2_CUDA(cudaGetLastError());
     }
     idx->data = idx->data_own.data();
   }
   idx->norms.alloc(static_cast<size_t>(std::max<int64_t>(idx->n, 1)));
   with_rows(*idx, [&](auto x, int64_t ld) { row_norms(stream, x, idx->n, idx->d, ld, idx->norms.data()); });
-  {
-    dbuf<float> mx(1, stream);
-    B2_CUDA(cudaMemsetAsync(mx.data(), 0, sizeof(float), stream));
-    if (idx->n) max_kernel<<<std::min<int64_t>(1024, (idx->n + 255) / 256), 256, 0, stream>>>(idx->norms.data(), idx->n, mx.data());
-    B2_CUDA(cudaGetLastError());
-    B2_CUDA(cudaMemcpyAsync(&idx->xn_max, mx.data(), sizeof(float), cudaMemcpyDeviceToHost, stream));
-    B2_CUDA(cudaStreamSynchronize(stream));
-  }
+  // the norms are >= 0: their largest |value|.  A NaN norm (a row holding NaN) ranks above +inf, so xn_max is NaN; the
+  // certificate's budget is then NaN and fails every query it is applied to: those queries take the exact path.
+  const uint32_t xn_max_bits = abs_max_host(stream, idx->norms.data(), idx->n);
+  std::memcpy(&idx->xn_max, &xn_max_bits, sizeof(float));
   if (idx->i8_scan()) {
     idx->norms8.alloc(static_cast<size_t>(idx->rows_pad));
-    count_launch();
-    if (idx->row_type == kBfU8)
-      i8_norms_kernel<true><<<blocks_for(idx->rows_pad * 32, 256), 256, 0, stream>>>(idx->rows.data(), idx->n, idx->rows_pad, idx->Kp, idx->norms8.data());
-    else
-      i8_norms_kernel<false><<<blocks_for(idx->rows_pad * 32, 256), 256, 0, stream>>>(idx->rows.data(), idx->n, idx->rows_pad, idx->Kp, idx->norms8.data());
-    B2_CUDA(cudaGetLastError());
+    tc_i8_norms(stream, idx->type == row_type::u8, idx->rows.data(), idx->rows_pad, idx->n, idx->Kp, nullptr, nullptr, 0, idx->norms8.data());
   } else if (idx->f16_scan()) {
     idx->hx.alloc(static_cast<size_t>(idx->rows_pad) * 16);
     tc_half_norms(stream, l2 ? idx->norms.data() : nullptr, idx->n, idx->rows_pad, idx->hx.data());
@@ -340,7 +258,7 @@ static bf_index* bf_build(resources* res, const DLTensor& ds, cuvsDistanceType m
       rsqrt_rows(stream, idx->norms.data(), idx->n, idx->inv_norm.data());
       scale = idx->inv_norm.data();
     }
-    if (idx->row_type == kBfF32) {
+    if (idx->type == row_type::f32) {
       tc_split_planes(stream, idx->data, idx->n, idx->d, idx->d, idx->Kp, idx->hi.data(), idx->lo.data(), idx->rows_pad, scale);
     } else {
       // cosine over narrow rows: the planes of the unit rows from bounded chunks of widened rows, which are not kept
@@ -349,7 +267,7 @@ static bf_index* bf_build(resources* res, const DLTensor& ds, cuvsDistanceType m
       for (int64_t r0 = 0; r0 < idx->n; r0 += chunk) {
         const int64_t c   = std::min(chunk, idx->n - r0);
         const int64_t pad = r0 + chunk >= idx->n ? idx->rows_pad - r0 : c;  // the last chunk zeroes the padding rows
-        widen_async(stream, idx->rows.data() + r0 * idx->ld * elem_bytes(idx->row_type), dtype_of(idx->row_type), c * idx->d, w.data());
+        widen_async(stream, idx->rows.data() + r0 * idx->ld * row_bytes(idx->type), dtype_of(idx->type), c * idx->d, w.data());
         tc_split_planes(stream, w.data(), c, idx->d, idx->d, idx->Kp, idx->hi.data() + r0 * idx->Kp, idx->lo.data() + r0 * idx->Kp,
                         pad, scale + r0);
       }
@@ -432,7 +350,7 @@ static void bf_tc_candidates(resources* res, const bf_index& idx, const float* q
     B2_EXPECTS(q_narrow, "brute_force: an 8-bit index is scanned with queries of its own type");
     q8.alloc(static_cast<size_t>(a_elems), stream);
     count_launch();
-    if (idx.row_type == kBfU8)
+    if (idx.type == row_type::u8)
       pack_queries_kernel<<<blocks_for(a_elems, 256), 256, 0, stream>>>(q, nq, idx.d, idx.Kp, nq_pad, q8.data());
     else
       pack_queries_kernel<<<blocks_for(a_elems, 256), 256, 0, stream>>>(q, nq, idx.d, idx.Kp, nq_pad, reinterpret_cast<int8_t*>(q8.data()));
@@ -461,9 +379,7 @@ static void bf_tc_candidates(resources* res, const bf_index& idx, const float* q
 
   dbuf<tc_item> items(static_cast<size_t>(n_items), stream);
   const int KCW = KC * kTcListsPerItem;  // candidates per (item, query row)
-  make_items_kernel<<<(n_items + 127) / 128, 128, 0, stream>>>(items.data(), m_tiles, splits, nq, static_cast<uint32_t>(b_tiles), KCW);
-  B2_CUDA(cudaGetLastError());
-  count_launch();
+  tc_split_items(stream, items.data(), m_tiles, splits, nq, static_cast<uint32_t>(b_tiles), KCW);
 
   const int64_t row_stride = static_cast<int64_t>(splits) * KCW;
   dbuf<float> cs(static_cast<size_t>(nq_pad) * row_stride, stream);
@@ -475,7 +391,7 @@ static void bf_tc_candidates(resources* res, const bf_index& idx, const float* q
   bnd.keys = bkeys.data();
   // equal-sized items in split-major order: static round-robin keeps each column range L2 resident
   if (idx.i8_scan()) {
-    tc_scan_i8(stream, res->device, idx.row_type == kBfU8, q8.data(), nq_pad, idx.rows.data(), idx.rows_pad, idx.Kp, idx.norms8.data(),
+    tc_scan_i8(stream, res->device, idx.type == row_type::u8, q8.data(), nq_pad, idx.rows.data(), idx.rows_pad, idx.Kp, idx.norms8.data(),
                idx.metric != InnerProduct, items.data(), n_items, nullptr, KC, cs.data(), cp.data(), row_stride, &bnd, false);
     count_launch();
     const int64_t cnt = nq_pad * row_stride;
@@ -539,7 +455,7 @@ static void bf_search(resources* res, const bf_index& idx, const DLTensor& qt, c
   if (!dl_is_c_contiguous(qt)) {
     B2_EXPECTS(dl_is_f_contiguous(qt), "queries input to cuvsBruteForceSearch must be contiguous (non-strided)");
     qcopy.alloc(static_cast<size_t>(nq) * idx.d, stream);
-    transpose_kernel<<<static_cast<unsigned>((nq * idx.d + 255) / 256), 256, 0, stream>>>(q, qcopy.data(), nq, idx.d);
+    transpose_into_kernel<<<blocks_for(nq * idx.d, 256), 256, 0, stream>>>(q, qcopy.data(), nq, idx.d, int64_t(idx.d));
     B2_CUDA(cudaGetLastError());
     q = qcopy.data();
   }
@@ -692,17 +608,17 @@ cuvsError_t cuvsBruteForceSerialize(cuvsResources_t res, const char* filename, c
     auto r = as_res(res);
     B2_EXPECTS(filename, "null argument");
     auto& idx    = index_of<bf_index>(index);
-    const int es = elem_bytes(idx.row_type);
+    const size_t es = row_bytes(idx.type);
     std::vector<char> host(static_cast<size_t>(idx.n) * idx.d * es);
-    const void* src      = idx.row_type == kBfF32 ? static_cast<const void*>(idx.data) : idx.rows.data();
-    const size_t pitch   = static_cast<size_t>(idx.row_type == kBfF32 ? idx.d : idx.ld) * es;
+    const void* src      = idx.type == row_type::f32 ? static_cast<const void*>(idx.data) : idx.rows.data();
+    const size_t pitch   = static_cast<size_t>(idx.type == row_type::f32 ? idx.d : idx.ld) * es;
     if (!host.empty())
       B2_CUDA(cudaMemcpy2DAsync(host.data(), static_cast<size_t>(idx.d) * es, src, pitch, static_cast<size_t>(idx.d) * es, idx.n,
                                 cudaMemcpyDeviceToHost, r->stream));
     B2_CUDA(cudaStreamSynchronize(r->stream));
     std::ofstream os(filename, std::ios::out | std::ios::binary);
     B2_EXPECTS(bool(os), "Cannot open file %s", filename);
-    const char* descr = npy::file_dtype_for(dtype_of(idx.row_type)).descr;  // "<f4", "<f2", "|i1", "|u1"
+    const char* descr = npy::file_dtype_for(dtype_of(idx.type)).descr;  // "<f4", "<f2", "|i1", "|u1"
     const char tag[4] = {descr[0], descr[1], descr[2], 0};
     os.write(tag, 4);
     int64_t n = idx.n, d = idx.d;
@@ -749,7 +665,7 @@ cuvsError_t cuvsB200BruteForceIndexInfo(cuvsBruteForceIndex_t index, int* row_ty
   return guarded([=] {
     B2_EXPECTS(row_type && device_bytes, "null argument");
     auto& idx     = index_of<bf_index>(index);
-    *row_type     = idx.row_type;
+    *row_type     = static_cast<int>(idx.type);
     *device_bytes = idx.device_bytes();
   });
 }

@@ -12,6 +12,7 @@
 #include <atomic>
 #include <cstring>
 #include <string>
+#include <type_traits>
 
 namespace b200 {
 
@@ -24,13 +25,15 @@ __global__ void widen_kernel(const T* __restrict__ in, int64_t n, float* __restr
 
 void widen_async(cudaStream_t s, const void* in, DLDataType dt, int64_t count, float* out)
 {
+  const row_type rt = row_type_of(dt);
+  B2_EXPECTS(rt != row_type::f32, "widen_async: the rows are float32 already");
   if (count == 0) return;
   const unsigned grid = static_cast<unsigned>((count + 255) / 256);
   count_launch();
-  if (dt.code == kDLFloat && dt.bits == 16) widen_kernel<__half><<<grid, 256, 0, s>>>(static_cast<const __half*>(in), count, out);
-  else if (dt.code == kDLInt && dt.bits == 8) widen_kernel<int8_t><<<grid, 256, 0, s>>>(static_cast<const int8_t*>(in), count, out);
-  else if (dt.code == kDLUInt && dt.bits == 8) widen_kernel<uint8_t><<<grid, 256, 0, s>>>(static_cast<const uint8_t*>(in), count, out);
-  else B2_FAIL("widen_async: unsupported dtype code %d bits %d", int(dt.code), int(dt.bits));
+  with_row_type(rt, [&](auto t) {
+    using T = decltype(t);
+    if constexpr (!std::is_same_v<T, float>) widen_kernel<T><<<grid, 256, 0, s>>>(static_cast<const T*>(in), count, out);
+  });
   B2_CUDA(cudaGetLastError());
 }
 

@@ -1070,17 +1070,9 @@ static uint32_t walk_prefetch_bytes(const cagra_launch& p, size_t elem)
   return static_cast<uint32_t>(std::min(row, pitch));
 }
 
-// element type of an index's rows, as the walk kernels' template argument
-enum class row_type { f32, f16, i8, u8 };
-row_type row_type_of(DLDataType t)
-{
-  if (t.code == kDLFloat) return t.bits == 32 ? row_type::f32 : row_type::f16;
-  return t.code == kDLInt ? row_type::i8 : row_type::u8;
-}
-size_t row_elem_size(row_type rt) { return rt == row_type::f32 ? 4 : (rt == row_type::f16 ? 2 : 1); }
 int query_words_of(row_type rt, cuvsDistanceType metric, int dim)
 {
-  return row_elem_size(rt) == 1 && metric != CosineExpanded ? query_words<true>(dim) : query_words<false>(dim);
+  return row_bytes(rt) == 1 && metric != CosineExpanded ? query_words<true>(dim) : query_words<false>(dim);
 }
 
 template <bool MULTI>
@@ -1106,7 +1098,7 @@ void launch_search(void (*kern)(cagra_launch), cudaStream_t s, const cagra_launc
   B2_CUDA(cudaMemsetAsync(counter.data(), 0, sizeof(unsigned long long), s));
   cagra_launch pl = p;
   pl.work_counter = counter.data();
-  pl.prefetch_row_bytes = walk_prefetch_bytes(p, row_elem_size(rt));
+  pl.prefetch_row_bytes = walk_prefetch_bytes(p, row_bytes(rt));
   // measured (10M x 96 fp32, batch 10k, one box, scripts/ab_cagra.py): off 5.73-5.75 ms, line prefetches 6.06-6.08 ms (slower: three
   // CCTL per row and lane compete with the team loads for the LSU), bulk prefetch 5.56-5.58 ms -> the bulk form is the default
   pl.prefetch_mode      = [] { const char* e = getenv("CUVS_B200_CAGRA_PREFETCH"); return e != nullptr && e[0] == '1' ? 1 : 2; }();
@@ -1116,22 +1108,14 @@ void launch_search(void (*kern)(cagra_launch), cudaStream_t s, const cagra_launc
   B2_CUDA(cudaGetLastError());
 }
 
-template <int EB, int MINB, bool MULTI, typename T>
-void launch_general_rows(cudaStream_t s, const cagra_launch& p, size_t per_warp_smem, row_type rt)
-{
-  launch_search<MULTI>(p.metric == CosineExpanded ? cagra_search_kernel<EB, MINB, MULTI, true, T> : cagra_search_kernel<EB, MINB, MULTI, false, T>,
-                       s, p, per_warp_smem, rt);
-}
-
 template <int EB, int MINB, bool MULTI>
 void launch_general(cudaStream_t s, const cagra_launch& p, size_t per_warp_smem, row_type rt)
 {
-  switch (rt) {
-    case row_type::f32: return launch_general_rows<EB, MINB, MULTI, float>(s, p, per_warp_smem, rt);
-    case row_type::f16: return launch_general_rows<EB, MINB, MULTI, __half>(s, p, per_warp_smem, rt);
-    case row_type::i8: return launch_general_rows<EB, MINB, MULTI, int8_t>(s, p, per_warp_smem, rt);
-    case row_type::u8: return launch_general_rows<EB, MINB, MULTI, uint8_t>(s, p, per_warp_smem, rt);
-  }
+  with_row_type(rt, [&](auto t) {
+    using T = decltype(t);
+    launch_search<MULTI>(p.metric == CosineExpanded ? cagra_search_kernel<EB, MINB, MULTI, true, T> : cagra_search_kernel<EB, MINB, MULTI, false, T>,
+                         s, p, per_warp_smem, rt);
+  });
 }
 
 template <int EI, int EC, bool MULTI>
@@ -1198,7 +1182,7 @@ void cagra_search_multi(resources* res, const cagra_index& idx, const cuvsCagraS
                         uint32_t* out32, int64_t* out64, float* out_dist, const uint32_t* keep_bits, int64_t n_bits)
 {
   auto s = res->stream;
-  const row_type rt = row_type_of(idx.dtype);
+  const row_type rt = idx.type;
   size_t itopk = sp.itopk_size ? sp.itopk_size : 64;
   if (itopk % 32) itopk += 32 - itopk % 32;
   const size_t walkers_req = std::max<size_t>(std::max<size_t>(sp.search_width, 1), (itopk + 31) / 32);
@@ -1272,10 +1256,10 @@ void cagra_search(resources* res, const cagra_index& idx, const cuvsCagraSearchP
   auto s = res->stream;
   if (nq == 0) return;
   B2_EXPECTS(idx.metric == L2Expanded || idx.metric == InnerProduct || idx.metric == L2SqrtExpanded || idx.metric == CosineExpanded ||
-               (idx.metric == BitwiseHamming && idx.elem_size() == 1),
+               (idx.metric == BitwiseHamming && row_bytes(idx.type) == 1),
              "cagra search: unsupported metric %d", int(idx.metric));
   B2_EXPECTS(!sp.persistent, "cagra search: the persistent (latency) mode is out of scope of this library");
-  const row_type rt = row_type_of(idx.dtype);
+  const row_type rt = idx.type;
   dbuf<float> unit_q;
   if (idx.metric == CosineExpanded) {
     // the walk scores against q / |q| (a zero query stays zero: distance 1 to every row); the caller's tensor is not touched
@@ -1338,21 +1322,6 @@ __global__ void to_half_rows_kernel(const float* __restrict__ x, int64_t n, int 
   const int64_t r = i / ld16;
   const int c     = static_cast<int>(i % ld16);
   out[i]          = __float2half_rn(c < dim ? x[r * ld + c] : 0.f);
-}
-
-// |x_i|^2 of float16 / int8 / uint8 rows: fp32 fmaf in ascending order, the sum row_norms makes of the widened values
-template <typename T>
-__global__ void narrow_row_norms_kernel(const T* __restrict__ x, int64_t n, int d, int64_t ld, float* __restrict__ out)
-{
-  int64_t i = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x;
-  if (i >= n) return;
-  const T* r = x + i * ld;
-  float acc  = 0.f;
-  for (int k = 0; k < d; ++k) {
-    const float v = static_cast<float>(r[k]);
-    acc           = fmaf(v, v, acc);
-  }
-  out[i] = acc;
 }
 
 __global__ void knn_to_graph_kernel(const int64_t* __restrict__ knn, int64_t n, int kk, int keep, uint32_t* __restrict__ graph, int degree)
@@ -1520,8 +1489,8 @@ static void set_dataset(resources* r, cagra_index& idx, const DLTensor& ds)
 {
   B2_EXPECTS(dl_is_dataset_dtype(ds), "Unsupported dataset DLtensor dtype: %d and bits: %d", ds.dtype.code, ds.dtype.bits);
   B2_EXPECTS(ds.ndim == 2 && dl_is_c_contiguous(ds), "dataset must be a row-major 2-D tensor");
-  idx.dtype       = DLDataType{ds.dtype.code, ds.dtype.bits, 1};
-  const size_t es = idx.elem_size();
+  idx.type        = row_type_of(ds.dtype);
+  const size_t es = row_bytes(idx.type);
   const int per16 = static_cast<int>(16 / es);
   idx.n   = ds.shape[0];
   idx.dim = static_cast<int>(ds.shape[1]);
@@ -1544,16 +1513,10 @@ void b200::set_inv_norms(resources* r, cagra_index& idx)
   idx.inv_norm.release();
   if (idx.metric != CosineExpanded || idx.n == 0) return;
   idx.inv_norm.alloc(static_cast<size_t>(idx.n));
-  if (idx.is_f32()) {
-    row_norms(r->stream, idx.rows_f32(), idx.n, idx.dim, idx.ld, idx.inv_norm.data());
-  } else {
-    const unsigned grid = blocks_for(idx.n, 128);
-    count_launch();
-    if (idx.dtype.code == kDLFloat) narrow_row_norms_kernel<<<grid, 128, 0, r->stream>>>(static_cast<const __half*>(idx.data), idx.n, idx.dim, idx.ld, idx.inv_norm.data());
-    else if (idx.dtype.code == kDLInt) narrow_row_norms_kernel<<<grid, 128, 0, r->stream>>>(static_cast<const int8_t*>(idx.data), idx.n, idx.dim, idx.ld, idx.inv_norm.data());
-    else narrow_row_norms_kernel<<<grid, 128, 0, r->stream>>>(static_cast<const uint8_t*>(idx.data), idx.n, idx.dim, idx.ld, idx.inv_norm.data());
-    B2_CUDA(cudaGetLastError());
-  }
+  with_row_type(idx.type, [&](auto t) {
+    using T = decltype(t);
+    row_norms(r->stream, static_cast<const T*>(idx.data), idx.n, idx.dim, idx.ld, idx.inv_norm.data());
+  });
   rsqrt_rows(r->stream, idx.inv_norm.data(), idx.n, idx.inv_norm.data());
 }
 
@@ -1659,7 +1622,7 @@ cuvsError_t cuvsCagraIndexGetDataset(cuvsCagraIndex_t index, DLManagedTensor* da
   return guarded([=] {
     auto& idx        = index_of<cagra_index>(index);
     int64_t shape[2] = {idx.n, idx.dim};
-    dl_fill_view(dataset, const_cast<void*>(idx.data), idx.device, idx.dtype, 2, shape);
+    dl_fill_view(dataset, const_cast<void*>(idx.data), idx.device, dtype_of(idx.type), 2, shape);
     if (idx.ld != idx.dim) {
       dataset->dl_tensor.strides    = new int64_t[2];
       dataset->dl_tensor.strides[0] = idx.ld;
@@ -1704,7 +1667,7 @@ cuvsError_t cuvsCagraIndexFromArgs(cuvsResources_t res, cuvsDistanceType metric,
       idx->graph = idx->graph_own.data();
     }
     B2_CUDA(cudaStreamSynchronize(r->stream));
-    const DLDataType dtype = idx->dtype;
+    const DLDataType dtype = dtype_of(idx->type);
     set_index(index, idx.release(), dtype);
   });
 }
@@ -1741,7 +1704,7 @@ cuvsError_t cuvsCagraBuild(cuvsResources_t res, cuvsCagraIndexParams_t params, D
       // intermediate_graph_degree, lists of 1.5 times that while iterating, nn_descent_niter iterations)
       di = static_cast<int>(std::min<int64_t>(n - 1, di_want));
       nbr.alloc(static_cast<size_t>(n) * di, r->stream);
-      nn_descent_graph(r, idx->data, idx->dtype, n, idx->dim, idx->ld, idx->metric, di, di + di / 2,
+      nn_descent_graph(r, idx->data, idx->type, n, idx->dim, idx->ld, idx->metric, di, di + di / 2,
                        static_cast<int>(std::min<size_t>(params->nn_descent_niter, 1u << 30)), 0.0001f, NND_DIST_COMP_AUTO, nbr.data(), nullptr);
     } else {
       // ---- kNN stage through the library's own scans: exact for small inputs, IVF-Flat self-search beyond
@@ -1751,7 +1714,7 @@ cuvsError_t cuvsCagraBuild(cuvsResources_t res, cuvsCagraIndexParams_t params, D
       dbuf<float> compact;
       f32_matrix widened;  // float16 / 8-bit rows: the scans want fp32, a temporary that lives until the graph is made
       const float* data = idx->rows_f32();
-      if (!idx->is_f32()) {
+      if (idx->type != row_type::f32) {
         widen_to_f32(r, dataset_t->dl_tensor, widened);
         data = dl_ptr<float>(widened.t);
       } else if (idx->ld != idx->dim) {  // the scans want unpadded rows
@@ -1784,7 +1747,7 @@ cuvsError_t cuvsCagraBuild(cuvsResources_t res, cuvsCagraIndexParams_t params, D
     B2_CUDA(cudaStreamSynchronize(r->stream));
     idx->graph  = idx->graph_own.data();
     idx->degree = degree;
-    const DLDataType dtype = idx->dtype;
+    const DLDataType dtype = dtype_of(idx->type);
     set_index(index, idx.release(), dtype);
   });
 }
@@ -1826,7 +1789,7 @@ cuvsError_t cuvsCagraSerialize(cuvsResources_t res, const char* filename, cuvsCa
     auto& idx = index_of<cagra_index>(index);
     std::ofstream os(filename, std::ios::out | std::ios::binary);
     B2_EXPECTS(bool(os), "Cannot open file %s", filename);
-    const npy::file_dtype& ft = npy::file_dtype_for(idx.dtype);
+    const npy::file_dtype& ft = npy::file_dtype_for(dtype_of(idx.type));
     os.write(ft.tag, 4);  // three characters and the terminating zero
     npy::write_scalar<int32_t>(os, 5);
     npy::write_scalar<uint32_t>(os, static_cast<uint32_t>(idx.n));
@@ -1845,7 +1808,7 @@ cuvsError_t cuvsCagraSerialize(cuvsResources_t res, const char* filename, cuvsCa
       npy::write_scalar<int64_t>(os, idx.n);
       npy::write_scalar<uint32_t>(os, static_cast<uint32_t>(idx.dim));
       npy::write_scalar<uint32_t>(os, static_cast<uint32_t>(idx.ld));
-      const size_t es = idx.elem_size();
+      const size_t es = row_bytes(idx.type);
       std::vector<char> d(static_cast<size_t>(idx.n) * idx.dim * es);
       B2_CUDA(cudaMemcpy2DAsync(d.data(), es * idx.dim, idx.data, es * idx.ld, es * idx.dim, idx.n, cudaMemcpyDeviceToHost, r->stream));
       B2_CUDA(cudaStreamSynchronize(r->stream));
@@ -1876,9 +1839,9 @@ cuvsError_t cuvsCagraDeserialize(cuvsResources_t res, const char* filename, cuvs
     idx->dim    = static_cast<int>(npy::read_scalar<uint32_t>(is, filename));
     idx->degree = static_cast<int>(npy::read_scalar<uint32_t>(is, filename));
     idx->metric = static_cast<cuvsDistanceType>(npy::read_scalar<int32_t>(is, filename));
-    idx->dtype  = dtype;
+    idx->type   = row_type_of(dtype);
     check_hamming_rows("cagra::deserialize", idx->metric, dtype);
-    const size_t es = idx->elem_size();
+    const size_t es = row_bytes(idx->type);
     const int per16 = static_cast<int>(16 / es);
     idx->ld     = (idx->dim + per16 - 1) / per16 * per16;
     std::vector<uint32_t> g(static_cast<size_t>(idx->n) * idx->degree);
@@ -1931,8 +1894,8 @@ cuvsError_t cuvsB200CagraSetWalkPrecision(cuvsResources_t res, cuvsCagraIndex_t 
     auto r    = as_res(res);
     auto& idx = index_of<cagra_index>(index);
     B2_EXPECTS(bits == 16 || bits == 32, "walk precision must be 16 or 32 bits");
-    B2_EXPECTS(bits == 32 || idx.elem_size() != 1, "walk precision 16 is refused: the index's rows are 8-bit, already narrower than fp16");
-    if (!idx.is_f32()) return;
+    B2_EXPECTS(bits == 32 || row_bytes(idx.type) != 1, "walk precision 16 is refused: the index's rows are 8-bit, already narrower than fp16");
+    if (idx.type != row_type::f32) return;
     if (bits == 32) { idx.data16.release(); idx.ld16 = 0; return; }
     set_half_rows(r, idx);
   });

@@ -13,15 +13,13 @@ struct cagra_index {
   cuvsDistanceType metric = L2Expanded;
   int64_t n               = 0;
   int dim                 = 0;
-  DLDataType dtype        = DLDataType{kDLFloat, 32, 1};  // element type of the rows: float32, float16, int8 or uint8
+  row_type type           = row_type::f32;  // element type of the rows
   int ld                  = 0;  // row pitch in elements (rows padded to 16 bytes, cagra.hpp:610)
   int degree              = 0;
   const void* data        = nullptr;  // rows in the element type they were given in; a view of the caller's buffer or data_own
   const uint32_t* graph   = nullptr;
   owned<unsigned char> data_own;
   owned<uint32_t> graph_own;
-  size_t elem_size() const { return dtype.bits / 8; }
-  bool is_f32() const { return dtype.code == kDLFloat && dtype.bits == 32; }
   const float* rows_f32() const { return static_cast<const float*>(data); }  // float32 indexes only
   // float32 indexes only: optional fp16 copy of the vectors for the walk (cuvsB200CagraSetWalkPrecision): the walk is bound
   // by random row gathers from HBM, half-width rows halve its bytes; the returned neighbours are re-ranked with the fp32 rows.

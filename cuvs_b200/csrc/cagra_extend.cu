@@ -268,7 +268,7 @@ static void extend_chunk(resources* r, cagra_index& g, int64_t n0, int64_t nc, u
 {
   auto s = r->stream;
   const int d = g.degree, B = 2 * d, half = d / 2;
-  const size_t es = g.elem_size();
+  const size_t es = row_bytes(g.type);
   uint32_t* graph = const_cast<uint32_t*>(g.graph);
   // ---- step 0
   B2_CUDA(cudaMemsetAsync(cnt, 0, sizeof(uint32_t) * static_cast<size_t>(n0 + nc), s));
@@ -282,7 +282,7 @@ static void extend_chunk(resources* r, cagra_index& g, int64_t n0, int64_t nc, u
     dbuf<unsigned char> rows(static_cast<size_t>(nc) * g.dim * es, s);
     B2_CUDA(cudaMemcpy2DAsync(rows.data(), es * g.dim, static_cast<const unsigned char*>(g.data) + static_cast<size_t>(n0) * g.ld * es, es * g.ld,
                               es * g.dim, nc, cudaMemcpyDeviceToDevice, s));
-    const dl_view q(rows.data(), DLDevice{kDLCUDA, r->device}, g.dtype, nc, g.dim);
+    const dl_view q(rows.data(), DLDevice{kDLCUDA, r->device}, dtype_of(g.type), nc, g.dim);
     f32_rows wq;
     widen_to_f32(r, q.t(), wq);
     search_params_guard sp;
@@ -348,7 +348,7 @@ static void cagra_extend(resources* r, const cuvsCagraExtendParams& ep, const DL
 {
   auto& idx = index_of<cagra_index>(index);
   B2_EXPECTS(dl_is_dataset_dtype(add), "Unsupported dataset DLtensor dtype: %d and bits: %d", add.dtype.code, add.dtype.bits);
-  B2_EXPECTS(add.dtype.code == idx.dtype.code && add.dtype.bits == idx.dtype.bits, "type mismatch between index and additional dataset");
+  B2_EXPECTS(row_type_of(add.dtype) == idx.type, "type mismatch between index and additional dataset");
   B2_EXPECTS(add.ndim == 2 && dl_is_c_contiguous(add), "additional dataset must be a row-major 2-D tensor");
   B2_EXPECTS(add.shape[1] == idx.dim, "additional dataset dim (%lld) != index dim (%d)", (long long)add.shape[1], idx.dim);
   const int64_t n_add = add.shape[0], n0 = idx.n, n_total = n0 + n_add;
@@ -359,8 +359,8 @@ static void cagra_extend(resources* r, const cuvsCagraExtendParams& ep, const DL
   auto s = r->stream;
   // the grown index is built beside the old one and replaces it only when every chunk succeeded
   auto g    = std::make_unique<cagra_index>();
-  g->device = idx.device; g->metric = idx.metric; g->dtype = idx.dtype; g->dim = idx.dim; g->ld = idx.ld; g->degree = d; g->n = n_total;
-  const size_t es = idx.elem_size();
+  g->device = idx.device; g->metric = idx.metric; g->type = idx.type; g->dim = idx.dim; g->ld = idx.ld; g->degree = d; g->n = n_total;
+  const size_t es = row_bytes(idx.type);
   {
     timed_section ts("cagra_extend_copy", s);
     g->data_own.alloc(static_cast<size_t>(n_total) * idx.ld * es);

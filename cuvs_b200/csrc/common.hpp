@@ -6,6 +6,7 @@
 // thread-local error text, and DLPack validation.  Plain C++ over the CUDA runtime.
 #pragma once
 
+#include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <dlpack/dlpack.h>
 
@@ -262,6 +263,39 @@ inline bool dl_is_dataset_dtype(const DLTensor& t)
 {
   return dl_is(t, kDLFloat, 32) || dl_is(t, kDLFloat, 16) || dl_is(t, kDLInt, 8) || dl_is(t, kDLUInt, 8);
 }
+
+/** The element type of dataset rows.  The values are the row_type cuvsB200BruteForceIndexInfo publishes. */
+enum class row_type { f32 = 0, f16 = 1, s8 = 2, u8 = 3 };
+inline row_type row_type_of(DLDataType t)
+{
+  if (t.lanes == 1 && t.code == kDLFloat && t.bits == 32) return row_type::f32;
+  if (t.lanes == 1 && t.code == kDLFloat && t.bits == 16) return row_type::f16;
+  if (t.lanes == 1 && t.code == kDLInt && t.bits == 8) return row_type::s8;
+  if (t.lanes == 1 && t.code == kDLUInt && t.bits == 8) return row_type::u8;
+  B2_FAIL("rows are float32, float16, int8 or uint8 (got dtype code %d, bits %d)", int(t.code), int(t.bits));
+}
+inline DLDataType dtype_of(row_type rt)
+{
+  switch (rt) {
+    case row_type::f16: return {kDLFloat, 16, 1};
+    case row_type::s8: return {kDLInt, 8, 1};
+    case row_type::u8: return {kDLUInt, 8, 1};
+    default: return {kDLFloat, 32, 1};
+  }
+}
+inline size_t row_bytes(row_type rt) { return rt == row_type::f32 ? 4 : (rt == row_type::f16 ? 2 : 1); }
+/** f(T{}) with T the element type of `rt`: float, __half, int8_t or uint8_t. */
+template <typename F>
+decltype(auto) with_row_type(row_type rt, F&& f)
+{
+  switch (rt) {
+    case row_type::f16: return f(__half{});
+    case row_type::s8: return f(int8_t{});
+    case row_type::u8: return f(uint8_t{});
+    default: return f(float{});
+  }
+}
+
 void widen_to_f32(struct resources* res, const DLTensor& src, f32_matrix& out);
 void widen_to_f32(struct resources* res, const DLTensor& src, f32_rows& out);
 /** out[i] = float(in[i]) for `count` device elements of type `dt` (float16, int8 or uint8), stream-ordered. */

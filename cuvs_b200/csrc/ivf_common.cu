@@ -18,38 +18,6 @@
 namespace b200 {
 namespace {
 
-__global__ void iota_items_kernel(tc_item* items, int m_tiles, int64_t n_rows, uint32_t b_tiles, int64_t row_stride)
-{
-  int m = blockIdx.x * blockDim.x + threadIdx.x;
-  if (m >= m_tiles) return;
-  tc_item it;
-  it.a_row0     = m * 128;
-  it.b_row0     = 0;
-  it.n_tiles    = b_tiles;
-  int64_t valid = n_rows - static_cast<int64_t>(m) * 128;
-  it.valid_rows = valid > 128 ? 128 : static_cast<uint32_t>(valid);
-  it.out_off    = static_cast<uint64_t>(m) * 128 * row_stride;
-  items[m]      = it;
-}
-
-// (query tile, centre range) items of the fused coarse search: item i = (split i / m_tiles, query tile i % m_tiles)
-__global__ void split_items_kernel(tc_item* items, int m_tiles, int splits, int64_t nq, uint32_t tiles_total, int KCW)
-{
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= m_tiles * splits) return;
-  const int sp = i / m_tiles, m = i % m_tiles;
-  const uint32_t per = (tiles_total + splits - 1) / splits;
-  const uint32_t t0 = min(tiles_total, sp * per), t1 = min(tiles_total, t0 + per);
-  tc_item it;
-  it.a_row0     = m * 128;
-  it.b_row0     = t0 * 128;
-  it.n_tiles    = t1 - t0;
-  const int64_t valid = nq - static_cast<int64_t>(m) * 128;
-  it.valid_rows = valid > 128 ? 128 : static_cast<uint32_t>(valid);
-  it.out_off    = (static_cast<uint64_t>(m) * 128 * splits + sp) * KCW;
-  items[i]      = it;
-}
-
 // Fused coarse search, merge step: one CTA per query ranks the W = splits * lists * KC candidates its items kept
 // (sorted lists of KC per centre range and column half) by (score, centre id) — the order select_k imposes on the dense
 // score row, where position == centre id — and writes the n_probes best.  The scan rejects a centre only when its score is
@@ -679,9 +647,7 @@ static bool coarse_select_fused(resources* res, const tc_rows_tmp& q, const tc_r
   if (W > kCoarseMaxW || W < 4 * n_probes) return false;
   const int n_items = m_tiles * splits;
   dbuf<tc_item> items(static_cast<size_t>(n_items), s);
-  count_launch();
-  split_items_kernel<<<blocks_for(n_items, 128), 128, 0, s>>>(items.data(), m_tiles, splits, q.n, static_cast<uint32_t>(b_tiles), KCW);
-  B2_CUDA(cudaGetLastError());
+  tc_split_items(s, items.data(), m_tiles, splits, q.n, static_cast<uint32_t>(b_tiles), KCW);  // (centre range, query tile) items
   dbuf<float> cs(static_cast<size_t>(nq_pad) * W, s);
   dbuf<uint32_t> cp(static_cast<size_t>(nq_pad) * W, s);
   dbuf<int> bkeys(static_cast<size_t>(nq_pad) + 1, s);
@@ -726,9 +692,7 @@ void coarse_select(resources* res, const tc_rows_tmp& q, const tc_rows& centers,
   const int m_tiles    = static_cast<int>(nq_pad / 128);
   const int64_t ld     = centers.rows_pad;
   dbuf<tc_item> items(static_cast<size_t>(m_tiles), s);
-  count_launch();
-  iota_items_kernel<<<blocks_for(m_tiles, 128), 128, 0, s>>>(items.data(), m_tiles, q.n, static_cast<uint32_t>(ld / 128), ld);
-  B2_CUDA(cudaGetLastError());
+  tc_split_items(s, items.data(), m_tiles, 1, q.n, static_cast<uint32_t>(ld / 128), ld);
   dbuf<float> scores(static_cast<size_t>(nq_pad) * ld, s);
   const bool three = q.lo.data() != nullptr && centers.lo.data() != nullptr;
   tc_scan_topk(s, res->device, q.hi.data(), q.lo.data(), q.rows_pad, centers.hi.data(), centers.lo.data(), centers.rows_pad,
@@ -752,10 +716,7 @@ void assign_nearest(resources* res, const __nv_bfloat16* x_hi, const __nv_bfloat
   for (int64_t r0 = 0; r0 < n; r0 += chunk) {
     const int64_t rows = std::min(chunk, n - r0);
     const int m_tiles  = static_cast<int>(tc_pad_rows(rows) / 128);
-    count_launch();
-    iota_items_kernel<<<blocks_for(m_tiles, 128), 128, 0, s>>>(items.data(), m_tiles, rows,
-                                                                static_cast<uint32_t>(centers.rows_pad / 128), KCW);
-    B2_CUDA(cudaGetLastError());
+    tc_split_items(s, items.data(), m_tiles, 1, rows, static_cast<uint32_t>(centers.rows_pad / 128), KCW);
     tc_scan_topk(s, res->device, x_hi + r0 * Kp, x_lo ? x_lo + r0 * Kp : nullptr, x_rows_pad - r0, centers.hi.data(),
                  centers.lo.data(), centers.rows_pad, Kp, centers.hx.data(), items.data(), m_tiles, nullptr, KC,
                  three ? 3 : 1, cs.data(), cp.data(), KCW);
@@ -795,9 +756,7 @@ void assign_exact(resources* res, const float* x, const float* xn, const tc_rows
   for (int64_t r0 = 0; r0 < n; r0 += chunk) {
     const int64_t rows = std::min(chunk, n - r0);
     const int m_tiles  = static_cast<int>(tc_pad_rows(rows) / 128);
-    count_launch();
-    iota_items_kernel<<<blocks_for(m_tiles, 128), 128, 0, s>>>(items.data(), m_tiles, rows, static_cast<uint32_t>(cp.rows_pad / 128), KCW);
-    B2_CUDA(cudaGetLastError());
+    tc_split_items(s, items.data(), m_tiles, 1, rows, static_cast<uint32_t>(cp.rows_pad / 128), KCW);
     tc_scan_topk(s, res->device, xp.hi.data() + r0 * xp.Kp, xp.lo.data() + r0 * xp.Kp, xp.rows_pad - r0, cp.hi.data(), cp.lo.data(),
                  cp.rows_pad, xp.Kp, cp.hx.data(), items.data(), m_tiles, nullptr, KC, 3, cs.data(), cpos.data(), KCW);
     const float* xc  = x + r0 * d;

@@ -70,8 +70,8 @@ struct ivf_flat_index {
   owned<float> rn_max;       // [n_lists] max |x - c|^2 over the list's rows (the certificate's error budget)
   owned<float> cn;           // [n_lists] |c|^2 of the fp32 centres (the inner-product budget)
   int Kp = 0;
-  // 8-bit lists (row_type kRowS8 / kRowU8; DESIGN.md §4 "Row types"): data, hi, hx, xn, rn and rn_max stay empty
-  int row_type = 0;
+  // 8-bit lists (row_type s8 / u8; DESIGN.md §4 "Row types"): data, hi, hx, xn, rn and rn_max stay empty
+  row_type type = row_type::f32;
   owned<uint8_t> rows8;      // [rows_total, Kp8] the rows' bytes, zero padding rows and columns
   owned<int> norms8;         // [rows_total] exact |x|^2, kI8PadNorm on padding rows
   int Kp8 = 0;
@@ -80,11 +80,11 @@ struct ivf_flat_index {
 namespace {
 
 // How an index stores its list rows: fp32 (float32 and float16 datasets, and cosine on 8-bit ones), or the 8-bit rows themselves.
-constexpr int kRowF32 = 0, kRowS8 = 1, kRowU8 = 2;
-int row_type_for(DLDataType t, cuvsDistanceType metric)
+row_type row_type_for(DLDataType t, cuvsDistanceType metric)
 {
-  if (metric == CosineExpanded || t.bits != 8) return kRowF32;  // a cosine distance is no integer function of the rows
-  return t.code == kDLInt ? kRowS8 : kRowU8;
+  const row_type rt = row_type_of(t);
+  if (metric == CosineExpanded || row_bytes(rt) != 1) return row_type::f32;  // a cosine distance is no integer function of the rows
+  return rt;
 }
 
 // 8-bit rows from a widened chunk x (integer values as fp32): one thread per byte of a padded row, written to row dst_rows[r]
@@ -98,28 +98,6 @@ __global__ void narrow_rows_kernel(const float* __restrict__ x, int64_t n, int d
   const int64_t o = dst_rows[r];
   if (o < 0) return;
   out[o * Kp8 + j] = j < dim ? static_cast<uint8_t>(static_cast<int>(x[r * dim + j])) : uint8_t(0);
-}
-
-// norms[r] = |x_r|^2 exactly, or kI8PadNorm on padding rows and on rows the bitset (bit = 1 keeps; null: all) hides.  One warp
-// per row.
-template <bool U8>
-__global__ void i8_norms_kernel(const uint8_t* __restrict__ rows, int64_t n, int Kp8, const int64_t* __restrict__ ids,
-                                const uint32_t* __restrict__ keep_bits, int64_t n_bits, int* __restrict__ norms)
-{
-  const int64_t r = (blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x) >> 5;
-  const int lane  = threadIdx.x & 31;
-  if (r >= n) return;
-  int acc = 0;
-  for (int j = lane; j < Kp8; j += 32) {
-    const int v = U8 ? static_cast<int>(rows[r * Kp8 + j]) : static_cast<int>(static_cast<int8_t>(rows[r * Kp8 + j]));
-    acc += v * v;
-  }
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
-  if (lane != 0) return;
-  const int64_t id = ids[r];
-  const bool keep  = id != kPadId && (keep_bits == nullptr || (id >= 0 && id < n_bits && ((keep_bits[id >> 5] >> (id & 31)) & 1u)));
-  norms[r]         = keep ? acc : kI8PadNorm;
 }
 
 // The A rows of an 8-bit scan: the bytes of each pair slot's query (slots past the live pairs: zero), 16 per thread
@@ -547,14 +525,7 @@ void refresh_i8_side(resources* res, ivf_flat_index& idx)
   const int64_t R = idx.lists.rows_total;
   idx.norms8.alloc(static_cast<size_t>(std::max<int64_t>(R, 128)));
   if (R == 0) return;
-  count_launch();
-  if (idx.row_type == kRowU8)
-    i8_norms_kernel<true><<<blocks_for(R * 32, 256), 256, 0, res->stream>>>(idx.rows8.data(), R, idx.Kp8, idx.ids.data(), nullptr, 0,
-                                                                            idx.norms8.data());
-  else
-    i8_norms_kernel<false><<<blocks_for(R * 32, 256), 256, 0, res->stream>>>(idx.rows8.data(), R, idx.Kp8, idx.ids.data(), nullptr, 0,
-                                                                             idx.norms8.data());
-  B2_CUDA(cudaGetLastError());
+  tc_i8_norms(res->stream, idx.type == row_type::u8, idx.rows8.data(), R, R, idx.Kp8, idx.ids.data(), nullptr, 0, idx.norms8.data());
 }
 
 void refresh_centers_tc(resources* res, ivf_flat_index& idx)
@@ -596,7 +567,7 @@ void ivf_flat_extend(resources* res, ivf_flat_index& idx, const DLTensor& t, con
   auto write = [&](const float* x, int64_t n, uint32_t*, const int64_t* dst_rows, float* data) {
     scatter_rows(s, x, n, int64_t(idx.dim), dst_rows, data);
   };
-  if (idx.row_type != kRowF32) {
+  if (idx.type != row_type::f32) {
     auto write8 = [&](const float* x, int64_t n, uint32_t*, const int64_t* dst_rows, uint8_t* rows) {
       count_launch();
       narrow_rows_kernel<<<blocks_for(n * idx.Kp8, 256), 256, 0, s>>>(x, n, idx.dim, idx.Kp8, dst_rows, rows);
@@ -613,7 +584,7 @@ void ivf_flat_extend(resources* res, ivf_flat_index& idx, const DLTensor& t, con
 // The derived rows of the index's row type
 void refresh_rows(resources* res, ivf_flat_index& idx)
 {
-  if (idx.row_type != kRowF32) refresh_i8_side(res, idx);
+  if (idx.type != row_type::f32) refresh_i8_side(res, idx);
   else refresh_tc_side(res, idx);
 }
 
@@ -636,9 +607,9 @@ ivf_flat_index* ivf_flat_build(resources* res, const cuvsIvfFlatIndexParams& p, 
   idx->adaptive_centers  = p.adaptive_centers;
   idx->kmeans_n_iters    = p.kmeans_n_iters;
   idx->kmeans_trainset_fraction = p.kmeans_trainset_fraction;
-  idx->row_type          = row_type_for(ds.dtype, p.metric);
+  idx->type              = row_type_for(ds.dtype, p.metric);
   idx->Kp8               = tc_pad_k_i8(d);
-  B2_EXPECTS(idx->row_type != kRowF32 || dl_is(ds, kDLFloat, 32), "ivf_flat_build: float16 rows, and 8-bit rows of a cosine index, must be widened to float32 first");
+  B2_EXPECTS(idx->type != row_type::f32 || dl_is(ds, kDLFloat, 32), "ivf_flat_build: float16 rows, and 8-bit rows of a cosine index, must be widened to float32 first");
   auto s = res->stream;
 
   int64_t n_train   = 0;
@@ -740,12 +711,7 @@ void ivf_flat_search_i8(resources* res, const ivf_flat_index& idx, uint32_t n_pr
   dbuf<int> norms_f;
   if (keep_bits != nullptr && R > 0) {
     norms_f.alloc(static_cast<size_t>(std::max<int64_t>(R, 128)), s);
-    count_launch();
-    if (idx.row_type == kRowU8)
-      i8_norms_kernel<true><<<blocks_for(R * 32, 256), 256, 0, s>>>(idx.rows8.data(), R, idx.Kp8, idx.ids.data(), keep_bits, n_bits, norms_f.data());
-    else
-      i8_norms_kernel<false><<<blocks_for(R * 32, 256), 256, 0, s>>>(idx.rows8.data(), R, idx.Kp8, idx.ids.data(), keep_bits, n_bits, norms_f.data());
-    B2_CUDA(cudaGetLastError());
+    tc_i8_norms(s, idx.type == row_type::u8, idx.rows8.data(), R, R, idx.Kp8, idx.ids.data(), keep_bits, n_bits, norms_f.data());
     norms = norms_f.data();
   }
 
@@ -761,7 +727,7 @@ void ivf_flat_search_i8(resources* res, const ivf_flat_index& idx, uint32_t n_pr
   B2_CUDA(cudaGetLastError());
 
   // ---- 3. fine scan on the integer tensor cores
-  const bool u8       = idx.row_type == kRowU8;
+  const bool u8       = idx.type == row_type::u8;
   const int64_t b_rows = std::max<int64_t>(R, 128);
   dbuf<float> cs;
   dbuf<uint32_t> cp;
@@ -826,7 +792,7 @@ void ivf_flat_search(resources* res, const ivf_flat_index& idx, uint32_t n_probe
   B2_EXPECTS(n_probes >= 1, "n_probes must be >= 1");
   if (nq == 0) return;
   n_probes         = std::min<uint32_t>(n_probes, idx.n_lists);
-  if (idx.row_type != kRowF32) return ivf_flat_search_i8(res, idx, n_probes, qt, nt, dt, keep_bits, n_bits, dump);
+  if (idx.type != row_type::f32) return ivf_flat_search_i8(res, idx, n_probes, qt, nt, dt, keep_bits, n_bits, dump);
   // k > 64 (DESIGN.md §4 "k > 64"): the scan stores every (pair, list row) score and a segmented select keeps kc2 per pair.
   const bool large_k = k > 64;
   const int large_kc = std::min(2 * k, kSelectMaxK);
@@ -1126,7 +1092,7 @@ cuvsError_t cuvsIvfFlatBuild(cuvsResources_t res, cuvsIvfFlatIndexParams_t param
     drop_index<ivf_flat_index>(index);
     // int8 / uint8 datasets in L2 or inner product keep their type; float16 ones, and 8-bit ones for cosine, are widened to fp32
     // rows (c/src/neighbors/ivf_flat.cpp dtype switch)
-    if (row_type_for(ds.dtype, params->metric) != kRowF32) {
+    if (row_type_for(ds.dtype, params->metric) != row_type::f32) {
       set_index(index, ivf_flat_build(r, *params, ds), ds.dtype);
     } else {
       f32_matrix w;
@@ -1165,7 +1131,7 @@ cuvsError_t cuvsIvfFlatExtend(cuvsResources_t res, DLManagedTensor* new_vectors,
     B2_EXPECTS(dl_is_dataset_dtype(new_vectors->dl_tensor), "Unsupported new_vectors DLtensor dtype: %d and bits: %d",
                new_vectors->dl_tensor.dtype.code, new_vectors->dl_tensor.dtype.bits);
     f32_rows wv;
-    if (idx.row_type != kRowF32) {  // 8-bit lists take rows of their own type
+    if (idx.type != row_type::f32) {  // 8-bit lists take rows of their own type
       const DLTensor& nv = new_vectors->dl_tensor;
       B2_EXPECTS(nv.dtype.code == index->dtype.code && nv.dtype.bits == 8, "type mismatch between index and new_vectors");
       B2_EXPECTS(nv.ndim == 2 && dl_is_c_contiguous(nv), "matrix must be a row-major 2-D tensor");
@@ -1245,7 +1211,7 @@ cuvsError_t cuvsIvfFlatSerialize(cuvsResources_t res, const char* filename, cuvs
     std::vector<uint32_t> sizes(idx.n_lists);
     for (uint32_t l = 0; l < idx.n_lists; ++l) sizes[l] = static_cast<uint32_t>(idx.lists.h_sizes[l]);
     npy::write_array<uint32_t>(os, sizes.data(), {static_cast<int64_t>(idx.n_lists)});
-    const bool native = idx.row_type != kRowF32;
+    const bool native = idx.type != row_type::f32;
     const int dim = idx.dim, es = ft.size, vl = flat_veclen(dim, es);
     std::vector<float> rows;
     std::vector<uint8_t> rows8, inter;
@@ -1300,7 +1266,7 @@ cuvsError_t cuvsIvfFlatDeserialize(cuvsResources_t res, const char* filename, cu
     idx->n_lists  = npy::read_scalar<uint32_t>(is, filename);
     idx->metric   = static_cast<cuvsDistanceType>(npy::read_scalar<int32_t>(is, filename));
     idx->adaptive_centers = npy::read_scalar<uint8_t>(is, filename) != 0;
-    idx->row_type = row_type_for(dtype, idx->metric);
+    idx->type     = row_type_for(dtype, idx->metric);
     idx->Kp8      = tc_pad_k_i8(idx->dim);
     (void)npy::read_scalar<uint8_t>(is, filename);  // conservative_memory_allocation: an allocation policy, nothing to restore
     std::vector<float> c(static_cast<size_t>(idx->n_lists) * idx->dim);
@@ -1319,7 +1285,7 @@ cuvsError_t cuvsIvfFlatDeserialize(cuvsResources_t res, const char* filename, cu
     idx->lists.set_sizes(r->stream, sizes);
     B2_EXPECTS(idx->lists.size == n_rows, "ivf_flat::deserialize: list sizes sum to %lld, header says %lld rows", (long long)idx->lists.size,
                (long long)n_rows);
-    const bool native = idx->row_type != kRowF32;
+    const bool native = idx->type != row_type::f32;
     if (native) alloc_list_storage(r->stream, idx->lists, idx->Kp8, idx->rows8, idx->ids);
     else alloc_list_storage(r->stream, idx->lists, idx->dim, idx->data, idx->ids);
     const int es = dtype.bits / 8, dim = idx->dim, vl = flat_veclen(dim, es);

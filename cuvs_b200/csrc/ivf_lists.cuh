@@ -8,14 +8,12 @@
 // 2-D TMA box; no per-list pointer table, no interleaving).
 #pragma once
 #include "common.hpp"
+#include "scan_tc.cuh"  // kPadId
 
 #include <functional>
 #include <vector>
 
 namespace b200 {
-
-/** id stored on the padding rows of a list (any other int64, negative ones included, is a user id). */
-constexpr int64_t kPadId = INT64_MIN;
 
 struct list_layout {
   int64_t n_lists = 0;

@@ -623,20 +623,6 @@ __global__ void fresh_count_kernel(uint64_t* __restrict__ L, int64_t count, unsi
 }
 
 // ------------------------------------------------------------------------------------------------------ row preparation
-// 1 / |x_i| in fp32 (ascending fmaf; 0 for a zero row)
-template <typename T>
-__global__ void inv_norm_kernel(const T* __restrict__ x, int64_t n, int d, int64_t ld, float* __restrict__ out)
-{
-  const int64_t i = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x;
-  if (i >= n) return;
-  float acc = 0.f;
-  for (int k = 0; k < d; ++k) {
-    const float v = static_cast<float>(load_acc(x[i * ld + k]));
-    acc = fmaf(v, v, acc);
-  }
-  out[i] = acc > 0.f ? 1.0f / sqrtf(acc) : 0.f;
-}
-
 // sum of squares of a row in its join type, ascending (fmaf over fp16 values, exact int over 8-bit ones)
 template <typename T>
 __global__ void sq_norm_kernel(const T* __restrict__ x, int64_t n, int d, int64_t ld, typename acc_of<T>::type* __restrict__ out)
@@ -698,28 +684,19 @@ __global__ void to_half_kernel(const T* __restrict__ x, int64_t n, int d, int64_
 }
 
 // ------------------------------------------------------------------------------------------------------------ re-score
+// the batch's rows widened to the fp32 query block of rescore_topk
 template <typename T>
-__global__ void gather_widen_kernel(const T* __restrict__ x, int64_t ld, int d, const uint32_t* __restrict__ ids, int64_t count, float* __restrict__ out)
+__global__ void widen_rows_kernel(const T* __restrict__ x, int64_t ld, int d, int64_t count, float* __restrict__ out)
 {
   const int64_t i = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x;
   if (i >= count * d) return;
-  const int64_t r = i / d;
-  out[i] = static_cast<float>(load_acc(x[static_cast<int64_t>(ids[r]) * ld + i % d]));
+  out[i] = static_cast<float>(load_acc(x[(i / d) * ld + i % d]));
 }
 
-__global__ void list_ids_kernel(const uint64_t* __restrict__ L, int64_t count, uint32_t* __restrict__ ids, int64_t* __restrict__ ids64)
+__global__ void list_ids_kernel(const uint64_t* __restrict__ L, int64_t count, uint32_t* __restrict__ ids)
 {
   const int64_t i = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x;
-  if (i >= count) return;
-  const uint32_t id = static_cast<uint32_t>(L[i]) & kIdMask;
-  ids[i] = id;
-  if (ids64) ids64[i] = id;
-}
-
-__global__ void iota_kernel(uint32_t* __restrict__ out, int64_t n)
-{
-  const int64_t i = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x;
-  if (i < n) out[i] = static_cast<uint32_t>(i);
+  if (i < count) ids[i] = static_cast<uint32_t>(L[i]) & kIdMask;
 }
 
 __global__ void narrow_ids_kernel(const int64_t* __restrict__ in, int64_t count, uint32_t* __restrict__ out)
@@ -876,48 +853,35 @@ void rescore(resources* r, const T* x, int64_t ld, int d, cuvsDistanceType metri
   constexpr bool f32 = std::is_same<T, float>::value;
   const bool norms   = metric == L2Expanded || metric == L2SqrtExpanded || metric == CosineExpanded;
   dbuf<float> xn;
-  if (f32 && norms) {
+  if (norms) {
     xn.alloc(static_cast<size_t>(n), s);
-    row_norms(s, reinterpret_cast<const float*>(x), n, d, ld, xn.data());
+    row_norms(s, x, n, d, ld, xn.data());
   }
-  // narrow rows: the batch's rows and their candidates' rows are widened into a temporary of about 1 GiB
-  const int64_t per_row = f32 ? 0 : static_cast<int64_t>(Ki + 1) * d * 4;
-  const int64_t batch   = f32 ? std::min<int64_t>(n, 1 << 20) : std::max<int64_t>(1, std::min<int64_t>(n, (int64_t(1) << 30) / per_row));
+  // narrow rows: the batch's own rows are widened into the fp32 query block rescore_topk reads; the batch's temporaries (that
+  // block, the candidate ids and the kept ids and distances) stay within about 1 GiB
+  const int64_t per_row = 4 * static_cast<int64_t>(d) + 4 * static_cast<int64_t>(Ki) + 12 * static_cast<int64_t>(degree);
+  const int64_t batch   = std::min<int64_t>(std::min<int64_t>(n, 1 << 20), f32 ? n : std::max<int64_t>(1, (int64_t(1) << 30) / per_row));
   dbuf<uint32_t> cand(static_cast<size_t>(batch) * Ki, s);
-  dbuf<int64_t> cand64, out_idx(static_cast<size_t>(batch) * degree, s);
-  dbuf<float> out_dist(static_cast<size_t>(batch) * degree, s), qf, xf, qn, xfn;
-  if (!f32) {
-    cand64.alloc(static_cast<size_t>(batch) * Ki, s);
-    qf.alloc(static_cast<size_t>(batch) * d, s);
-    xf.alloc(static_cast<size_t>(batch) * Ki * d, s);
-    if (norms) { qn.alloc(static_cast<size_t>(batch), s); xfn.alloc(static_cast<size_t>(batch) * Ki, s); }
-  }
-  dbuf<uint32_t> self_ids;
-  if (!f32) self_ids.alloc(static_cast<size_t>(batch), s);
+  dbuf<int64_t> out_idx(static_cast<size_t>(batch) * degree, s);
+  dbuf<float> out_dist(static_cast<size_t>(batch) * degree, s), qf;
+  if (!f32) qf.alloc(static_cast<size_t>(batch) * d, s);
   for (int64_t b0 = 0; b0 < n; b0 += batch) {
     const int64_t nb = std::min(batch, n - b0);
     count_launch();
-    list_ids_kernel<<<blocks_for(nb * Ki, 256), 256, 0, s>>>(L + b0 * Ki, nb * Ki, cand.data(), f32 ? nullptr : cand64.data());
+    list_ids_kernel<<<blocks_for(nb * Ki, 256), 256, 0, s>>>(L + b0 * Ki, nb * Ki, cand.data());
+    const float* q = qf.data();
+    int64_t ldq    = d;
     if constexpr (f32) {
-      const float* q = reinterpret_cast<const float*>(x) + b0 * ld;
-      rescore_topk(s, q, nb, ld, reinterpret_cast<const float*>(x), ld, d, norms ? xn.data() + b0 : nullptr, norms ? xn.data() : nullptr, metric,
-                   cand.data(), Ki, nullptr, degree, out_idx.data(), out_dist.data(), -1);
+      q   = x + b0 * ld;
+      ldq = ld;
     } else {
-      count_launch(3);
-      iota_kernel<<<blocks_for(nb, 256), 256, 0, s>>>(self_ids.data(), nb);
-      // self_ids holds 0..nb-1; offset to the batch's rows through the base pointer
-      gather_widen_kernel<T><<<blocks_for(nb * d, 256), 256, 0, s>>>(x + b0 * ld, ld, d, self_ids.data(), nb, qf.data());
-      gather_widen_kernel<T><<<blocks_for(nb * Ki * d, 256), 256, 0, s>>>(x, ld, d, cand.data(), nb * Ki, xf.data());
-      B2_CUDA(cudaGetLastError());
-      if (norms) {
-        row_norms(s, qf.data(), nb, d, d, qn.data());
-        row_norms(s, xf.data(), nb * Ki, d, d, xfn.data());
-      }
       count_launch();
-      iota_kernel<<<blocks_for(nb * Ki, 256), 256, 0, s>>>(cand.data(), nb * Ki);
-      rescore_topk(s, qf.data(), nb, d, xf.data(), d, d, norms ? qn.data() : nullptr, norms ? xfn.data() : nullptr, metric, cand.data(), Ki,
-                   cand64.data(), degree, out_idx.data(), out_dist.data(), -1);
+      widen_rows_kernel<T><<<blocks_for(nb * d, 256), 256, 0, s>>>(x + b0 * ld, ld, d, nb, qf.data());
     }
+    B2_CUDA(cudaGetLastError());
+    // candidate positions are row ids: ties rank by id
+    rescore_topk(s, q, nb, ldq, x, ld, d, norms ? xn.data() + b0 : nullptr, norms ? xn.data() : nullptr, metric, cand.data(), Ki, nullptr,
+                 degree, out_idx.data(), out_dist.data(), -1);
     count_launch();
     narrow_ids_kernel<<<blocks_for(nb * degree, 256), 256, 0, s>>>(out_idx.data(), nb * degree, graph + b0 * degree);
     B2_CUDA(cudaGetLastError());
@@ -946,9 +910,8 @@ void run_typed(resources* r, const T* x, int64_t n, int d, int64_t ld, cuvsDista
   dbuf<float> inv;
   if (kind == kCos) {
     inv.alloc(static_cast<size_t>(n), s);
-    count_launch();
-    inv_norm_kernel<T><<<blocks_for(n, 128), 128, 0, s>>>(x, n, d, ld, inv.data());
-    B2_CUDA(cudaGetLastError());
+    row_norms(s, x, n, d, ld, inv.data());
+    rsqrt_rows(s, inv.data(), n, inv.data());
   }
   constexpr bool is_half = std::is_same<T, __half>::value;
   if (!half_path || (is_half && kind != kCos)) {
@@ -982,7 +945,7 @@ void run_typed(resources* r, const T* x, int64_t n, int d, int64_t ld, cuvsDista
 
 }  // namespace
 
-void nn_descent_graph(resources* r, const void* rows, DLDataType dt, int64_t n, int dim, int64_t ld, cuvsDistanceType metric, int degree,
+void nn_descent_graph(resources* r, const void* rows, row_type rt, int64_t n, int dim, int64_t ld, cuvsDistanceType metric, int degree,
                       int intermediate, int max_iterations, float termination_threshold, int dist_comp, uint32_t* graph, float* dist)
 {
   int kind = kL2;
@@ -993,7 +956,8 @@ void nn_descent_graph(resources* r, const void* rows, DLDataType dt, int64_t n, 
                   "nn-descent: metric %s (%d) is not supported; use L2Expanded, L2SqrtExpanded, InnerProduct, CosineExpanded or "
                   "BitwiseHamming (int8 / uint8 rows)",
                   metric_name(metric), static_cast<int>(metric));
-  B2_EXPECTS(kind != kHam || (dt.bits == 8 && (dt.code == kDLInt || dt.code == kDLUInt)),
+  const DLDataType dt = dtype_of(rt);
+  B2_EXPECTS(kind != kHam || row_bytes(rt) == 1,
              "nn-descent: BitwiseHamming distance is only supported for int8 and uint8 rows (got dtype code %d, bits %d)", dt.code, dt.bits);
   B2_EXPECTS(n >= 2 && n < (int64_t(1) << 30), "nn-descent: the dataset must have between 2 and 2^30 - 1 rows (got %lld)", (long long)n);
   B2_EXPECTS(dim >= 1, "nn-descent: the dataset has no columns");
@@ -1003,23 +967,15 @@ void nn_descent_graph(resources* r, const void* rows, DLDataType dt, int64_t n, 
   const int Ki = static_cast<int>(std::min<int64_t>(ki_want, n - 1));
   B2_EXPECTS(Ki <= kMaxKi, "nn-descent: intermediate_graph_degree %d exceeds %d", static_cast<int>(ki_want), kMaxKi);
   B2_EXPECTS(max_iterations >= 0, "nn-descent: max_iterations must be >= 0");
-  const bool f32 = dt.code == kDLFloat && dt.bits == 32;
-  B2_EXPECTS(dt.bits != 8 || dim <= 32768, "nn-descent: 8-bit rows are limited to 32768 columns (exact int32 sums), got %d", dim);
+  const bool f32 = rt == row_type::f32;
+  B2_EXPECTS(row_bytes(rt) != 1 || dim <= 32768, "nn-descent: 8-bit rows are limited to 32768 columns (exact int32 sums), got %d", dim);
   B2_EXPECTS(f32 || dist_comp != NND_DIST_COMP_FP32, "nn-descent: dist_comp_dtype FP32 is valid for float32 data only");
-  const bool half_path = f32 ? (dist_comp == NND_DIST_COMP_FP16 || (dist_comp == NND_DIST_COMP_AUTO && dim > 16)) : true;
-  if (f32)
-    run_typed<float>(r, static_cast<const float*>(rows), n, dim, ld, metric, kind, half_path, degree, Ki, max_iterations, termination_threshold,
-                     graph, dist);
-  else if (dt.code == kDLFloat && dt.bits == 16)
-    run_typed<__half>(r, static_cast<const __half*>(rows), n, dim, ld, metric, kind, true, degree, Ki, max_iterations, termination_threshold,
-                      graph, dist);
-  else if (dt.code == kDLInt && dt.bits == 8)
-    run_typed<int8_t>(r, static_cast<const int8_t*>(rows), n, dim, ld, metric, kind, false, degree, Ki, max_iterations, termination_threshold,
-                      graph, dist);
-  else if (dt.code == kDLUInt && dt.bits == 8)
-    run_typed<uint8_t>(r, static_cast<const uint8_t*>(rows), n, dim, ld, metric, kind, false, degree, Ki, max_iterations, termination_threshold,
-                       graph, dist);
-  else B2_FAIL("nn-descent: unsupported dataset dtype (code %d, bits %d)", dt.code, dt.bits);
+  const bool half_path = f32 ? (dist_comp == NND_DIST_COMP_FP16 || (dist_comp == NND_DIST_COMP_AUTO && dim > 16)) : rt == row_type::f16;
+  with_row_type(rt, [&](auto t) {
+    using T = decltype(t);
+    run_typed<T>(r, static_cast<const T*>(rows), n, dim, ld, metric, kind, half_path, degree, Ki, max_iterations, termination_threshold, graph,
+                 dist);
+  });
 }
 
 }  // namespace b200
@@ -1100,7 +1056,7 @@ cuvsError_t cuvsNNDescentBuild(cuvsResources_t res, cuvsNNDescentIndexParams_t p
     idx->degree = static_cast<int>(params->graph_degree);
     idx->graph.alloc(static_cast<size_t>(n) * idx->degree);
     if (params->return_distances) idx->dist.alloc(static_cast<size_t>(n) * idx->degree);
-    nn_descent_graph(r, rows, ds.dtype, n, dim, dim, params->metric, idx->degree,
+    nn_descent_graph(r, rows, row_type_of(ds.dtype), n, dim, dim, params->metric, idx->degree,
                      static_cast<int>(std::min<size_t>(params->intermediate_graph_degree, 1u << 30)),
                      static_cast<int>(std::min<size_t>(params->max_iterations, 1u << 30)), params->termination_threshold,
                      static_cast<int>(params->dist_comp_dtype), idx->graph.data(), idx->dist.data());

@@ -657,6 +657,47 @@ __global__ void pack_half_norms_kernel(const float* __restrict__ hn, int64_t row
   store_ext_row(hx + i * 16, hn[i]);
 }
 
+__global__ void split_items_kernel(tc_item* items, int m_tiles, int splits, int64_t nq, uint32_t b_tiles, int64_t row_stride)
+{
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= m_tiles * splits) return;
+  const int sp = i / m_tiles, m = i % m_tiles;
+  const uint32_t per = (b_tiles + splits - 1) / splits;
+  const uint32_t t0 = min(b_tiles, sp * per), t1 = min(b_tiles, t0 + per);
+  tc_item it;
+  it.a_row0     = m * 128;
+  it.b_row0     = t0 * 128;
+  it.n_tiles    = t1 - t0;
+  const int64_t valid = nq - static_cast<int64_t>(m) * 128;
+  it.valid_rows = valid > 128 ? 128 : static_cast<uint32_t>(valid);
+  it.out_off    = (static_cast<uint64_t>(m) * 128 * splits + sp) * row_stride;
+  items[i]      = it;
+}
+
+// One warp per row
+template <bool U8>
+__global__ void i8_norms_kernel(const uint8_t* __restrict__ rows, int64_t n_rows, int64_t n_live, int Kp, const int64_t* __restrict__ ids,
+                                const uint32_t* __restrict__ keep_bits, int64_t n_bits, int* __restrict__ norms)
+{
+  const int64_t r = (blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x) >> 5;
+  const int lane  = threadIdx.x & 31;
+  if (r >= n_rows) return;
+  int acc = 0;
+  for (int j = lane; j < Kp; j += 32) {
+    const int v = U8 ? static_cast<int>(rows[r * Kp + j]) : static_cast<int>(static_cast<int8_t>(rows[r * Kp + j]));
+    acc += v * v;
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
+  if (lane != 0) return;
+  bool live = r < n_live;
+  if (live && ids != nullptr) {
+    const int64_t id = ids[r];
+    live = id != kPadId && (keep_bits == nullptr || (id >= 0 && id < n_bits && ((keep_bits[id >> 5] >> (id & 31)) & 1u)));
+  }
+  norms[r] = live ? acc : kI8PadNorm;
+}
+
 }  // namespace
 
 bool tc_supported(int device, int d)
@@ -690,6 +731,27 @@ void tc_pack_half_norms(cudaStream_t stream, const float* hn, int64_t rows_pad, 
   if (rows_pad == 0) return;
   count_launch();
   pack_half_norms_kernel<<<static_cast<unsigned>((rows_pad + 255) / 256), 256, 0, stream>>>(hn, rows_pad, hx);
+  B2_CUDA(cudaGetLastError());
+}
+
+void tc_split_items(cudaStream_t stream, tc_item* items, int m_tiles, int splits, int64_t nq, uint32_t b_tiles, int64_t row_stride)
+{
+  const int n_items = m_tiles * splits;
+  if (n_items == 0) return;
+  count_launch();
+  split_items_kernel<<<blocks_for(n_items, 128), 128, 0, stream>>>(items, m_tiles, splits, nq, b_tiles, row_stride);
+  B2_CUDA(cudaGetLastError());
+}
+
+void tc_i8_norms(cudaStream_t stream, bool is_unsigned, const uint8_t* rows, int64_t n_rows, int64_t n_live, int Kp, const int64_t* ids,
+                 const uint32_t* keep_bits, int64_t n_bits, int* norms)
+{
+  if (n_rows == 0) return;
+  count_launch();
+  if (is_unsigned)
+    i8_norms_kernel<true><<<blocks_for(n_rows * 32, 256), 256, 0, stream>>>(rows, n_rows, n_live, Kp, ids, keep_bits, n_bits, norms);
+  else
+    i8_norms_kernel<false><<<blocks_for(n_rows * 32, 256), 256, 0, stream>>>(rows, n_rows, n_live, Kp, ids, keep_bits, n_bits, norms);
   B2_CUDA(cudaGetLastError());
 }
 

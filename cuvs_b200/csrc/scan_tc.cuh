@@ -25,6 +25,12 @@ struct tc_item {
   uint64_t out_off;     // element offset of (row 0, slot 0) in out_score/out_pos
 };
 
+/** items[m_tiles * splits]: every 128-row tile of the nq A rows against each of `splits` equal ranges of the b_tiles B tiles.
+ *  Item i is (range i / m_tiles, A tile i % m_tiles): split-major, so CTAs that run at the same time stream the same B range
+ *  (L2 reuse).  An item's out_off is (a_row0 * splits + s) * row_stride for range s: with an output row stride of
+ *  splits * row_stride, each A row keeps its ranges' outputs side by side. */
+void tc_split_items(cudaStream_t stream, tc_item* items, int m_tiles, int splits, int64_t nq, uint32_t b_tiles, int64_t row_stride);
+
 /**
  * Optional cross-item pruning bound (the role of `query_kths` in the reference's compute_similarity kernel,
  * cpp/src/neighbors/ivf_pq/detail/jit_lto_kernels/compute_distances_impl.cuh:64-65,96): work items that scan different
@@ -102,6 +108,15 @@ constexpr int kI8PadNorm = 0x7fffffff;
 __device__ __forceinline__ float tc_i8_key(int s) { return __int_as_float(s + kI8KeyBias); }
 __device__ __forceinline__ int tc_i8_score(float key) { return __float_as_int(key) - kI8KeyBias; }
 inline int tc_pad_k_i8(int d) { return (d + 127) / 128 * 128; }
+
+/** id stored on padding rows (the padding of IVF lists; any other int64, negative ones included, is a user id). */
+constexpr int64_t kPadId = INT64_MIN;
+
+/** norms[r] = the exact |x_r|^2 of the rows [n_rows, Kp] of a padded 8-bit plane (uint8 when `is_unsigned`), or kI8PadNorm
+ *  where row r is not live.  A row is live when r < n_live and, given ids, ids[r] is not kPadId and the bitset keep_bits
+ *  (n_bits bits, 1 = keep; null: all) keeps ids[r]. */
+void tc_i8_norms(cudaStream_t stream, bool is_unsigned, const uint8_t* rows, int64_t n_rows, int64_t n_live, int Kp, const int64_t* ids,
+                 const uint32_t* keep_bits, int64_t n_bits, int* norms);
 
 /**
  * tc_scan_topk over 8-bit rows: A [a_rows_pad, Kp] and B [b_rows_pad, Kp] int8 (uint8 when `is_unsigned`), K-major, Kp a
