@@ -24,69 +24,128 @@ namespace {
 // not below a full list's worst entry (its own list's, or through the bound shared between a query's items, another list's at
 // an earlier time; such entries only decrease), so every centre outside the candidates scores >= floor = the minimum over
 // the full lists of their worst entry.  If the n_probes-th candidate lies STRICTLY below the floor the selection — ties
-// included — is the dense one; otherwise, or when fewer than n_probes candidates exist, the query is counted in *n_flagged
-// and the caller redoes the batch through the dense path.
-constexpr int kCoarseMergeThreads = 128;
-constexpr int kCoarseMaxW         = 1024;
-template <int E>  // candidates per thread: W <= E * kCoarseMergeThreads
-__global__ void __launch_bounds__(kCoarseMergeThreads)
-coarse_merge_kernel(const float* __restrict__ cs, const uint32_t* __restrict__ cp, int W, int KC, int n_probes, uint32_t* __restrict__ probes,
-                    float* __restrict__ probe_scores, int* __restrict__ n_flagged)
+// included — is the dense one; otherwise, or when fewer than n_probes candidates exist, the query is flagged: its id goes to
+// flagged[*n_flagged] (in order of arrival) and the dense fallback recomputes its probes.
+constexpr int kCoarseMergeThreads = 128;  // four queries per CTA, one warp each
+constexpr int kCoarseMaxW         = 512;
+constexpr int kCoarseSlotBits     = 10;  // W < 2^10: a candidate's slot rides in its sort key, below the centre id
+constexpr int64_t kCoarseMaxCenters = int64_t(1) << (32 - kCoarseSlotBits);
+
+// Ascending bitonic sort of the warp's 32 E keys, key i = v[i / 32] of lane i % 32: partners 32 or more apart sit in the
+// lane's own registers, nearer ones in another lane (shuffles).
+template <int E>
+__device__ __forceinline__ void warp_bitonic_sort(unsigned long long (&v)[E], int lane)
 {
-  extern __shared__ unsigned long long ckeys[];
-  __shared__ float s_floor;
-  __shared__ int s_valid;
-  const int64_t q = blockIdx.x;
-  const int tid   = threadIdx.x;
-  unsigned long long mine[E];
-  int n_mine = 0;
-  if (tid == 0) s_valid = 0;
-  if (tid < 32) {
-    float m = INFINITY;
-    for (int l = tid; l * KC < W; l += 32) m = fminf(m, cs[q * W + l * KC + KC - 1]);
 #pragma unroll
-    for (int o = 16; o > 0; o >>= 1) m = fminf(m, __shfl_xor_sync(0xffffffffu, m, o));
-    if (tid == 0) s_floor = m;
+  for (int size = 2; size <= 32 * E; size <<= 1) {
+#pragma unroll
+    for (int j = size >> 1; j > 0; j >>= 1) {
+      if (j >= 32) {
+#pragma unroll
+        for (int e = 0; e < E; ++e) {
+          const int f = e ^ (j / 32);
+          if (f > e) {
+            const bool up = ((e * 32 + lane) & size) == 0;
+            const unsigned long long a = v[e], b = v[f];
+            if ((a > b) == up) { v[e] = b; v[f] = a; }
+          }
+        }
+      } else {
+#pragma unroll
+        for (int e = 0; e < E; ++e) {
+          const unsigned long long o = __shfl_xor_sync(0xffffffffu, v[e], j);
+          const bool up    = ((e * 32 + lane) & size) == 0;
+          const bool lower = (lane & j) == 0;
+          v[e] = (lower == up) ? (o < v[e] ? o : v[e]) : (o > v[e] ? o : v[e]);
+        }
+      }
+    }
   }
-  __syncthreads();
+}
+
+// The W keys (score key << 32 | centre id << 10 | slot) of a query, padded to 32 E with ~0, are sorted by its warp; keys
+// are unique, so sorted position r holds the candidate of rank r, whose score is read back through its slot.
+template <int E>
+__global__ void __launch_bounds__(kCoarseMergeThreads)
+coarse_merge_kernel(const float* __restrict__ cs, const uint32_t* __restrict__ cp, int64_t nq, int W, int KC, int n_probes,
+                    uint32_t* __restrict__ probes, float* __restrict__ probe_scores, int* __restrict__ n_flagged,
+                    uint32_t* __restrict__ flagged)
+{
+  const int64_t q = (blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x) >> 5;
+  const int lane  = threadIdx.x & 31;
+  if (q >= nq) return;
+  float m = INFINITY;
+  for (int l = lane; l * KC < W; l += 32) m = fminf(m, cs[q * W + l * KC + KC - 1]);
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) m = fminf(m, __shfl_xor_sync(0xffffffffu, m, o));
+  const float floor = m;
+  unsigned long long v[E];
+  int n_valid = 0;
 #pragma unroll
   for (int e = 0; e < E; ++e) {
-    const int c = e * kCoarseMergeThreads + tid;
-    unsigned long long K = ~0ull;
+    const int c = e * 32 + lane;
+    v[e]        = ~0ull;
     if (c < W) {
       const uint32_t pos = cp[q * W + c];
       if (pos != 0xffffffffu) {
         uint32_t u = __float_as_uint(cs[q * W + c]);
         if ((u << 1) == 0) u = 0;  // -0.0 == +0.0, as in select_k
         u = (u & 0x80000000u) ? ~u : (u | 0x80000000u);
-        K = (static_cast<unsigned long long>(u) << 32) | pos;
-        ++n_mine;
+        v[e] = (static_cast<unsigned long long>(u) << 32) | (static_cast<unsigned long long>(pos) << kCoarseSlotBits) | c;
       }
-      ckeys[c] = K;
     }
-    mine[e] = K;
+    n_valid += __popc(__ballot_sync(0xffffffffu, v[e] != ~0ull));
   }
-  if (n_mine) atomicAdd(&s_valid, n_mine);
-  __syncthreads();
-  int rank[E];
-#pragma unroll
-  for (int e = 0; e < E; ++e) rank[e] = 0;
-  for (int o = 0; o < W; ++o) {
-    const unsigned long long Ko = ckeys[o];  // (broadcast)
-#pragma unroll
-    for (int e = 0; e < E; ++e) rank[e] += Ko < mine[e] ? 1 : 0;
-  }
+  warp_bitonic_sort<E>(v, lane);
+  bool flag = n_valid < n_probes;
 #pragma unroll
   for (int e = 0; e < E; ++e) {
-    if (mine[e] != ~0ull && rank[e] < n_probes) {
-      const int c       = e * kCoarseMergeThreads + tid;
-      const float score = cs[q * W + c];
-      probes[q * n_probes + rank[e]]       = static_cast<uint32_t>(mine[e]);
-      probe_scores[q * n_probes + rank[e]] = score;
-      if (rank[e] == n_probes - 1 && !(score < s_floor)) atomicAdd(n_flagged, 1);  // (strict: also rules out boundary ties)
+    const int r = e * 32 + lane;
+    if (r < n_probes && v[e] != ~0ull) {
+      const float score              = cs[q * W + static_cast<int>(v[e] & ((1u << kCoarseSlotBits) - 1))];
+      probes[q * n_probes + r]       = static_cast<uint32_t>(v[e]) >> kCoarseSlotBits;
+      probe_scores[q * n_probes + r] = score;
+      if (r == n_probes - 1 && !(score < floor)) flag = true;  // (strict: also rules out boundary ties)
     }
   }
-  if (tid == 0 && s_valid < n_probes) atomicAdd(n_flagged, 1);
+  if (__any_sync(0xffffffffu, flag) && lane == 0) flagged[atomicAdd(n_flagged, 1)] = static_cast<uint32_t>(q);
+}
+
+// Dense fallback of the fused coarse search, for the flagged queries only, in passes of at most `rows` of them (the dense
+// score block of a pass is bounded, whatever the batch).  Every launch is sized for a full pass and reads the counts the
+// merge left on the device, so the search never waits for the host.  Pass p serves flagged[p * rows ...]: cnt[2] = its
+// queries, packed into rows [0, cnt[2]) of the planes, rows up to the next full tile zero; cnt[1] = their tiles, the
+// scan's item count.  cnt[0] = all flagged queries.
+__global__ void gather_flagged_rows_kernel(const uint4* __restrict__ hi, const uint4* __restrict__ lo, int row_vecs,
+                                           const uint32_t* __restrict__ flagged, int* __restrict__ cnt, int64_t first,
+                                           int64_t rows, uint4* __restrict__ f_hi, uint4* __restrict__ f_lo)
+{
+  const int64_t r   = (blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x) >> 5;
+  const int lane    = threadIdx.x & 31;
+  const int64_t nf  = min(rows, max(static_cast<int64_t>(cnt[0]) - first, int64_t(0)));
+  if (r == 0 && lane == 0) {
+    cnt[1] = static_cast<int>((nf + kTcTile - 1) / kTcTile);
+    cnt[2] = static_cast<int>(nf);
+  }
+  if (r >= (nf + kTcTile - 1) / kTcTile * kTcTile) return;
+  const int64_t src = r < nf ? static_cast<int64_t>(flagged[first + r]) : -1;
+  for (int j = lane; j < row_vecs; j += 32) {
+    f_hi[r * row_vecs + j] = src >= 0 ? hi[src * row_vecs + j] : make_uint4(0, 0, 0, 0);
+    if (f_lo) f_lo[r * row_vecs + j] = src >= 0 ? lo[src * row_vecs + j] : make_uint4(0, 0, 0, 0);
+  }
+}
+
+// a pass's probes (its row i: flagged query flagged[first + i]) over the fused path's
+__global__ void scatter_flagged_probes_kernel(const uint32_t* __restrict__ flagged, const int* __restrict__ cnt, int64_t first,
+                                              int n_probes, int64_t total, const uint32_t* __restrict__ f_probes,
+                                              const float* __restrict__ f_scores, uint32_t* __restrict__ probes,
+                                              float* __restrict__ probe_scores)
+{
+  const int64_t t = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x;
+  if (t >= total || t / n_probes >= cnt[2]) return;
+  const int64_t at  = static_cast<int64_t>(flagged[first + t / n_probes]) * n_probes + t % n_probes;
+  probes[at]        = f_probes[t];
+  probe_scores[at]  = f_scores[t];
 }
 
 // best entry among the heads of the `lists` sorted candidate lists of each row
@@ -123,14 +182,16 @@ __global__ void count_probes_kernel(const uint32_t* __restrict__ probes, int64_t
     atomicAdd(&counts[2 * l + (static_cast<int>(t % n_probes) < near_ranks ? 0 : 1)], 1u);
 }
 
-// single CTA: exclusive scans over lists of (a) pair counts, (b) "has a first item", (c) further items ceil(cnt/group) - 1
+// single CTA: exclusive scans over lists of (a) pair counts, (b) "has a first item", (c) further items ceil(cnt/group) - 1;
+// per 1024-list chunk, warp-shuffle scans and one scan of the 32 warp totals
 __global__ void __launch_bounds__(1024) scan_lists_kernel(const uint32_t* __restrict__ counts, int64_t n_lists, uint32_t group,
                                                            uint32_t* __restrict__ pair_off, uint32_t* __restrict__ first_off,
                                                            uint32_t* __restrict__ rest_off, int* __restrict__ n_items,
                                                            uint32_t* __restrict__ cursor)
 {
-  __shared__ uint32_t s_pairs[1024], s_first[1024], s_rest[1024];
+  __shared__ uint3 w_tot[32];
   __shared__ uint32_t run_pairs, run_first, run_rest;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   if (threadIdx.x == 0) { run_pairs = 0; run_first = 0; run_rest = 0; }
   __syncthreads();
   for (int64_t base = 0; base < n_lists; base += 1024) {
@@ -139,29 +200,39 @@ __global__ void __launch_bounds__(1024) scan_lists_kernel(const uint32_t* __rest
     uint32_t c  = c0 + (l < n_lists ? counts[2 * l + 1] : 0);
     uint32_t f  = c > 0 ? 1u : 0u;
     uint32_t g  = c > 0 ? (c + group - 1) / group - 1 : 0u;
-    s_pairs[threadIdx.x] = c;
-    s_first[threadIdx.x] = f;
-    s_rest[threadIdx.x]  = g;
-    __syncthreads();
-    for (int o = 1; o < 1024; o <<= 1) {
-      uint32_t a = 0, b = 0, d = 0;
-      if (threadIdx.x >= o) { a = s_pairs[threadIdx.x - o]; b = s_first[threadIdx.x - o]; d = s_rest[threadIdx.x - o]; }
-      __syncthreads();
-      s_pairs[threadIdx.x] += a;
-      s_first[threadIdx.x] += b;
-      s_rest[threadIdx.x]  += d;
-      __syncthreads();
+    uint32_t sp = c, sf = f, sg = g;  // inclusive scans within the warp
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+      const uint32_t a = __shfl_up_sync(0xffffffffu, sp, o), b = __shfl_up_sync(0xffffffffu, sf, o),
+                     d = __shfl_up_sync(0xffffffffu, sg, o);
+      if (lane >= o) { sp += a; sf += b; sg += d; }
     }
+    if (lane == 31) w_tot[warp] = make_uint3(sp, sf, sg);
+    __syncthreads();
+    if (warp == 0) {  // exclusive scan of the warp totals
+      const uint3 t = w_tot[lane];
+      uint32_t ip = t.x, iff = t.y, ig = t.z;
+#pragma unroll
+      for (int o = 1; o < 32; o <<= 1) {
+        const uint32_t a = __shfl_up_sync(0xffffffffu, ip, o), b = __shfl_up_sync(0xffffffffu, iff, o),
+                       d = __shfl_up_sync(0xffffffffu, ig, o);
+        if (lane >= o) { ip += a; iff += b; ig += d; }
+      }
+      w_tot[lane] = make_uint3(ip - t.x, iff - t.y, ig - t.z);
+    }
+    __syncthreads();
+    const uint3 w = w_tot[warp];
+    sp += w.x; sf += w.y; sg += w.z;  // inclusive over the chunk
     if (l < n_lists) {
-      pair_off[2 * l]     = run_pairs + s_pairs[threadIdx.x] - c;
-      pair_off[2 * l + 1] = run_pairs + s_pairs[threadIdx.x] - c + c0;
-      first_off[l]        = run_first + s_first[threadIdx.x] - f;
-      rest_off[l]         = run_rest + s_rest[threadIdx.x] - g;
+      pair_off[2 * l]     = run_pairs + sp - c;
+      pair_off[2 * l + 1] = run_pairs + sp - c + c0;
+      first_off[l]        = run_first + sf - f;
+      rest_off[l]         = run_rest + sg - g;
       cursor[2 * l]       = 0;
       cursor[2 * l + 1]   = 0;
     }
     __syncthreads();
-    if (threadIdx.x == 1023) { run_pairs += s_pairs[1023]; run_first += s_first[1023]; run_rest += s_rest[1023]; }
+    if (threadIdx.x == 1023) { run_pairs += sp; run_first += sf; run_rest += sg; }
     __syncthreads();
   }
   if (threadIdx.x == 0) {
@@ -328,13 +399,16 @@ __device__ __forceinline__ float order_key_inv(uint32_t k)
   return __uint_as_float((k & 0x80000000u) ? (k & 0x7fffffffu) : ~k);
 }
 
-constexpr int kMergeThreads = 256;
-constexpr int kMergeCap     = 1024;
+constexpr int kMergeCap = 1024;
 
+// kMergeThreads: 128 while a query has at most 2048 candidates (a filter trip takes 4 x 128 of them: the flagship's 48 x 32
+// take three trips, and twice the CTAs fit an SM; 0.09 ms per 10k batch against 0.11 ms with 256), else 256 (more loads in
+// flight per query: at 192 probes x 64 candidates the search took 0.7 ms longer per 10k batch with 128)
+template <int kMergeThreads>
 __global__ void __launch_bounds__(kMergeThreads)
 merge_pairs_kernel(const float* __restrict__ cs, const uint32_t* __restrict__ cp, const uint32_t* __restrict__ slot_of,
                    const float* __restrict__ add, float scale, const int* __restrict__ bound_keys, int n_probes, int KCW,
-                   int k, float* __restrict__ out_val, uint32_t* __restrict__ out_pos)
+                   int kcw_shift, int k, float* __restrict__ out_val, uint32_t* __restrict__ out_pos)
 {
   __shared__ unsigned long long surv[kMergeCap];  // (order key << 32 | position)
   __shared__ unsigned long long red[kMergeThreads / 32];
@@ -366,12 +440,12 @@ merge_pairs_kernel(const float* __restrict__ cs, const uint32_t* __restrict__ cp
 #pragma unroll
     for (int u = 0; u < 4; ++u) {
       const int e = e0 + u * kMergeThreads;
-      slot[u]     = e < total ? my_slots[e / KCW] : 0xffffffffu;
+      slot[u]     = e < total ? my_slots[kcw_shift >= 0 ? e >> kcw_shift : e / KCW] : 0xffffffffu;
     }
 #pragma unroll
     for (int u = 0; u < 4; ++u) {
       const int e = e0 + u * kMergeThreads;
-      const int c = e % KCW;
+      const int c = kcw_shift >= 0 ? e & (KCW - 1) : e % KCW;
       pos[u] = 0xffffffffu; sc[u] = 0.f; ad[u] = 0.f;
       if (slot[u] != 0xffffffffu) {
         pos[u] = cp[static_cast<int64_t>(slot[u]) * KCW + c];
@@ -399,7 +473,7 @@ merge_pairs_kernel(const float* __restrict__ cs, const uint32_t* __restrict__ cp
     for (int size = 2; size <= n2; size <<= 1) {
       for (int stride = size >> 1; stride > 0; stride >>= 1) {
         for (int i = threadIdx.x; i < n2 / 2; i += blockDim.x) {
-          const int lo = (i / stride) * stride * 2 + (i % stride);
+          const int lo = ((i & ~(stride - 1)) << 1) | (i & (stride - 1));  // (stride is a power of two)
           const int hi = lo + stride;
           const bool up = ((lo & size) == 0);
           const unsigned long long a = surv[lo], b = surv[hi];
@@ -619,30 +693,53 @@ void tc_rows_tmp::build(cudaStream_t s, const float* x, int64_t n_, int d_, bool
   tc_split_planes(s, x, n, d, d, Kp, hi.data(), with_lo ? lo.data() : nullptr, rows_pad, row_scale);
 }
 
+// The dense coarse search of the queries in rows [0, n) of the planes a_hi / a_lo: every score, then select_k.  With
+// n_rows_dev the planes' rows are sized for n queries and the count is the device's: launches past it exit at once.
+static void coarse_select_dense(resources* res, const __nv_bfloat16* a_hi, const __nv_bfloat16* a_lo, int64_t n, int64_t a_rows_pad,
+                                const tc_rows& centers, int n_probes, uint32_t* probes, float* probe_scores,
+                                const int* n_rows_dev = nullptr, const int* n_tiles_dev = nullptr)
+{
+  auto s               = res->stream;
+  const int m_tiles    = static_cast<int>(tc_pad_rows(n) / 128);
+  const int64_t ld     = centers.rows_pad;
+  dbuf<tc_item> items(static_cast<size_t>(m_tiles), s);
+  tc_split_items(s, items.data(), m_tiles, 1, n, static_cast<uint32_t>(ld / 128), ld);
+  dbuf<float> scores(static_cast<size_t>(tc_pad_rows(n)) * ld, s);
+  const bool three = a_lo != nullptr && centers.lo.data() != nullptr;
+  tc_scan_topk(s, res->device, a_hi, a_lo, a_rows_pad, centers.hi.data(), centers.lo.data(), centers.rows_pad, centers.Kp,
+               centers.hx.data(), items.data(), m_tiles, n_tiles_dev, 0, three ? 3 : 1, scores.data(), nullptr, ld);
+  select_k(s, scores.data(), nullptr, IDX_NONE, n, centers.n, ld, n_probes, probe_scores, probes, IDX_U32, true, n_rows_dev);
+}
+
 // Fused coarse search (large n_lists): instead of writing the dense [nq, n_lists] score block (655 MB at 10k x 16384) and
-// selecting from it, the scan keeps 32 candidates per (query, centre range, column half) in its epilogue — (query tile, centre
+// selecting from it, the scan keeps KC candidates per (query, centre range, column half) in its epilogue — (query tile, centre
 // range) items also give the SMs ~2 waves of work where one item per query tile gave 79 CTAs — and a small merge ranks
-// the 2 * splits * 32 candidates per query.  Exact (same scores, same (score, id) order as the dense select) whenever the merge
-// kernel's certificate holds for every query of the batch; returns false when the dense path has to run (one host read of
-// the flag count per search).
+// the 2 * splits * KC candidates per query.  Exact (same scores, same (score, id) order as the dense select) for every query
+// whose merge certificate holds; the queries it flags are packed and take the dense path, with launches sized for a fully
+// flagged batch (a row's scores do not depend on where it sits in the planes, so their probes are the dense path's too).
+// Nothing waits for the host: the whole search can be enqueued ahead of the device, or captured in a CUDA graph.  Returns
+// false when the shape does not suit the fused scan.
 static bool coarse_select_fused(resources* res, const tc_rows_tmp& q, const tc_rows& centers, int n_probes, uint32_t* probes,
                                 float* probe_scores)
 {
   const char* env = getenv("CUVS_B200_COARSE_FUSED");  // read per call (A/B inside one process): "0" = dense path
   if (env != nullptr && env[0] == '0') return false;
-  const int KC = 32;
-  if (n_probes > 2 * KC || centers.n < 4096) return false;
+  // Lists of 16: the epilogue's insertions, not the tensor cores, set the scan's pace, and a list of 16 costs about half
+  // of one of 32 (flagship shape, 10k queries x 8192 centres: 0.31 ms against 0.54 ms, the same probes).  More lists make
+  // up the candidates: W >= 4 n_probes below.
+  const int KC = 16;
+  if (n_probes > 64 || centers.n < 4096 || centers.n > kCoarseMaxCenters) return false;
   auto s               = res->stream;
   const int64_t nq_pad = tc_pad_rows(q.n);
   const int m_tiles    = static_cast<int>(nq_pad / 128);
   const int64_t b_tiles = centers.rows_pad / 128;
   const int sms        = res->sm_count ? res->sm_count : 132;
+  const int KCW = KC * kTcListsPerItem;
   // enough items for ~2 waves of CTAs, and enough lists that the n_probes best are spread thin (>= 4 n_probes candidates:
   // with only n_probes candidates the certificate could never hold and every batch would pay for both paths)
-  int splits = std::max((2 * sms + m_tiles - 1) / m_tiles, (n_probes + 15) / 16);
+  int splits = std::max((2 * sms + m_tiles - 1) / m_tiles, (4 * n_probes + KCW - 1) / KCW);
   splits     = static_cast<int>(std::min<int64_t>(splits, std::min<int64_t>(16, b_tiles / 4)));
   splits     = std::max(splits, 1);
-  const int KCW = KC * kTcListsPerItem;
   const int W   = splits * KCW;
   if (W > kCoarseMaxW || W < 4 * n_probes) return false;
   const int n_items = m_tiles * splits;
@@ -650,33 +747,54 @@ static bool coarse_select_fused(resources* res, const tc_rows_tmp& q, const tc_r
   tc_split_items(s, items.data(), m_tiles, splits, q.n, static_cast<uint32_t>(b_tiles), KCW);  // (centre range, query tile) items
   dbuf<float> cs(static_cast<size_t>(nq_pad) * W, s);
   dbuf<uint32_t> cp(static_cast<size_t>(nq_pad) * W, s);
-  dbuf<int> bkeys(static_cast<size_t>(nq_pad) + 1, s);
+  dbuf<int> bkeys(static_cast<size_t>(nq_pad) + 3, s);
   B2_CUDA(cudaMemsetAsync(bkeys.data(), tc_bound_init_byte, sizeof(int) * nq_pad, s));
-  int* n_flagged = bkeys.data() + nq_pad;
+  int* n_flagged = bkeys.data() + nq_pad;  // [0] flagged queries, [1] [2] a fallback pass's tiles and queries
   B2_CUDA(cudaMemsetAsync(n_flagged, 0, sizeof(int), s));
+  dbuf<uint32_t> flagged(static_cast<size_t>(q.n), s);
   tc_bound bnd;
   bnd.keys = bkeys.data();
-  bnd.kth  = 0;  // lists prune at, and publish, their last (32nd) entry: that is what the merge's certificate reasons about
+  bnd.kth  = 0;  // lists prune at, and publish, their last (KC-th) entry: that is what the merge's certificate reasons about
   const bool three = q.lo.data() != nullptr && centers.lo.data() != nullptr;
   tc_scan_topk(s, res->device, q.hi.data(), q.lo.data(), q.rows_pad, centers.hi.data(), centers.lo.data(), centers.rows_pad,
                q.Kp, centers.hx.data(), items.data(), n_items, nullptr, KC, three ? 3 : 1, cs.data(), cp.data(), W, &bnd);
   count_launch();
   {
-    const unsigned grid = static_cast<unsigned>(q.n);
-    const size_t smem   = static_cast<size_t>(W) * 8;
-    const int per       = (W + kCoarseMergeThreads - 1) / kCoarseMergeThreads;
-#define B2_CM(E_) coarse_merge_kernel<E_><<<grid, kCoarseMergeThreads, smem, s>>>(cs.data(), cp.data(), W, KC, n_probes, probes, probe_scores, n_flagged)
-    if (per <= 1) B2_CM(1);
-    else if (per <= 2) B2_CM(2);
-    else if (per <= 4) B2_CM(4);
-    else B2_CM(8);
+    const unsigned grid = static_cast<unsigned>(blocks_for(q.n * 32, kCoarseMergeThreads));
+#define B2_CM(E_) coarse_merge_kernel<E_><<<grid, kCoarseMergeThreads, 0, s>>>(cs.data(), cp.data(), q.n, W, KC, n_probes, probes, probe_scores, n_flagged, flagged.data())
+    if (W <= 64) B2_CM(2);
+    else if (W <= 128) B2_CM(4);
+    else if (W <= 256) B2_CM(8);
+    else B2_CM(16);
 #undef B2_CM
   }
   B2_CUDA(cudaGetLastError());
-  int flagged = 0;
-  B2_CUDA(cudaMemcpyAsync(&flagged, n_flagged, sizeof(int), cudaMemcpyDeviceToHost, s));
-  B2_CUDA(cudaStreamSynchronize(s));
-  return flagged == 0;
+  cs.release();
+  cp.release();
+  // the flagged queries, in passes: packed planes, the dense scan + select, their probes scattered over the fused ones.  A
+  // pass's dense scores stay within 256 MiB; the flagship batch (10k queries, 8192 centres) takes two passes, and each
+  // pass past the flagged count costs four near-empty launches.
+  const int64_t pass_rows = std::max<int64_t>(kTcTile, std::min<int64_t>(nq_pad, ((int64_t(1) << 26) / centers.rows_pad) / kTcTile * kTcTile));
+  dbuf<__nv_bfloat16> f_hi(static_cast<size_t>(pass_rows) * q.Kp, s), f_lo;
+  if (three) f_lo.alloc(static_cast<size_t>(pass_rows) * q.Kp, s);
+  dbuf<uint32_t> f_probes(static_cast<size_t>(pass_rows) * n_probes, s);
+  dbuf<float> f_scores(static_cast<size_t>(pass_rows) * n_probes, s);
+  const int64_t total = pass_rows * n_probes;
+  for (int64_t first = 0; first < q.n; first += pass_rows) {
+    count_launch();
+    gather_flagged_rows_kernel<<<blocks_for(pass_rows * 32, 256), 256, 0, s>>>(
+      reinterpret_cast<const uint4*>(q.hi.data()), three ? reinterpret_cast<const uint4*>(q.lo.data()) : nullptr, q.Kp / 8,
+      flagged.data(), n_flagged, first, pass_rows, reinterpret_cast<uint4*>(f_hi.data()),
+      three ? reinterpret_cast<uint4*>(f_lo.data()) : nullptr);
+    B2_CUDA(cudaGetLastError());
+    coarse_select_dense(res, f_hi.data(), f_lo.data(), pass_rows, pass_rows, centers, n_probes, f_probes.data(), f_scores.data(),
+                        n_flagged + 2, n_flagged + 1);
+    count_launch();
+    scatter_flagged_probes_kernel<<<blocks_for(total, 256), 256, 0, s>>>(flagged.data(), n_flagged, first, n_probes, total,
+                                                                          f_probes.data(), f_scores.data(), probes, probe_scores);
+    B2_CUDA(cudaGetLastError());
+  }
+  return true;
 }
 
 void coarse_select(resources* res, const tc_rows_tmp& q, const tc_rows& centers, int n_probes, uint32_t* probes,
@@ -688,16 +806,7 @@ void coarse_select(resources* res, const tc_rows_tmp& q, const tc_rows& centers,
   dbuf<float> tmp_scores;
   if (!probe_scores) { tmp_scores.alloc(static_cast<size_t>(q.n) * n_probes, s); probe_scores = tmp_scores.data(); }
   if (coarse_select_fused(res, q, centers, n_probes, probes, probe_scores)) return;
-  const int64_t nq_pad = tc_pad_rows(q.n);
-  const int m_tiles    = static_cast<int>(nq_pad / 128);
-  const int64_t ld     = centers.rows_pad;
-  dbuf<tc_item> items(static_cast<size_t>(m_tiles), s);
-  tc_split_items(s, items.data(), m_tiles, 1, q.n, static_cast<uint32_t>(ld / 128), ld);
-  dbuf<float> scores(static_cast<size_t>(nq_pad) * ld, s);
-  const bool three = q.lo.data() != nullptr && centers.lo.data() != nullptr;
-  tc_scan_topk(s, res->device, q.hi.data(), q.lo.data(), q.rows_pad, centers.hi.data(), centers.lo.data(), centers.rows_pad,
-               q.Kp, centers.hx.data(), items.data(), m_tiles, nullptr, 0, three ? 3 : 1, scores.data(), nullptr, ld);
-  select_k(s, scores.data(), nullptr, IDX_NONE, q.n, centers.n, ld, n_probes, probe_scores, probes, IDX_U32, true);
+  coarse_select_dense(res, q.hi.data(), q.lo.data(), q.n, q.rows_pad, centers, n_probes, probes, probe_scores);
 }
 
 void assign_nearest(resources* res, const __nv_bfloat16* x_hi, const __nv_bfloat16* x_lo, int64_t n, int64_t x_rows_pad,
@@ -964,8 +1073,13 @@ bool merge_probe_candidates(cudaStream_t s, const float* cs, const uint32_t* cp,
   // without a bound nothing is filtered: the generic gather + radix select is the better tool then
   if (bound_keys == nullptr && static_cast<int64_t>(n_probes) * KCW > kMergeCap) return false;
   count_launch();
-  merge_pairs_kernel<<<static_cast<unsigned>(nq), kMergeThreads, 0, s>>>(cs, cp, slot_of, add, scale, bound_keys, n_probes, KCW, k,
-                                                                          out_val, out_pos);
+  const int kcw_shift = (KCW & (KCW - 1)) == 0 ? __builtin_ctz(static_cast<unsigned>(KCW)) : -1;  // -1: not a power of two
+  if (static_cast<int64_t>(n_probes) * KCW <= 2048)
+    merge_pairs_kernel<128><<<static_cast<unsigned>(nq), 128, 0, s>>>(cs, cp, slot_of, add, scale, bound_keys, n_probes, KCW, kcw_shift,
+                                                                     k, out_val, out_pos);
+  else
+    merge_pairs_kernel<256><<<static_cast<unsigned>(nq), 256, 0, s>>>(cs, cp, slot_of, add, scale, bound_keys, n_probes, KCW, kcw_shift,
+                                                                     k, out_val, out_pos);
   B2_CUDA(cudaGetLastError());
   return true;
 }

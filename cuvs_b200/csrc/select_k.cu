@@ -66,7 +66,8 @@ __global__ void __launch_bounds__(1024) select_k_kernel(const float* __restrict_
                                                           float* __restrict__ out_val,
                                                           IdxOut* __restrict__ out_idx,
                                                           bool select_min,
-                                                          seg_rows seg = seg_rows{})
+                                                          seg_rows seg = seg_rows{},
+                                                          const int* __restrict__ live_rows = nullptr)
 {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   uint32_t* hist     = reinterpret_cast<uint32_t*>(smem_raw);
@@ -75,6 +76,7 @@ __global__ void __launch_bounds__(1024) select_k_kernel(const float* __restrict_
   uint64_t* skeys    = reinterpret_cast<uint64_t*>(warp_tot + 32);
 
   const int64_t row = blockIdx.x;
+  if (live_rows != nullptr && row >= *live_rows) return;
   const float* v    = in_val + row * in_ld;
   const int tid     = threadIdx.x;
   const int bs      = blockDim.x;
@@ -232,7 +234,8 @@ constexpr int kRegMaxK    = 256;
 template <int E, typename IdxIn, typename IdxOut, bool HasIdx>
 __global__ void __launch_bounds__(kRegThreads, E <= 32 ? 2 : 1) select_k_reg_kernel(const float* __restrict__ in_val, const IdxIn* __restrict__ in_idx,
                                                                    int64_t len, int64_t in_ld, int k, float* __restrict__ out_val,
-                                                                   IdxOut* __restrict__ out_idx, bool select_min, int sample_elems)
+                                                                   IdxOut* __restrict__ out_idx, bool select_min, int sample_elems,
+                                                                   int64_t batch, const int* __restrict__ live_rows)
 {
   __shared__ __align__(16) uint32_t hist[kRegBins];
   __shared__ unsigned long long okeys[kRegMaxK];
@@ -241,157 +244,162 @@ __global__ void __launch_bounds__(kRegThreads, E <= 32 ? 2 : 1) select_k_reg_ker
   __shared__ uint32_t wtot[kRegThreads / 32];
   __shared__ uint32_t scal[8];  // [0] threshold bucket [1] keys below it [2] keys in it [3] winners stored [4] bucket keys stored
 
-  const int64_t row = blockIdx.x;
-  const float* v    = in_val + row * in_ld;
-  const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
-  const int k_eff = len < k ? static_cast<int>(len) : k;
+  // rows past *live_rows (when given) are not selected; a grid smaller than the batch strides over its rows
+  const int64_t n_rows = live_rows != nullptr ? min(batch, static_cast<int64_t>(*live_rows)) : batch;
+  for (int64_t row = blockIdx.x; row < n_rows; row += gridDim.x) {
+    const float* v    = in_val + row * in_ld;
+    const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
+    const int k_eff = len < k ? static_cast<int>(len) : k;
 
-  uint32_t u[E];
-  uint32_t mn = 0xffffffffu, mx = 0u;  // bounds on the 32-bit keys are enough: the span only has to COVER the composites
-#pragma unroll
-  for (int j = 0; j < E; ++j) {
-    const int64_t i = static_cast<int64_t>(j) * kRegThreads + tid;
-    u[j] = 0u;
-    if (i < len) {
-      u[j] = f2key(v[i], select_min);
-      mn   = min(mn, u[j]);
-      mx   = max(mx, u[j]);
-    }
-  }
-  mn = __reduce_min_sync(0xffffffffu, mn);
-  mx = __reduce_max_sync(0xffffffffu, mx);
-  if (lane == 0) { red[wid] = mn; red[kRegThreads / 32 + wid] = mx; }
-  if (tid == 0) { scal[3] = 0; scal[4] = 0; }
-  __syncthreads();
-  uint32_t lo32 = red[lane & (kRegThreads / 32 - 1)], hi32 = red[kRegThreads / 32 + (lane & (kRegThreads / 32 - 1))];
-  lo32 = __reduce_min_sync(0xffffffffu, lo32);
-  hi32 = __reduce_max_sync(0xffffffffu, hi32);
-  unsigned long long lo = static_cast<unsigned long long>(lo32) << 32, hi = (static_cast<unsigned long long>(hi32) << 32) | 0xffffffffull;
-  const unsigned long long full_span = hi - lo;
-  unsigned long long span = full_span;  // keys in play: lo <= K <= lo + span
-  uint32_t need = static_cast<uint32_t>(k_eff);
-
-  // Sampled upper bound.  k << len (48 probes out of 16k centres): binning the whole row spends one shared-memory atomic per
-  // element on keys that cannot win.  Take the first `es` elements of every thread as a sample (es * 32 per warp, strided over
-  // the row), T = max over the warps of the warp's sample MINIMUM: every warp has a key <= T, and for es * 32 ~ 0.7 len / k
-  // about 1 % .. 3 % of the row lies below T, of which the k-th smallest is one with overwhelming probability (k = 48,
-  // len = 16384: miss rate ~ 4e-5 on exchangeable data).  The first binning round then only counts keys <= T; if fewer than
-  // `need` keys are there (adversarial order, e.g. a sorted row) the round is repeated over the full span — exactness never
-  // depends on the sample.  sample_elems (the launcher's ~0.7 len / (32 k), at most 64) is 0 when k is large against len.
-  if (sample_elems > 0) {
-    uint32_t smin = 0xffffffffu;
+    uint32_t u[E];
+    uint32_t mn = 0xffffffffu, mx = 0u;  // bounds on the 32-bit keys are enough: the span only has to COVER the composites
 #pragma unroll
     for (int j = 0; j < E; ++j) {
       const int64_t i = static_cast<int64_t>(j) * kRegThreads + tid;
-      if (j < sample_elems && i < len) smin = min(smin, u[j]);
-    }
-    smin = __reduce_min_sync(0xffffffffu, smin);
-    __syncthreads();  // (red[] is still being read above)
-    if (lane == 0) red[wid] = smin;
-    __syncthreads();
-    uint32_t t32 = red[lane & (kRegThreads / 32 - 1)];
-    t32 = __reduce_max_sync(0xffffffffu, t32);
-    if (t32 < hi32) span = ((static_cast<unsigned long long>(t32) << 32) | 0xffffffffull) - lo;
-  }
-
-  while (need > 0) {
-    const int s = span >= static_cast<unsigned long long>(kRegBins) ? (64 - __clzll(static_cast<long long>(span))) - 11 : 0;  // (span >> s) < 2048
-    for (int i = tid; i < kRegBins; i += kRegThreads) hist[i] = 0;
-    if (tid == 0) scal[0] = 0xffffffffu;  // "no bucket reaches `need`" until the scan says otherwise
-    __syncthreads();
-#pragma unroll
-    for (int j = 0; j < E; ++j) {
-      const int64_t i = static_cast<int64_t>(j) * kRegThreads + tid;
-      const unsigned long long K = (static_cast<unsigned long long>(u[j]) << 32) | static_cast<uint32_t>(i);
-      if (i < len && K >= lo && K - lo <= span) atomicAdd(&hist[static_cast<uint32_t>((K - lo) >> s)], 1u);
-    }
-    __syncthreads();
-    {
-      // two-level scan, all 16 warps: warp w owns buckets [128 w, 128 w + 128), lane l four of them (one conflict-free 128-bit load)
-      static_assert(kRegBins == 4 * kRegThreads, "one uint4 of buckets per thread");
-      const uint4 h4 = reinterpret_cast<const uint4*>(hist)[tid];
-      const uint32_t sum = h4.x + h4.y + h4.z + h4.w;
-      uint32_t incl = sum;
-#pragma unroll
-      for (int o = 1; o < 32; o <<= 1) {
-        const uint32_t t = __shfl_up_sync(0xffffffffu, incl, o);
-        if (lane >= o) incl += t;
+      u[j] = 0u;
+      if (i < len) {
+        u[j] = f2key(v[i], select_min);
+        mn   = min(mn, u[j]);
+        mx   = max(mx, u[j]);
       }
-      if (lane == 31) wtot[wid] = incl;
+    }
+    mn = __reduce_min_sync(0xffffffffu, mn);
+    mx = __reduce_max_sync(0xffffffffu, mx);
+    if (lane == 0) { red[wid] = mn; red[kRegThreads / 32 + wid] = mx; }
+    if (tid == 0) { scal[3] = 0; scal[4] = 0; }
+    __syncthreads();
+    uint32_t lo32 = red[lane & (kRegThreads / 32 - 1)], hi32 = red[kRegThreads / 32 + (lane & (kRegThreads / 32 - 1))];
+    lo32 = __reduce_min_sync(0xffffffffu, lo32);
+    hi32 = __reduce_max_sync(0xffffffffu, hi32);
+    unsigned long long lo = static_cast<unsigned long long>(lo32) << 32, hi = (static_cast<unsigned long long>(hi32) << 32) | 0xffffffffull;
+    const unsigned long long full_span = hi - lo;
+    unsigned long long span = full_span;  // keys in play: lo <= K <= lo + span
+    uint32_t need = static_cast<uint32_t>(k_eff);
+
+    // Sampled upper bound.  k << len (48 probes out of 16k centres): binning the whole row spends one shared-memory atomic per
+    // element on keys that cannot win.  Take the first `es` elements of every thread as a sample (es * 32 per warp, strided over
+    // the row), T = max over the warps of the warp's sample MINIMUM: every warp has a key <= T, and for es * 32 ~ 0.7 len / k
+    // about 1 % .. 3 % of the row lies below T, of which the k-th smallest is one with overwhelming probability (k = 48,
+    // len = 16384: miss rate ~ 4e-5 on exchangeable data).  The first binning round then only counts keys <= T; if fewer than
+    // `need` keys are there (adversarial order, e.g. a sorted row) the round is repeated over the full span — exactness never
+    // depends on the sample.  sample_elems (the launcher's ~0.7 len / (32 k), at most 64) is 0 when k is large against len.
+    if (sample_elems > 0) {
+      uint32_t smin = 0xffffffffu;
+#pragma unroll
+      for (int j = 0; j < E; ++j) {
+        const int64_t i = static_cast<int64_t>(j) * kRegThreads + tid;
+        if (j < sample_elems && i < len) smin = min(smin, u[j]);
+      }
+      smin = __reduce_min_sync(0xffffffffu, smin);
+      __syncthreads();  // (red[] is still being read above)
+      if (lane == 0) red[wid] = smin;
       __syncthreads();
-      uint32_t c = incl - sum;
+      uint32_t t32 = red[lane & (kRegThreads / 32 - 1)];
+      t32 = __reduce_max_sync(0xffffffffu, t32);
+      if (t32 < hi32) span = ((static_cast<unsigned long long>(t32) << 32) | 0xffffffffull) - lo;
+    }
+
+    while (need > 0) {
+      const int s = span >= static_cast<unsigned long long>(kRegBins) ? (64 - __clzll(static_cast<long long>(span))) - 11 : 0;  // (span >> s) < 2048
+      for (int i = tid; i < kRegBins; i += kRegThreads) hist[i] = 0;
+      if (tid == 0) scal[0] = 0xffffffffu;  // "no bucket reaches `need`" until the scan says otherwise
+      __syncthreads();
 #pragma unroll
-      for (int w = 0; w < kRegThreads / 32; ++w) c += w < wid ? wtot[w] : 0u;
-      if (c < need && need <= c + sum) {  // exactly one thread: the bucket where the running count reaches `need`
-        const uint32_t h[4] = {h4.x, h4.y, h4.z, h4.w};
+      for (int j = 0; j < E; ++j) {
+        const int64_t i = static_cast<int64_t>(j) * kRegThreads + tid;
+        const unsigned long long K = (static_cast<unsigned long long>(u[j]) << 32) | static_cast<uint32_t>(i);
+        if (i < len && K >= lo && K - lo <= span) atomicAdd(&hist[static_cast<uint32_t>((K - lo) >> s)], 1u);
+      }
+      __syncthreads();
+      {
+        // two-level scan, all 16 warps: warp w owns buckets [128 w, 128 w + 128), lane l four of them (one conflict-free 128-bit load)
+        static_assert(kRegBins == 4 * kRegThreads, "one uint4 of buckets per thread");
+        const uint4 h4 = reinterpret_cast<const uint4*>(hist)[tid];
+        const uint32_t sum = h4.x + h4.y + h4.z + h4.w;
+        uint32_t incl = sum;
 #pragma unroll
-        for (int e = 0; e < 4; ++e) {
-          if (c < need && need <= c + h[e]) { scal[0] = tid * 4 + e; scal[1] = c; scal[2] = h[e]; }
-          c += h[e];
+        for (int o = 1; o < 32; o <<= 1) {
+          const uint32_t t = __shfl_up_sync(0xffffffffu, incl, o);
+          if (lane >= o) incl += t;
+        }
+        if (lane == 31) wtot[wid] = incl;
+        __syncthreads();
+        uint32_t c = incl - sum;
+#pragma unroll
+        for (int w = 0; w < kRegThreads / 32; ++w) c += w < wid ? wtot[w] : 0u;
+        if (c < need && need <= c + sum) {  // exactly one thread: the bucket where the running count reaches `need`
+          const uint32_t h[4] = {h4.x, h4.y, h4.z, h4.w};
+#pragma unroll
+          for (int e = 0; e < 4; ++e) {
+            if (c < need && need <= c + h[e]) { scal[0] = tid * 4 + e; scal[1] = c; scal[2] = h[e]; }
+            c += h[e];
+          }
         }
       }
-    }
-    __syncthreads();
-    const uint32_t bstar = scal[0], below = scal[1], inb = scal[2];
-    if (bstar == 0xffffffffu) {  // (block-uniform; first round only) the sampled bound cut below the k-th key: full span
-      span = full_span;
       __syncthreads();
-      continue;
-    }
-    const bool finish = inb <= static_cast<uint32_t>(kRegEqCap);
+      const uint32_t bstar = scal[0], below = scal[1], inb = scal[2];
+      if (bstar == 0xffffffffu) {  // (block-uniform; first round only) the sampled bound cut below the k-th key: full span
+        span = full_span;
+        __syncthreads();
+        continue;
+      }
+      const bool finish = inb <= static_cast<uint32_t>(kRegEqCap);
 #pragma unroll
-    for (int j = 0; j < E; ++j) {
-      const int64_t i = static_cast<int64_t>(j) * kRegThreads + tid;
-      const unsigned long long K = (static_cast<unsigned long long>(u[j]) << 32) | static_cast<uint32_t>(i);
-      if (i < len && K >= lo && K - lo <= span) {
-        const uint32_t b = static_cast<uint32_t>((K - lo) >> s);
-        if (b < bstar) okeys[atomicAdd(&scal[3], 1u)] = K;
-        else if (b == bstar && finish) ebuf[atomicAdd(&scal[4], 1u)] = K;
+      for (int j = 0; j < E; ++j) {
+        const int64_t i = static_cast<int64_t>(j) * kRegThreads + tid;
+        const unsigned long long K = (static_cast<unsigned long long>(u[j]) << 32) | static_cast<uint32_t>(i);
+        if (i < len && K >= lo && K - lo <= span) {
+          const uint32_t b = static_cast<uint32_t>((K - lo) >> s);
+          if (b < bstar) okeys[atomicAdd(&scal[3], 1u)] = K;
+          else if (b == bstar && finish) ebuf[atomicAdd(&scal[4], 1u)] = K;
+        }
       }
-    }
-    need -= below;
-    __syncthreads();
-    if (finish) {
-      // the bucket's `need` smallest keys, by rank counting (keys are unique)
-      const uint32_t base = scal[3];
-      for (uint32_t e = tid; e < inb; e += kRegThreads) {
-        const unsigned long long K = ebuf[e];
-        uint32_t r = 0;
-        for (uint32_t o = 0; o < inb; ++o) r += ebuf[o] < K ? 1u : 0u;
-        if (r < need) okeys[base + r] = K;
+      need -= below;
+      __syncthreads();
+      if (finish) {
+        // the bucket's `need` smallest keys, by rank counting (keys are unique)
+        const uint32_t base = scal[3];
+        for (uint32_t e = tid; e < inb; e += kRegThreads) {
+          const unsigned long long K = ebuf[e];
+          uint32_t r = 0;
+          for (uint32_t o = 0; o < inb; ++o) r += ebuf[o] < K ? 1u : 0u;
+          if (r < need) okeys[base + r] = K;
+        }
+        need = 0;
+      } else {
+        lo += static_cast<unsigned long long>(bstar) << s;  // (s > 0 here: with s == 0 a bucket holds one key)
+        span = (1ull << s) - 1ull;
       }
-      need = 0;
-    } else {
-      lo += static_cast<unsigned long long>(bstar) << s;  // (s > 0 here: with s == 0 a bucket holds one key)
-      span = (1ull << s) - 1ull;
+      __syncthreads();
     }
-    __syncthreads();
-  }
 
-  // ascending (key, position): rank counting among the k winners
-  for (int t = tid; t < k; t += kRegThreads) {
-    if (t < k_eff) {
-      const unsigned long long K = okeys[t];
-      int r = 0;
-      for (int o = 0; o < k_eff; ++o) r += okeys[o] < K ? 1 : 0;
-      const uint32_t pos = static_cast<uint32_t>(K);
-      out_val[row * k + r] = v[pos];
-      if constexpr (HasIdx) out_idx[row * k + r] = static_cast<IdxOut>(in_idx[row * in_ld + pos]);
-      else out_idx[row * k + r] = static_cast<IdxOut>(pos);
-    } else {
-      out_val[row * k + t] = select_min ? FLT_MAX : -FLT_MAX;
-      out_idx[row * k + t] = all_ones<IdxOut>();
+    // ascending (key, position): rank counting among the k winners
+    for (int t = tid; t < k; t += kRegThreads) {
+      if (t < k_eff) {
+        const unsigned long long K = okeys[t];
+        int r = 0;
+        for (int o = 0; o < k_eff; ++o) r += okeys[o] < K ? 1 : 0;
+        const uint32_t pos = static_cast<uint32_t>(K);
+        out_val[row * k + r] = v[pos];
+        if constexpr (HasIdx) out_idx[row * k + r] = static_cast<IdxOut>(in_idx[row * in_ld + pos]);
+        else out_idx[row * k + r] = static_cast<IdxOut>(pos);
+      } else {
+        out_val[row * k + t] = select_min ? FLT_MAX : -FLT_MAX;
+        out_idx[row * k + t] = all_ones<IdxOut>();
+      }
     }
+    __syncthreads();  // the next row rewrites the shared buffers this one read last
   }
 }
 
 template <typename IdxIn, typename IdxOut, bool HasIdx>
 void launch(cudaStream_t stream, const float* in_val, const void* in_idx, int64_t batch, int64_t len, int64_t in_ld,
-            int k, float* out_val, void* out_idx, bool select_min)
+            int k, float* out_val, void* out_idx, bool select_min, const int* live_rows)
 {
   if (len >= 2048 && len <= 64 * kRegThreads && k <= kRegMaxK) {
     count_launch();
-    const unsigned grid = static_cast<unsigned>(batch);
+    // with a device row count the rows are usually few: a grid of at most 1024 CTAs strides over them
+    const unsigned grid = static_cast<unsigned>(live_rows != nullptr ? std::min<int64_t>(batch, 1024) : batch);
     static bool carve = [] {  // two resident CTAs need ~40 KB of shared memory: ask for the carve-out once per instantiation
       cudaFuncSetAttribute(select_k_reg_kernel<8, IdxIn, IdxOut, HasIdx>, cudaFuncAttributePreferredSharedMemoryCarveout, 50);
       cudaFuncSetAttribute(select_k_reg_kernel<16, IdxIn, IdxOut, HasIdx>, cudaFuncAttributePreferredSharedMemoryCarveout, 50);
@@ -404,10 +412,10 @@ void launch(cudaStream_t stream, const float* in_val, const void* in_idx, int64_
     auto oo = static_cast<IdxOut*>(out_idx);
     // sample elements per thread for the kernel's sampled bound: 32 * es ~ 0.7 * len / k samples per warp (0 = no sampling)
     const int es = static_cast<int>(std::min<int64_t>(64, (7 * len) / (320 * static_cast<int64_t>(std::max(k, 1)))));
-    if (len <= 8 * kRegThreads) select_k_reg_kernel<8, IdxIn, IdxOut, HasIdx><<<grid, kRegThreads, 0, stream>>>(in_val, ii, len, in_ld, k, out_val, oo, select_min, es);
-    else if (len <= 16 * kRegThreads) select_k_reg_kernel<16, IdxIn, IdxOut, HasIdx><<<grid, kRegThreads, 0, stream>>>(in_val, ii, len, in_ld, k, out_val, oo, select_min, es);
-    else if (len <= 32 * kRegThreads) select_k_reg_kernel<32, IdxIn, IdxOut, HasIdx><<<grid, kRegThreads, 0, stream>>>(in_val, ii, len, in_ld, k, out_val, oo, select_min, es);
-    else select_k_reg_kernel<64, IdxIn, IdxOut, HasIdx><<<grid, kRegThreads, 0, stream>>>(in_val, ii, len, in_ld, k, out_val, oo, select_min, es);
+    if (len <= 8 * kRegThreads) select_k_reg_kernel<8, IdxIn, IdxOut, HasIdx><<<grid, kRegThreads, 0, stream>>>(in_val, ii, len, in_ld, k, out_val, oo, select_min, es, batch, live_rows);
+    else if (len <= 16 * kRegThreads) select_k_reg_kernel<16, IdxIn, IdxOut, HasIdx><<<grid, kRegThreads, 0, stream>>>(in_val, ii, len, in_ld, k, out_val, oo, select_min, es, batch, live_rows);
+    else if (len <= 32 * kRegThreads) select_k_reg_kernel<32, IdxIn, IdxOut, HasIdx><<<grid, kRegThreads, 0, stream>>>(in_val, ii, len, in_ld, k, out_val, oo, select_min, es, batch, live_rows);
+    else select_k_reg_kernel<64, IdxIn, IdxOut, HasIdx><<<grid, kRegThreads, 0, stream>>>(in_val, ii, len, in_ld, k, out_val, oo, select_min, es, batch, live_rows);
     B2_CUDA(cudaGetLastError());
     return;
   }
@@ -419,7 +427,8 @@ void launch(cudaStream_t stream, const float* in_val, const void* in_idx, int64_
   size_t smem = (256 + 8 + 32) * sizeof(uint32_t) + static_cast<size_t>(kpow2) * sizeof(uint64_t);
   count_launch();
   select_k_kernel<IdxIn, IdxOut, HasIdx><<<static_cast<unsigned>(batch), threads, smem, stream>>>(
-    in_val, static_cast<const IdxIn*>(in_idx), len, in_ld, k, kpow2, out_val, static_cast<IdxOut*>(out_idx), select_min);
+    in_val, static_cast<const IdxIn*>(in_idx), len, in_ld, k, kpow2, out_val, static_cast<IdxOut*>(out_idx), select_min, seg_rows{},
+    live_rows);
   B2_CUDA(cudaGetLastError());
 }
 
@@ -441,20 +450,21 @@ __global__ void merge_gather_kernel(const float* __restrict__ in_keys, const int
 }  // namespace
 
 void select_k(cudaStream_t stream, const float* in_val, const void* in_idx, idx_kind in_kind, int64_t batch,
-              int64_t len, int64_t in_ld, int k, float* out_val, void* out_idx, idx_kind out_kind, bool select_min)
+              int64_t len, int64_t in_ld, int k, float* out_val, void* out_idx, idx_kind out_kind, bool select_min,
+              const int* batch_dev)
 {
   B2_EXPECTS(k >= 1 && k <= kMaxK, "select_k: k must be in [1, %d] (got %d)", kMaxK, k);
   B2_EXPECTS(len >= 0 && len < (int64_t(1) << 32), "select_k: row length out of range");
   B2_EXPECTS(batch < (int64_t(1) << 31), "select_k: batch too large");
   if (batch == 0) return;
   if (in_idx == nullptr) in_kind = IDX_NONE;
-  if (in_kind == IDX_NONE && out_kind == IDX_I64) return launch<int64_t, int64_t, false>(stream, in_val, nullptr, batch, len, in_ld, k, out_val, out_idx, select_min);
-  if (in_kind == IDX_NONE && out_kind == IDX_U32) return launch<uint32_t, uint32_t, false>(stream, in_val, nullptr, batch, len, in_ld, k, out_val, out_idx, select_min);
-  if (in_kind == IDX_NONE && out_kind == IDX_I32) return launch<int32_t, int32_t, false>(stream, in_val, nullptr, batch, len, in_ld, k, out_val, out_idx, select_min);
-  if (in_kind == IDX_I64 && out_kind == IDX_I64) return launch<int64_t, int64_t, true>(stream, in_val, in_idx, batch, len, in_ld, k, out_val, out_idx, select_min);
-  if (in_kind == IDX_U32 && out_kind == IDX_U32) return launch<uint32_t, uint32_t, true>(stream, in_val, in_idx, batch, len, in_ld, k, out_val, out_idx, select_min);
-  if (in_kind == IDX_U32 && out_kind == IDX_I64) return launch<uint32_t, int64_t, true>(stream, in_val, in_idx, batch, len, in_ld, k, out_val, out_idx, select_min);
-  if (in_kind == IDX_I32 && out_kind == IDX_I32) return launch<int32_t, int32_t, true>(stream, in_val, in_idx, batch, len, in_ld, k, out_val, out_idx, select_min);
+  if (in_kind == IDX_NONE && out_kind == IDX_I64) return launch<int64_t, int64_t, false>(stream, in_val, nullptr, batch, len, in_ld, k, out_val, out_idx, select_min, batch_dev);
+  if (in_kind == IDX_NONE && out_kind == IDX_U32) return launch<uint32_t, uint32_t, false>(stream, in_val, nullptr, batch, len, in_ld, k, out_val, out_idx, select_min, batch_dev);
+  if (in_kind == IDX_NONE && out_kind == IDX_I32) return launch<int32_t, int32_t, false>(stream, in_val, nullptr, batch, len, in_ld, k, out_val, out_idx, select_min, batch_dev);
+  if (in_kind == IDX_I64 && out_kind == IDX_I64) return launch<int64_t, int64_t, true>(stream, in_val, in_idx, batch, len, in_ld, k, out_val, out_idx, select_min, batch_dev);
+  if (in_kind == IDX_U32 && out_kind == IDX_U32) return launch<uint32_t, uint32_t, true>(stream, in_val, in_idx, batch, len, in_ld, k, out_val, out_idx, select_min, batch_dev);
+  if (in_kind == IDX_U32 && out_kind == IDX_I64) return launch<uint32_t, int64_t, true>(stream, in_val, in_idx, batch, len, in_ld, k, out_val, out_idx, select_min, batch_dev);
+  if (in_kind == IDX_I32 && out_kind == IDX_I32) return launch<int32_t, int32_t, true>(stream, in_val, in_idx, batch, len, in_ld, k, out_val, out_idx, select_min, batch_dev);
   B2_FAIL("select_k: unsupported index dtype combination (%d -> %d)", int(in_kind), int(out_kind));
 }
 
@@ -483,7 +493,7 @@ void select_k_segments(cudaStream_t stream, const float* in_val, const int64_t* 
   B2_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
   count_launch();
   timed_section ts("select_k_segments", stream);
-  kern<<<static_cast<unsigned>(batch), threads, smem, stream>>>(in_val, nullptr, 0, 0, k, kpow2, out_val, out_pos, select_min, seg);
+  kern<<<static_cast<unsigned>(batch), threads, smem, stream>>>(in_val, nullptr, 0, 0, k, kpow2, out_val, out_pos, select_min, seg, nullptr);
   B2_CUDA(cudaGetLastError());
 }
 

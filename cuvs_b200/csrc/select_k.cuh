@@ -17,9 +17,11 @@ enum idx_kind : int { IDX_NONE = 0, IDX_I64 = 1, IDX_U32 = 2, IDX_I32 = 3 };
  * supplies the payload, otherwise the payload is the column position.  Missing entries
  * (len < k) are padded with +/-FLT_MAX and the all-ones index.
  * `in_ld` is the row pitch of in_val/in_idx in elements (>= len).
+ * `batch_dev` (device, may be null): the rows to select are the first *batch_dev <= batch; `batch` sizes the launch.
  */
 void select_k(cudaStream_t stream, const float* in_val, const void* in_idx, idx_kind in_kind, int64_t batch,
-              int64_t len, int64_t in_ld, int k, float* out_val, void* out_idx, idx_kind out_kind, bool select_min);
+              int64_t len, int64_t in_ld, int k, float* out_val, void* out_idx, idx_kind out_kind, bool select_min,
+              const int* batch_dev = nullptr);
 
 /** Largest k of select_k and select_k_segments. */
 constexpr int kSelectMaxK = 2048;
